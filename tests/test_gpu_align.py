@@ -89,8 +89,18 @@ def _pose_err(Ta, Tb):
     return float(np.linalg.norm(se3.se3_log(se3.mul(se3.inv(Ta), Tb))))
 
 
-@pytest.mark.parametrize("levels,max_level", [(3, 2), (8, 3)])
-def test_sparse_align_pose_tolerance(levels, max_level, ctx3, ctx8, oracle):
+def _select_generation(monkeypatch, gen):
+    """ygzb_sparse_align runs the second-generation kernel (the tracker's) unless YGZB_SPARSE_GEN1 is set."""
+    if gen == 1:
+        monkeypatch.setenv("YGZB_SPARSE_GEN1", "1")
+    else:
+        monkeypatch.delenv("YGZB_SPARSE_GEN1", raising=False)
+
+
+@pytest.mark.parametrize("levels,max_level,gen", [(3, 2, 2), (8, 3, 2), (3, 2, 1), (8, 3, 1)],
+                         ids=["3-2", "8-3", "3-2-gen1", "8-3-gen1"])
+def test_sparse_align_pose_tolerance(levels, max_level, gen, ctx3, ctx8, oracle, monkeypatch):
+    _select_generation(monkeypatch, gen)
     ctx = ctx3 if levels == 3 else ctx8
     s = _scene(oracle, levels=levels)
     s2 = _scene(oracle, 2, 5, levels=levels)
@@ -146,9 +156,20 @@ def test_align1d_bit_exact(ctx3, oracle):
     fr.close()
 
 
-def test_alignment_and_klt_on_another_geometry(oracle):
+def test_alignment_and_klt_on_another_geometry(oracle, monkeypatch):
     """752 x 480, 4 levels (not the 640 x 480 default): FindDirectProjection bit-exact, SparseImgAlign and KLT within
     their tolerances -- the level geometry (pitches, offsets, borders) is a run-time parameter everywhere."""
+    _select_generation(monkeypatch, 2)
+    _another_geometry(oracle)
+
+
+def test_sparse_align_first_generation_on_another_geometry(oracle, monkeypatch):
+    """The same 752 x 480, 4-level checks with YGZB_SPARSE_GEN1: the first-generation sparse-alignment kernel."""
+    _select_generation(monkeypatch, 1)
+    _another_geometry(oracle)
+
+
+def _another_geometry(oracle):
     from ygz_slam_b200 import Context
     w, h, levels = 752, 480, 4
     tex = synth.texture(0x59475A00, 2048)
@@ -192,3 +213,41 @@ def test_alignment_and_klt_on_another_geometry(oracle):
         fr.close()
     finally:
         ctx.close()
+
+
+@pytest.mark.parametrize("gen", [2, 1])
+def test_sparse_align_global_staging_batch(ctx3, oracle, gen, monkeypatch):
+    """One batch of 6,000 features, none, and 800 features (random pixels of the rendered frames with their rendered depth,
+    map-point masks with holes).  The second-generation kernel runs 4 CTAs per problem and stages a CTA's features in shared
+    memory up to (227 KB - 8 KB of static arrays) / 360 B per record = 622 features: the 6,000-feature problem (1,500 per
+    CTA) stages in the global scratch, the 800-feature one (200 per CTA) in shared memory, and the empty one returns at once.
+    Every pose within 1e-4 of the oracle, identical measurement counts, iterations reported per level, and two calls are
+    bit-identical (each CTA sums its features in order, the cluster adds the CTA partials in rank order)."""
+    _select_generation(monkeypatch, gen)
+    g1, d1, T1 = synth.stream_frame(1)
+    g2, _, _ = synth.stream_frame(4)
+    g3, d3, T3 = synth.stream_frame(2)
+    g4, _, _ = synth.stream_frame(5)
+    fr = ctx3.frames(4)
+    fr.upload(np.stack([g1, g2, g3, g4]))
+    pxa, da = synth.pixel_features(d1, 6000, seed=61)
+    pxb, db = synth.pixel_features(d3, 800, seed=62)
+    assert -(-6000 // 4) > 622 >= -(-800 // 4)
+    ha = np.ones(6000, np.uint8)
+    ha[::7] = 0
+    hb = np.ones(800, np.uint8)
+    hb[3::5] = 0
+    T_ref = np.stack([T1.reshape(-1), T1.reshape(-1), T3.reshape(-1)])
+    args = ([0, 0, 2], [1, 1, 3], [0, 6000, 6000, 6800], np.concatenate([pxa, pxb]), np.concatenate([da, db]), np.concatenate([ha, hb]),
+            T_ref, T_ref)
+    T, n_meas, iters = fr.sparse_align(*args)
+    p1, p2, p3, p4 = (oracle.build_pyramid(g, 3) for g in (g1, g2, g3, g4))
+    for p, (rp, cp, px, d, h, Tr) in ((0, (p1, p2, pxa, da, ha, T1)), (2, (p3, p4, pxb, db, hb, T3))):
+        wT, wn, _ = oracle.sparse_align(rp, cp, 640, 480, 3, px, d, h, Tr, Tr)
+        assert _pose_err(T[p], wT) < 1e-4, p
+        assert n_meas[p] == wn, p
+        assert (iters[p, :3] <= 30).all() and iters[p, 2] >= 1 and not iters[p, 3:].any(), p   # levels 2..0 ran, coarsest first
+    assert n_meas[1] == 0 and np.array_equal(T[1].reshape(-1), T_ref[1]) and not iters[1].any()
+    T2, n_meas2, iters2 = fr.sparse_align(*args)
+    assert np.array_equal(T, T2) and np.array_equal(n_meas, n_meas2) and np.array_equal(iters, iters2)
+    fr.close()

@@ -113,8 +113,21 @@ def _t_aa(v):  # se3 log [upsilon; omega] -> [t; angle-axis] (the pose block of 
     return np.array(out)
 
 
-def test_local_ba_ceres_twin_matches_oracle(ctx3, oracle):
+def test_local_ba_ceres_twin_matches_oracle(ctx3, oracle, monkeypatch):
     """ba::LocalBA (BA.cpp:324-384): two problems in one launch, the second with a different size."""
+    monkeypatch.delenv("YGZB_BA_CLUSTER", raising=False)
+    _ceres_twin(ctx3, oracle)
+
+
+@pytest.mark.parametrize("cluster", [1, 16])
+def test_local_ba_ceres_twin_cluster_sizes(ctx3, oracle, cluster, monkeypatch):
+    """The same two problems at 1 and 16 CTAs per problem instead of the default 8: the kernel strides every loop over the
+    cluster."""
+    monkeypatch.setenv("YGZB_BA_CLUSTER", str(cluster))
+    _ceres_twin(ctx3, oracle)
+
+
+def _ceres_twin(ctx3, oracle):
     a = synth.ba_scene()
     b = synth.ba_scene(n_kf=6, n_pt=300, target_obs=1500, seed=12)
     fa = np.zeros(10, np.uint8); fa[0] = 1
@@ -187,3 +200,213 @@ def test_two_view_ba_matches_oracle(ctx3, oracle):
         assert np.array_equal(inl[sl], winl)
         assert st[p]["iters"] == wst["iters"] and st[p]["termination"] == wst["termination"]
         assert abs(st[p]["cost_final"] - wst["cost_final"]) < 1e-9 * max(wst["cost_final"], 1e-12) + 1e-15
+
+
+# ---- staging paths and cluster sizes of local_ba2_kernel (ba2.cu) ---------------------------------------------------------
+# Host arithmetic of launch_local_ba2 and the kernel's staging decision, restated: a CTA keeps its landmarks' state in shared
+# memory when ba2_stage_doubles(nl, no) fits what the launch left after the reduced system, and takes the block-pair entry
+# list only when that fits as well; otherwise it stages in global memory and accumulates by 32-landmark chunks.  The budget
+# is the sm_90 opt-in of 227 KB less the kernel's 24 KB of static arrays.
+_OPTIN_DOUBLES = (227 - 24) * 1024 // 8
+
+
+def _stage_doubles(nl, no):
+    return 14 * no + 30 * nl + ((nl + 1) * 4 + ((no + 7) & ~7) + nl * 16 + 7) // 8 + 1
+
+
+def _entry_doubles(nl, no, np_):
+    return (min((no * (np_ + 1) + 1) // 2, nl * (np_ * (np_ + 1) // 2)) + 1) // 2
+
+
+def _auto_cluster(max_pts, max_free):
+    c = 1
+    while c < 8 and max_pts > c * 320:
+        c *= 2
+    tasks = max_free * (max_free + 1) // 2 + max_free
+    while c < 16 and tasks * (((max_pts + c - 1) // c + 31) // 32) // 8 > 24:
+        c *= 2
+    return c
+
+
+def _ba2_staging(problems, cluster=None):
+    """problems: list of (fixed, pt_idx, n_pt) of one batch.  Returns the cluster size and, per problem, one flag per CTA:
+    True = its staging area is in shared memory (with the entry list), False = global staging + chunked accumulate."""
+    max_pts = max(n for _, _, n in problems)
+    max_free = max(int((f == 0).sum()) for f, _, _ in problems)
+    max_kf = max(len(f) for f, _, _ in problems)
+    max_obs = max(len(pt) for _, pt, _ in problems)
+    c = cluster or _auto_cluster(max_pts, max_free)
+    np_ = max_free
+    n_pairs = np_ * (np_ + 1) // 2
+    V = 42 * n_pairs + 27 * np_
+    sys_ = max(36 * np_ * np_ + 6 * np_, (n_pairs + np_ + 8) * 42)
+    nl_b = (max_pts + c - 1) // c
+    no_b = min(max_obs, nl_b * max_kf)
+    dyn = min(_OPTIN_DOUBLES, sys_ + 2 * V + _stage_doubles(nl_b, no_b) + 2 + _entry_doubles(nl_b, no_b, np_))
+    have = dyn - (sys_ + 2 * V)
+    out = []
+    for f, pt, n_pt in problems:
+        per = (n_pt + c - 1) // c
+        starts = np.r_[0, np.cumsum(np.bincount(pt, minlength=n_pt))]
+        flags = []
+        for r in range(c):
+            lo = min(n_pt, r * per)
+            hi = min(n_pt, lo + per)
+            nl, no = hi - lo, int(starts[hi] - starts[lo])
+            flags.append(_stage_doubles(nl, no) + _entry_doubles(nl, no, int((f == 0).sum())) <= have)
+        out.append(flags)
+    return c, out
+
+
+def _check_g2o(oracle, res, sc, fixed):
+    """res = (poses, points, outlier flags, stats) of one problem against the oracle, with the tolerances of C4."""
+    P, X, out, st = res
+    wP, wX, wout, wst = oracle.local_ba(_g2o(sc["poses_noisy"]), fixed, sc["pts_noisy"], sc["kf_idx"], sc["pt_idx"], sc["px"])
+    assert _pose_diff(P, wP) < 1e-4
+    assert np.abs(X - wX).max() < 1e-4
+    assert abs(st["chi2_final"] - wst["chi2_final"]) <= 1e-6 * wst["chi2_final"]
+    assert (out != wout).sum() <= 2
+
+
+def _one(ctx, sc, fixed):
+    n_kf, n_pt, n_obs = len(fixed), len(sc["pts_noisy"]), len(sc["kf_idx"])
+    P, X, out, st = ctx.local_ba([0, n_kf], [0, n_pt], [0, n_obs], _g2o(sc["poses_noisy"]), fixed, sc["pts_noisy"], sc["kf_idx"],
+                                 sc["pt_idx"], sc["px"])
+    return P, X, out, st[0]
+
+
+def _batch(ctx, scs, fixeds):
+    kf_off = np.cumsum([0] + [len(f) for f in fixeds])
+    pt_off = np.cumsum([0] + [len(s["pts_noisy"]) for s in scs])
+    obs_off = np.cumsum([0] + [len(s["kf_idx"]) for s in scs])
+    P, X, out, st = ctx.local_ba(kf_off, pt_off, obs_off, np.concatenate([_g2o(s["poses_noisy"]) for s in scs]), np.concatenate(fixeds),
+                                 np.concatenate([s["pts_noisy"] for s in scs]), np.concatenate([s["kf_idx"] for s in scs]),
+                                 np.concatenate([s["pt_idx"] for s in scs]), np.concatenate([s["px"] for s in scs]))
+    return [(P[kf_off[i]:kf_off[i + 1]], X[pt_off[i]:pt_off[i + 1]], out[obs_off[i]:obs_off[i + 1]], st[i]) for i in range(len(scs))]
+
+
+def _fixed(n_kf, *idx):
+    f = np.zeros(n_kf, np.uint8)
+    f[list(idx) or [0]] = 1
+    return f
+
+
+@pytest.mark.parametrize("cluster", [1, 2, 4, 8, 16])
+def test_local_ba_c4_every_cluster_size(ctx3, oracle, cluster, monkeypatch):
+    """C4 at every cluster size.  C4's reduced system (9 free poses) leaves 18,748 doubles of staging per CTA; a CTA of
+    2000 / cluster landmarks and ~4 x as many observations needs 178,002 / 89,002 / 44,502 / 22,252 / 11,127 of them at
+    cluster 1 / 2 / 4 / 8 / 16: clusters 1-8 stage globally and accumulate by chunks, 16 stages in shared memory.  Two
+    runs of one configuration are bit-identical (fixed partition, rank-ordered sums)."""
+    sc = synth.ba_scene()
+    fixed = _fixed(10)
+    _, flags = _ba2_staging([(fixed, sc["pt_idx"], 2000)], cluster)
+    assert flags[0] == [cluster == 16] * cluster
+    monkeypatch.setenv("YGZB_BA_CLUSTER", str(cluster))
+    r1 = _one(ctx3, sc, fixed)
+    r2 = _one(ctx3, sc, fixed)
+    _check_g2o(oracle, r1, sc, fixed)
+    for a, b in zip(r1[:3], r2[:3]):
+        assert np.array_equal(a, b)
+    assert r1[3] == r2[3]
+
+
+def test_local_ba_global_staging_alone_and_batched(ctx3, oracle):
+    """10 key-frames x 5,000 landmarks x 20,000 observations at the automatic cluster (16): a CTA holds 313 landmarks and
+    ~1,250 observations, ~27,000 staging doubles against 18,748 available, so every CTA stages globally and the CTAs'
+    regions of the global scratch must be disjoint.  Alone, then batched with a 300-landmark problem and the tracker's
+    3-key-frame shape (1,200 landmarks), where the large problem still stages globally and the small ones in shared memory."""
+    big = synth.ba_scene(n_kf=10, n_pt=5000, target_obs=20000, seed=31)
+    small = synth.ba_scene(n_kf=6, n_pt=300, target_obs=1500, seed=12)
+    kf3 = synth.ba_scene(n_kf=3, n_pt=1200, target_obs=3600, seed=33)
+    fb, fs, f3 = _fixed(10), _fixed(6), _fixed(3)
+    c, flags = _ba2_staging([(fb, big["pt_idx"], 5000)])
+    assert c == 16 and not any(flags[0])
+    _check_g2o(oracle, _one(ctx3, big, fb), big, fb)
+    c, flags = _ba2_staging([(fb, big["pt_idx"], 5000), (fs, small["pt_idx"], 300), (f3, kf3["pt_idx"], 1200)])
+    assert c == 16 and not any(flags[0]) and all(flags[1]) and all(flags[2])
+    for r, sc, f in zip(_batch(ctx3, [big, small, kf3], [fb, fs, f3]), (big, small, kf3), (fb, fs, f3)):
+        _check_g2o(oracle, r, sc, f)
+
+
+@pytest.mark.parametrize("solver", ["0", "1"])
+def test_local_ba_sixteen_free_poses(ctx3, oracle, solver, monkeypatch):
+    """kBA2MaxFree = 16 (17 key-frames, one fixed): a 96 x 96 reduced system leaves 4,384 staging doubles per CTA.  At 150
+    landmarks (8 CTAs of <= 19 landmarks, <= 2,766 doubles) every CTA stages in shared memory; at 2,000 landmarks (16 CTAs of
+    125 landmarks, ~11,000 doubles) every CTA stages globally.  Both with the blocked (0) and the scalar (1) factorisation."""
+    monkeypatch.setenv("YGZB_BA_SOLVER", solver)
+    f = _fixed(17)
+    for n_pt, per_pt, shared in ((150, 8, True), (2000, 4, False)):
+        sc = synth.ba_scene(n_kf=17, n_pt=n_pt, target_obs=per_pt * n_pt, seed=40)
+        _, flags = _ba2_staging([(f, sc["pt_idx"], n_pt)])
+        assert all(fl == shared for fl in flags[0]), n_pt
+        _check_g2o(oracle, _one(ctx3, sc, f), sc, f)
+
+
+def test_local_ba_rejects_invalid_problems(ctx3, oracle):
+    """17 free poses, 65 poses, an out-of-range index and a point observed twice by one free key-frame return
+    YGZB_ERR_INVALID (-1) with the library's message (both in the YgzbError); a valid call afterwards still matches."""
+    from ygz_slam_b200.capi import YgzbError
+    sc = synth.ba_scene(n_kf=10, n_pt=300, target_obs=1200, seed=50)
+    f = _fixed(10)
+    n_obs = len(sc["kf_idx"])
+    with pytest.raises(YgzbError, match=r"rc=-1\).*17 free poses"):
+        ctx3.local_ba([0, 18], [0, 300], [0, n_obs], np.zeros((18, 6)), _fixed(18), sc["pts_noisy"], sc["kf_idx"], sc["pt_idx"], sc["px"])
+    with pytest.raises(YgzbError, match=r"rc=-1\).*65 poses"):
+        ctx3.local_ba([0, 65], [0, 300], [0, n_obs], np.zeros((65, 6)), np.ones(65, np.uint8), sc["pts_noisy"], sc["kf_idx"], sc["pt_idx"],
+                      sc["px"])
+    bad = sc["kf_idx"].copy()
+    bad[7] = 10
+    with pytest.raises(YgzbError, match=r"rc=-1\).*index out of range"):
+        ctx3.local_ba([0, 10], [0, 300], [0, n_obs], _g2o(sc["poses_noisy"]), f, sc["pts_noisy"], bad, sc["pt_idx"], sc["px"])
+    # a second observation of landmark 0 by a free key-frame that already sees it (the kernel's duplicate check)
+    q = int(np.flatnonzero((sc["pt_idx"] == 0) & (sc["kf_idx"] > 0))[0])
+    kf_idx, pt_idx, px = (np.insert(sc["kf_idx"], q, sc["kf_idx"][q]), np.insert(sc["pt_idx"], q, 0), np.insert(sc["px"], q, sc["px"][q], 0))
+    with pytest.raises(YgzbError, match=r"rc=-1\).*observed twice"):
+        ctx3.local_ba([0, 10], [0, 300], [0, n_obs + 1], _g2o(sc["poses_noisy"]), f, sc["pts_noisy"], kf_idx, pt_idx, px)
+    _check_g2o(oracle, _one(ctx3, sc, f), sc, f)
+
+
+def test_local_ba_structural_edge_cases(ctx3, oracle, monkeypatch):
+    """One batch at YGZB_BA_CLUSTER=16: landmarks seen only by the fixed key-frames, landmarks with a single observation (on
+    a free and on a fixed key-frame), a problem without observations, and a 10-landmark problem, so that 6 of its 16 CTAs own
+    no landmark.  A single-observation landmark is free along its ray (its 3 x 3 block has rank 2 and only the damping fixes
+    the step), so for those the check is finiteness; poses, the other landmarks, chi2 and outlier flags match the oracle."""
+    edge = synth.ba_edge_scene()
+    fe = _fixed(6, 0, 1)
+    empty = synth.ba_scene(n_kf=3, n_pt=20, seed=42)
+    empty.update(kf_idx=np.zeros(0, np.int32), pt_idx=np.zeros(0, np.int32), px=np.zeros((0, 2)))
+    f3 = _fixed(3)
+    tiny = synth.ba_scene(n_kf=4, n_pt=10, target_obs=40, seed=43)
+    f4 = _fixed(4)
+    assert len(np.unique(tiny["pt_idx"])) == 10 and len(edge["pts_noisy"]) == 380
+    monkeypatch.setenv("YGZB_BA_CLUSTER", "16")
+    res = _batch(ctx3, [edge, empty, tiny], [fe, f3, f4])
+    P, X, out, st = res[0]
+    wP, wX, wout, wst = oracle.local_ba(_g2o(edge["poses_noisy"]), fe, edge["pts_noisy"], edge["kf_idx"], edge["pt_idx"], edge["px"])
+    well = np.setdiff1d(np.arange(380), edge["single"])
+    assert _pose_diff(P, wP) < 1e-4
+    assert np.abs(X[well] - wX[well]).max() < 1e-4 and np.isfinite(X).all()
+    assert abs(st["chi2_final"] - wst["chi2_final"]) <= 1e-6 * wst["chi2_final"]
+    assert (out != wout).sum() <= 2
+    assert np.array_equal(P[:2], _g2o(edge["poses_noisy"])[:2])
+    # no observations: nothing moves (a free pose makes a round trip through SE3 and back to its log, hence not bit-equal)
+    P0, X0, _, st0 = res[1]
+    assert _pose_diff(P0, _g2o(empty["poses_noisy"])) < 1e-12 and np.allclose(X0, empty["pts_noisy"], rtol=0, atol=1e-12)
+    assert st0["chi2_final"] == 0
+    _check_g2o(oracle, res[2], tiny, f4)
+
+
+def test_pose_only_large_frames(ctx3, oracle):
+    """ygzb_pose_only runs 8 CTAs of 256 threads per frame and stages k points per thread when k <= min(32, (227 - 8) KB /
+    (5 x 256 x 8 B)) = 21, i.e. up to 21 x 2048 = 43,008 points.  40,000 points (k = 20) are staged; 45,000 (k = 22) are
+    read from global memory (stage_k = 0).  Each frame alone (the stage decision is per call), with 10 % gross outliers."""
+    for n in (40000, 45000):
+        sc = synth.pose_only_scene(n, seed=n)
+        px = sc["px"].copy()
+        px[::10] += 30
+        T, inl, depth, cnt = ctx3.pose_only([0, n], sc["pw"], px, sc["T0"].reshape(1, 12))
+        wT, winl, wdepth, wcnt = oracle.pose_only(sc["pw"], px, sc["T0"])
+        assert np.linalg.norm(se3.se3_log(se3.mul(se3.inv(T[0]), wT))) < 1e-4, n
+        assert cnt[0] == wcnt, n
+        assert np.array_equal(inl, winl), n
+        assert np.allclose(depth, wdepth, atol=1e-6), n

@@ -88,3 +88,17 @@ def test_sparse_align_recovers_relative_pose(oracle):
     # a feature without map point is skipped; no features -> pose untouched, 0 measurements
     T0, nm0, _ = oracle.sparse_align(s["p1"], s["p2"], 640, 480, 3, s["px"], s["depth"], np.zeros(n, np.uint8), s["T1"], s["T1"])
     assert nm0 == 0
+
+
+def test_sparse_align_dense_pixel_features(oracle):
+    """The GPU suite's large sparse-alignment problem: 6,000 random pixels of the rendered frame with their rendered depth
+    (not detections), every seventh without a map point.  The oracle recovers the relative pose from them."""
+    g1, d1, T1 = synth.stream_frame(1)
+    g2, _, T2 = synth.stream_frame(4)
+    p1, p2 = oracle.build_pyramid(g1, 3), oracle.build_pyramid(g2, 3)
+    px, depth = synth.pixel_features(d1, 6000, seed=61)
+    has = np.ones(6000, np.uint8)
+    has[::7] = 0
+    T, n_meas, iters = oracle.sparse_align(p1, p2, 640, 480, 3, px, depth, has, T1, T1)
+    assert np.linalg.norm(se3.se3_log(se3.mul(T, se3.inv(T2)))) < 2e-3
+    assert 0.8 * has.sum() < n_meas <= has.sum() and (iters[:3] > 0).all()

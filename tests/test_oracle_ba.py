@@ -119,3 +119,51 @@ def test_two_view_ba(oracle):
     assert np.abs(dirn(T[:, 3]) - dirn(sc["T_cur"][:, 3])).max() < 0.05         # translation direction (scale is gauge)
     assert cnt == inl.sum() and cnt >= len(inl) - 2
     assert inl[sc["inlier"] == 0].sum() >= (sc["inlier"] == 0).sum() - 2        # the restarted points were recovered
+
+
+def test_local_ba_large_and_sixteen_free_scenes(oracle):
+    """The scenes of the GPU suite's staging tests: 10 key-frames x 5,000 landmarks x 20,000 observations, and 17 key-frames
+    (16 free) at 150 and 2,000 landmarks.  The oracle must reach the synthetic truth on each, so that the GPU tests compare
+    against a validated specification."""
+    for n_kf, n_pt, per_pt in ((10, 5000, 4), (17, 150, 8), (17, 2000, 4)):
+        sc = synth.ba_scene(n_kf=n_kf, n_pt=n_pt, target_obs=per_pt * n_pt, seed=31 if n_kf == 10 else 40)
+        fixed = np.zeros(n_kf, np.uint8)
+        fixed[0] = 1
+        P, X, outl, st = oracle.local_ba(_g2o(sc["poses_noisy"]), fixed, sc["pts_noisy"], sc["kf_idx"], sc["pt_idx"], sc["px"])
+        assert st["chi2_final"] < 2e-3 * st["chi2_initial"], (n_kf, n_pt)
+        est = np.concatenate([P[:, 3:], P[:, :3]], 1)
+        assert np.abs(est - sc["poses_true"]).max() < 0.01, (n_kf, n_pt)
+        assert np.median(np.abs(X - sc["pts_true"])) < 0.05, (n_kf, n_pt)
+        assert outl.mean() < 0.05             # ~ the share of 1 px Gaussian residuals above chi2 = 5.991
+
+
+def test_local_ba_structural_edge_cases(oracle):
+    """Landmarks seen only by fixed key-frames, landmarks with one observation, a problem without observations: the oracle
+    returns finite results, the constrained part converges to the truth, and an unobserved problem is left as it was."""
+    sc = synth.ba_edge_scene()
+    fixed = np.zeros(6, np.uint8)
+    fixed[:2] = 1
+    P, X, outl, st = oracle.local_ba(_g2o(sc["poses_noisy"]), fixed, sc["pts_noisy"], sc["kf_idx"], sc["pt_idx"], sc["px"])
+    assert np.isfinite(P).all() and np.isfinite(X).all() and np.isfinite(st["chi2_final"])
+    est = np.concatenate([P[:, 3:], P[:, :3]], 1)
+    assert np.abs(est - sc["poses_true"]).max() < 0.01
+    assert np.median(np.abs(X[:340] - sc["pts_true"][:340])) < 0.05    # every landmark with two or more observations
+    e = synth.ba_scene(n_kf=3, n_pt=20, seed=42)
+    f3 = np.array([1, 0, 0], np.uint8)
+    none = np.zeros(0, np.int32)
+    P0, X0, _, st0 = oracle.local_ba(_g2o(e["poses_noisy"]), f3, e["pts_noisy"], none, none, np.zeros((0, 2)))
+    assert np.array_equal(P0, _g2o(e["poses_noisy"])) and np.array_equal(X0, e["pts_noisy"]) and st0["chi2_final"] == 0
+
+
+def test_pose_only_large_frames(oracle):
+    """Frames of 40,000 and 45,000 points (the GPU suite's staged and unstaged pose-only paths) with every tenth point
+    moved 30 px: the oracle rejects those and comes back to the true pose."""
+    for n in (40000, 45000):
+        sc = synth.pose_only_scene(n, seed=n)
+        px = sc["px"].copy()
+        px[::10] += 30
+        T, inl, depth, cnt = oracle.pose_only(sc["pw"], px, sc["T0"])
+        # (as in test_pose_only_rejects_outliers, the outlier-biased pose of round 0 costs later rounds many good points)
+        assert not inl[::10].any() and cnt == inl.sum() and 0.3 * n < cnt < 0.95 * n
+        assert np.linalg.norm(se3.se3_log(se3.mul(T, se3.inv(sc["T_true"])))) < 2e-3
+        assert np.all(depth[inl] > 0)

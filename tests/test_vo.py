@@ -88,3 +88,30 @@ def _check_native(name, traj, stats, sec, V, data, n_streams, n_frames):
             assert np.linalg.norm(se3.se3_log(se3.mul(traj[s, k], se3.inv(st.trajectory[k])))) < 1e-4, (name, s, k)
         # and both follow the exact ground truth of the sliding-crop stream
         assert np.linalg.norm(se3.se3_log(se3.mul(traj[s, -1], se3.inv(data[s][2][-1])))) < 3e-3
+
+
+@pytest.mark.gpu
+def test_native_driver_track_cluster_sizes(ctx3, monkeypatch):
+    """The device-resident engine at YGZB_TRACK_CLUSTER = 1, 2 and 8 (the default is 4) against the Python loop, with the
+    assertions of test_native_driver_matches_python_loop on 2 streams.  The variable is read by ygzb_tracker_create, which
+    vo_native.run calls for every run; it sets the CTAs per problem of sparse alignment and pose-only.  At cluster 1 a
+    key-frame's ~1,200 features exceed the 622 that fit one CTA's shared memory: the sparse alignment stages them globally.
+    A changed partition changes the summation order, so each run must differ in the last bits from the default run: that
+    shows the variable took effect."""
+    from ygz_slam_b200 import vo_native
+    n_streams, n_frames = 2, 26
+    data = [synth.shift_stream(s, n_frames) for s in range(n_streams)]
+    be = vo.GpuBackend(ctx3, n_streams * vo.VisualOdometry.SLOTS_PER_STREAM)
+    V = vo.VisualOdometry(be, n_streams, kf_min_frames=5, kf_min_rot=0.03, kf_min_trans=0.03)
+    for k in range(n_frames):
+        V.add_frames([data[s][0][k] for s in range(n_streams)], [data[s][1] for s in range(n_streams)], k)
+    be.fr.close()
+    run = lambda: vo_native.run(ctx3, [d[0] for d in data], [d[1] for d in data], 5, 0.03, 0.03, window=1)
+    monkeypatch.delenv("YGZB_TRACK_CLUSTER", raising=False)
+    default = run()
+    _check_native("cluster 4", *default, V, data, n_streams, n_frames)
+    for cluster in (1, 2, 8):
+        monkeypatch.setenv("YGZB_TRACK_CLUSTER", str(cluster))
+        traj, stats, sec = run()
+        _check_native(f"cluster {cluster}", traj, stats, sec, V, data, n_streams, n_frames)
+        assert not np.array_equal(traj, default[0]), cluster

@@ -366,7 +366,7 @@ int ygzb_tracker_create(ygzb_frames* f, int n_streams, int max_jobs, const doubl
     t->f = f;
     t->ctx = ctx;
     t->max_jobs = max_jobs;
-    t->cluster = 4;
+    t->cluster = kTrackCluster;
     if (const char* e = getenv("YGZB_TRACK_CLUSTER")) {   // tuning knob: 1, 2, 4 or 8
         const int v = atoi(e);
         if (v == 1 || v == 2 || v == 4 || v == 8) t->cluster = v;

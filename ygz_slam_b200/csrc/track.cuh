@@ -68,6 +68,5 @@ int launch_pose_only_dev(ygzb_ctx* ctx, int n_problems, const int32_t* d_offsets
                          const double* d_px, double* d_T_cw, uint8_t* d_inlier, double* d_depth, int32_t* d_n_inlier, uint8_t* d_enable,
                          double* d_ws, int cluster, int max_points);
 size_t pose_only_ws_doubles(int n_problems);
-size_t sparse_align2_scratch_bytes(int n_problems, int cells);
 
 }  // namespace ygzb

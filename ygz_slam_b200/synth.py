@@ -185,6 +185,53 @@ def two_view_scene(seed=21, n=120, n_bad=12):
     return dict(T_ref=T_ref, T_cur=T_cur, T_cur0=T_cur0, X=X, X0=X + rng.normal(0, 0.05, X.shape), px_ref=px_ref, px_cur=px_cur, inlier=inlier)
 
 
+def pixel_features(depth: np.ndarray, n: int, seed: int, margin: int = 8):
+    """n random sub-pixel positions inside a rendered frame and their rendered depth: sparse-alignment features of any
+    count (a detector caps the count by the grid)."""
+    rng = np.random.default_rng(seed)
+    h, w = depth.shape
+    px = np.stack([rng.uniform(margin, w - margin, n), rng.uniform(margin, h - margin, n)], 1)
+    return px, depth[px[:, 1].astype(int), px[:, 0].astype(int)].astype(np.float64)
+
+
+def pose_only_scene(n_pts: int, seed: int = 5, pose_sigma: float = 0.002, pixel_sigma: float = 1.0):
+    """One frame for the pose-only refinement: n_pts world points on the planes z = 2 and 4 in front of the camera,
+    their noisy projections, the true pose T_cw and a start pose perturbed by pose_sigma in se3."""
+    from .se3 import se3_exp, se3_log
+    rng = np.random.default_rng(seed)
+    T = trajectory(30)
+    z = np.where(rng.random(n_pts) < 0.75, 2.0, 4.0)
+    u, v = rng.uniform(20, W - 20, n_pts), rng.uniform(20, H - 20, n_pts)
+    pc = np.stack([(u - CX) / FX * z, (v - CY) / FY * z, z], 1)
+    pw = (pc - T[:, 3]) @ T[:, :3]                        # camera -> world: R^T (x - t)
+    px = np.stack([u, v], 1) + rng.normal(0, pixel_sigma, (n_pts, 2))
+    T0 = se3_exp(se3_log(T) + rng.normal(0, pose_sigma, 6))
+    return dict(pw=pw, px=px, T_true=T, T0=T0)
+
+
+def ba_edge_scene(seed: int = 41):
+    """Local-BA problem with the structural corner cases of a sliding window: 6 key-frames (0 and 1 fixed), 300 landmarks
+    seen by 4 key-frames, plus 40 landmarks seen only by the two fixed key-frames and 40 landmarks with one observation
+    (20 on a free key-frame, 20 on a fixed one).  Returns ba_scene's dict plus `single`: the single-observation landmarks."""
+    sc = ba_scene(n_kf=6, n_pt=380, target_obs=1520, seed=seed)
+    sc["poses_noisy"][1] = sc["poses_true"][1]            # key-frame 1 is fixed too: at its true pose
+    rng = np.random.default_rng(seed)
+    keep = sc["pt_idx"] < 300
+    kf, pt, px = [sc["kf_idx"][keep]], [sc["pt_idx"][keep]], [sc["px"][keep]]
+    from .se3 import se3_exp
+    for j in range(300, 380):
+        kfs = [0, 1] if j < 340 else [int(rng.integers(2, 6)) if j < 360 else int(rng.integers(0, 2))]
+        for k in kfs:
+            T = se3_exp(sc["poses_true"][k])
+            pc = T[:, :3] @ sc["pts_true"][j] + T[:, 3]
+            kf.append(np.array([k], np.int32))
+            pt.append(np.array([j], np.int32))
+            px.append(np.array([[FX * pc[0] / pc[2] + CX, FY * pc[1] / pc[2] + CY]]) + rng.normal(0, 1, (1, 2)))
+    sc.update(kf_idx=np.concatenate(kf).astype(np.int32), pt_idx=np.concatenate(pt).astype(np.int32), px=np.concatenate(px),
+              single=np.arange(340, 380))
+    return sc
+
+
 def shift_stream(stream: int, n_frames: int, noise_sigma: float = 2.0, plane_z: float = 2.0):
     """Cheap exact-ground-truth VO stream: a fronto-parallel textured plane seen by a camera that only translates
     parallel to it, i.e. integer-pixel sliding crops of one render.  Returns (frames u8 (n,H,W), depth (H,W) constant,
