@@ -8,6 +8,8 @@
 // f32 normal equations scaled by 2^-20, min-eigenvalue test, <= 30 iterations, eps^2 stop, the |delta + prev| <
 // 0.01 oscillation stop -- and pinned against cv2.calcOpticalFlowPyrLK in tests/test_oracle_klt.py (OpenCV's SIMD
 // build sums the f32 terms in a different order, so the pin is a tolerance, not bit-exactness).
+// The min-eigenvalue threshold is compared in float, as OpenCV stores it.  exact_sums = 1 adds the window sums in int64
+// and converts each once to float, which is klt.cu's arithmetic: in that mode the GPU must match bit for bit.
 #include <cmath>
 #include <cstring>
 #include <vector>
@@ -68,6 +70,8 @@ extern "C" void ora_klt(const uint8_t* ref, const uint8_t* cur, int w, int h, in
     const int W_BITS = 14;
     const float FLT_SCALE = 1.f / (1 << 20);
     const int max_count = std::min(std::max(p->max_iter, 0), 100);
+    const float min_eig = (float)p->min_eig;
+    const bool exact = p->exact_sums != 0;
     double eps = std::min(std::max(p->eps, 0.), 10.);
     eps *= eps;
     std::vector<short> Iw((size_t)win * win), dIw((size_t)2 * win * win);
@@ -105,6 +109,7 @@ extern "C" void ora_klt(const uint8_t* ref, const uint8_t* cur, int w, int h, in
             int iw00 = cv_round((1.f - a) * (1.f - b) * (1 << W_BITS)), iw01 = cv_round(a * (1.f - b) * (1 << W_BITS)),
                 iw10 = cv_round((1.f - a) * b * (1 << W_BITS)), iw11 = (1 << W_BITS) - iw00 - iw01 - iw10;
             float iA11 = 0, iA12 = 0, iA22 = 0;
+            int64_t xA11 = 0, xA12 = 0, xA22 = 0;
             for (int y = 0; y < win; ++y)
                 for (int x = 0; x < win; ++x) {
                     const int X = ipx + x, Y = ipy + y;
@@ -119,14 +124,26 @@ extern "C" void ora_klt(const uint8_t* ref, const uint8_t* cur, int w, int h, in
                     Iw[(size_t)y * win + x] = (short)ival;
                     dIw[2 * ((size_t)y * win + x)] = (short)ixval;
                     dIw[2 * ((size_t)y * win + x) + 1] = (short)iyval;
-                    iA11 += (float)(ixval * ixval);
-                    iA12 += (float)(ixval * iyval);
-                    iA22 += (float)(iyval * iyval);
+                    if (exact) {
+                        xA11 += (int64_t)ixval * ixval;
+                        xA12 += (int64_t)ixval * iyval;
+                        xA22 += (int64_t)iyval * iyval;
+                    } else {
+                        iA11 += (float)(ixval * ixval);
+                        iA12 += (float)(ixval * iyval);
+                        iA22 += (float)(iyval * iyval);
+                    }
                 }
+            if (exact) {
+                iA11 = (float)xA11;
+                iA12 = (float)xA12;
+                iA22 = (float)xA22;
+            }
             const float A11 = iA11 * FLT_SCALE, A12 = iA12 * FLT_SCALE, A22 = iA22 * FLT_SCALE;
             float D = A11 * A22 - A12 * A12;
             const float minEig = (A22 + A11 - std::sqrt((A11 - A22) * (A11 - A22) + 4.f * A12 * A12)) / (2 * win * win);
-            if (minEig < p->min_eig || D < 1.1920929e-07f) {
+            if (p->get_min_eig) err[i] = minEig;  // the last write is level 0's
+            if (minEig < min_eig || D < 1.1920929e-07f) {
                 if (level == 0) status[i] = 0;
                 continue;
             }
@@ -147,14 +164,24 @@ extern "C" void ora_klt(const uint8_t* ref, const uint8_t* cur, int w, int h, in
                 iw10 = cv_round((1.f - a) * b * (1 << W_BITS));
                 iw11 = (1 << W_BITS) - iw00 - iw01 - iw10;
                 float ib1 = 0, ib2 = 0;
+                int64_t xb1 = 0, xb2 = 0;
                 for (int y = 0; y < win; ++y)
                     for (int x = 0; x < win; ++x) {
                         const int X = inx + x, Y = iny + y;
                         const int diff = descale(J.I(X, Y) * iw00 + J.I(X + 1, Y) * iw01 + J.I(X, Y + 1) * iw10 + J.I(X + 1, Y + 1) * iw11, W_BITS - 5) -
                                          Iw[(size_t)y * win + x];
-                        ib1 += (float)(diff * dIw[2 * ((size_t)y * win + x)]);
-                        ib2 += (float)(diff * dIw[2 * ((size_t)y * win + x) + 1]);
+                        if (exact) {
+                            xb1 += diff * dIw[2 * ((size_t)y * win + x)];
+                            xb2 += diff * dIw[2 * ((size_t)y * win + x) + 1];
+                        } else {
+                            ib1 += (float)(diff * dIw[2 * ((size_t)y * win + x)]);
+                            ib2 += (float)(diff * dIw[2 * ((size_t)y * win + x) + 1]);
+                        }
                     }
+                if (exact) {
+                    ib1 = (float)xb1;
+                    ib2 = (float)xb2;
+                }
                 const float b1 = ib1 * FLT_SCALE, b2 = ib2 * FLT_SCALE;
                 const float dx = (float)((A12 * b2 - A22 * b1) * D), dy = (float)((A12 * b1 - A11 * b2) * D);
                 nx += dx;
@@ -170,7 +197,7 @@ extern "C" void ora_klt(const uint8_t* ref, const uint8_t* cur, int w, int h, in
                 pdx = dx;
                 pdy = dy;
             }
-            if (status[i] && level == 0) {  // err = mean |diff| / 32 at the final position
+            if (status[i] && level == 0 && !p->get_min_eig) {  // err = mean |diff| / 32 at the final position
                 const float fx = cur_xy[2 * i] - half, fy = cur_xy[2 * i + 1] - half;
                 const int inx = (int)std::floor(fx), iny = (int)std::floor(fy);
                 if (inx < -win || inx >= J.w || iny < -win || iny >= J.h) {
@@ -183,13 +210,18 @@ extern "C" void ora_klt(const uint8_t* ref, const uint8_t* cur, int w, int h, in
                 iw10 = cv_round((1.f - aa) * bb * (1 << W_BITS));
                 iw11 = (1 << W_BITS) - iw00 - iw01 - iw10;
                 float errval = 0.f;
+                int64_t xerr = 0;
                 for (int y = 0; y < win; ++y)
                     for (int x = 0; x < win; ++x) {
                         const int X = inx + x, Y = iny + y;
                         const int diff = descale(J.I(X, Y) * iw00 + J.I(X + 1, Y) * iw01 + J.I(X, Y + 1) * iw10 + J.I(X + 1, Y + 1) * iw11, W_BITS - 5) -
                                          Iw[(size_t)y * win + x];
-                        errval += std::abs((float)diff);
+                        if (exact)
+                            xerr += std::abs(diff);
+                        else
+                            errval += std::abs((float)diff);
                     }
+                if (exact) errval = (float)xerr;
                 err[i] = errval * 1.f / (32 * win * win);
             }
         }

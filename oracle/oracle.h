@@ -204,12 +204,19 @@ int ora_pose_only(const ora_camera* cam, int n, const double* pt_world /*3n*/, c
                   double* T_cw, uint8_t* inlier, double* depth);
 
 /* ---- KLT (src/Algorithm/Tracker.cpp:65-113 -> cv::calcOpticalFlowPyrLK) ------------------ */
+/* min_eig is compared in float, as OpenCV stores minEigThreshold: the threshold is (float)min_eig.
+ * exact_sums = 0 adds the window sums (A11, A12, A22, b1, b2 and the err sum) in f32 like OpenCV's scalar code;
+ * exact_sums = 1 adds the same integer products in int64 and converts each sum to float once, which is klt.cu's
+ * arithmetic (every other step is the same round-to-nearest f32 on both sides, so this mode matches it bit for bit).
+ * get_min_eig = 1 writes the level-0 minimum eigenvalue into err instead of the mean |diff| (OPTFLOW_LK_GET_MIN_EIGENVALS). */
 typedef struct {
-    int win;        /* 21 */
-    int max_level;  /* 4  */
-    int max_iter;   /* 30 */
-    double eps;     /* 0.001 */
-    double min_eig; /* 1e-4  */
+    int win;         /* 21 */
+    int max_level;   /* 4  */
+    int max_iter;    /* 30 */
+    double eps;      /* 0.001 */
+    double min_eig;  /* 1e-4  */
+    int exact_sums;  /* 0 */
+    int get_min_eig; /* 0 */
 } ora_klt_params;
 void ora_klt(const uint8_t* ref, const uint8_t* cur, int w, int h, int n, const float* ref_xy,
              float* cur_xy_inout, uint8_t* status, float* err, const ora_klt_params* p);

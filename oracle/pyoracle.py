@@ -58,7 +58,7 @@ class CeresStats(C.Structure):
 
 class KLTParams(C.Structure):
     _fields_ = [("win", C.c_int), ("max_level", C.c_int), ("max_iter", C.c_int), ("eps", C.c_double),
-                ("min_eig", C.c_double)]
+                ("min_eig", C.c_double), ("exact_sums", C.c_int), ("get_min_eig", C.c_int)]
 
 
 def _p(a):
@@ -426,13 +426,16 @@ class Oracle:
         return T, inl.astype(bool), depth, cnt
 
     # ---- KLT -------------------------------------------------------------------------------
-    def klt(self, ref, cur, ref_xy, cur_xy, win=21, max_level=4, max_iter=30, eps=0.001):
+    def klt(self, ref, cur, ref_xy, cur_xy, win=21, max_level=4, max_iter=30, eps=0.001, min_eig=1e-4, exact=False,
+            get_min_eig=False):
+        """cv::calcOpticalFlowPyrLK with OPTFLOW_USE_INITIAL_FLOW.  exact=True sums the window in int64 like klt.cu (bit-exact
+        to the GPU); the default sums in f32 like OpenCV.  get_min_eig=True returns the level-0 minimum eigenvalue as err."""
         h, w = ref.shape
         n = len(ref_xy)
         out = np.ascontiguousarray(cur_xy, np.float32).copy()
         status = np.zeros(n, np.uint8)
         err = np.zeros(n, np.float32)
-        prm = KLTParams(win, max_level, max_iter, eps, 1e-4)
+        prm = KLTParams(win, max_level, max_iter, eps, min_eig, int(exact), int(get_min_eig))
         self.lib.ora_klt(_p(np.ascontiguousarray(ref)), _p(np.ascontiguousarray(cur)), w, h, n,
                          _p(np.ascontiguousarray(ref_xy, np.float32)), _p(out), _p(status), _p(err), C.byref(prm))
         return out, status, err

@@ -653,7 +653,9 @@ class KLTParams(C.Structure):
     _fields_ = [("win", C.c_int), ("max_level", C.c_int), ("max_iter", C.c_int), ("eps", C.c_double), ("min_eig", C.c_double)]
 
 
-def _klt(self, ref_slot, cur_slot, offsets, ref_xy, cur_xy):
+def _klt(self, ref_slot, cur_slot, offsets, ref_xy, cur_xy, **overrides):
+    """Batched calcOpticalFlowPyrLK; keyword overrides (win, max_level, max_iter, eps, min_eig) replace fields of
+    ygzb_default_klt_params."""
     ref_slot = np.ascontiguousarray(ref_slot, np.int32)
     offsets = np.ascontiguousarray(offsets, np.int32)
     n = int(offsets[-1])
@@ -662,6 +664,10 @@ def _klt(self, ref_slot, cur_slot, offsets, ref_xy, cur_xy):
     err = np.zeros(n, np.float32)
     prm = KLTParams()
     self.lib.ygzb_default_klt_params(C.byref(prm))
+    for k, v in overrides.items():
+        if k not in ("win", "max_level", "max_iter", "eps", "min_eig"):
+            raise TypeError(f"unknown KLT parameter {k}")
+        setattr(prm, k, v)
     self.ctx.check(self.lib.ygzb_klt(self.h, len(ref_slot), _p(ref_slot), _p(np.ascontiguousarray(cur_slot, np.int32)), _p(offsets),
                                      _p(np.ascontiguousarray(ref_xy, np.float32)), _p(out), _p(status), _p(err), C.byref(prm)),
                    "ygzb_klt")

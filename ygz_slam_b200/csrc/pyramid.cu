@@ -11,6 +11,8 @@
 // multiple pitch (so level rows can be moved with 16-byte vectors / TMA boxes).
 // Roofline class: HBM.  Algorithmic bytes per frame (8 levels, grey in): 307,200 read + 102,400
 // written = 409,600 B.  One launch handles one level of `count` frames.
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace ygzb {
@@ -292,10 +294,14 @@ int launch_pyrdown_ptrs(ygzb_ctx* ctx, const uint8_t* const* d_src_ptr, uint8_t*
                         int dw, int dh, int dpitch, int count) {
     if (count <= 0) return YGZB_OK;
     const LevelGeom src{sw, sh, spitch, 0}, dst{dw, dh, dpitch, 0};
-    dim3 grid((dw + kDW - 1) / kDW, (dh + kDH - 1) / kDH, count);
-    ProfScope ps(ctx, kStagePyrDown);
-    pyrdown_ptr_kernel<<<grid, 256, 0, ctx->stream>>>(d_src_ptr, d_dst_ptr, src, dst);
-    YGZB_LAUNCHED(ctx);
+    // one image per gridDim.z index, which is limited to 65,535: larger batches (KLT with > 32,767 pairs) go in chunks
+    constexpr int kMaxGridZ = 65535;
+    for (int first = 0; first < count; first += kMaxGridZ) {
+        dim3 grid((dw + kDW - 1) / kDW, (dh + kDH - 1) / kDH, std::min(count - first, kMaxGridZ));
+        ProfScope ps(ctx, kStagePyrDown);
+        pyrdown_ptr_kernel<<<grid, 256, 0, ctx->stream>>>(d_src_ptr + first, d_dst_ptr + first, src, dst);
+        YGZB_LAUNCHED(ctx);
+    }
     return YGZB_OK;
 }
 

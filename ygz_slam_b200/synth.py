@@ -120,6 +120,25 @@ def stream_frame(k: int, stream: int = 0, noise_sigma: float = 2.0, tex_size: in
     return gray, depth, T
 
 
+def shifted_pair(w: int, h: int, dx: int, dy: int, seed: int = 0, noise: int = 2):
+    """Two w x h crops of the stream-0 texture: what is at (x, y) in the first is at (x + dx, y + dy) in the second.
+    Each crop gets its own seeded integer noise in [-noise, noise].  For optical flow with a known answer."""
+    key = (0, 2048)
+    if key not in _TEX_CACHE:
+        _TEX_CACHE[key] = texture(0x59475A00, 2048)
+    tex = _TEX_CACHE[key]
+    x0 = y0 = 128
+    n = tex.shape[0]
+    if not (0 <= x0 - dx and max(x0, x0 - dx) + w <= n and 0 <= y0 - dy and max(y0, y0 - dy) + h <= n):
+        raise ValueError("crop outside the texture")
+    rng = np.random.default_rng(seed)
+    out = []
+    for ys, xs in ((y0, x0), (y0 - dy, x0 - dx)):
+        g = tex[ys:ys + h, xs:xs + w].astype(np.int16) + rng.integers(-noise, noise + 1, (h, w))
+        out.append(np.clip(g, 0, 255).astype(np.uint8))
+    return out[0], out[1]
+
+
 def to_bgr(gray: np.ndarray) -> np.ndarray:
     return np.repeat(gray[..., None], 3, axis=-1).copy()
 
