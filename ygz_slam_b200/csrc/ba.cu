@@ -1036,19 +1036,8 @@ __global__ void __launch_bounds__(kPoseThreads) pose_only_kernel(const PoseOnlyA
         }
         finish_reduce(cnt);
     };
-    auto reduce32 = [&](double* part) {   // 32 values: a reduce-scatter butterfly, lane l ends with the warp total of part[l]
-        int off = 16;
-#pragma unroll
-        for (int m = 16; m >= 1; m >>= 1, off >>= 1) {
-            const bool up = (lane & off) != 0;
-#pragma unroll
-            for (int i = 0; i < m; ++i) {
-                const double keep = up ? part[i + m] : part[i];
-                const double send = up ? part[i] : part[i + m];
-                part[i] = keep + __shfl_xor_sync(0xFFFFFFFFu, send, off);
-            }
-        }
-        s_red[warp][lane] = part[0];
+    auto reduce32 = [&](double* part) {   // 32 values: lane l takes the warp total of part[l]
+        s_red[warp][lane] = warp_reduce_scatter<32>(part, lane);
         finish_reduce(32);
     };
     // R(aa) and dR / d aa of `pose` into shared memory (three threads, a column each); skipped when they are already there

@@ -51,28 +51,6 @@ __device__ __forceinline__ double warp_sum(double v) {
 }
 
 // block-wide sum of two values (result valid in every thread); s_tmp: 2 * (kW + 1) doubles
-// Sums of N per-lane values over the warp, all at once (a "reduce-scatter" butterfly): at every step a lane keeps one half of
-// its values and hands the other half to its partner, so N values cost N - 1 (+ log2(32 / N)) shuffles instead of 5 N.
-// N = 32: lane l returns the total of v[l]; N = 16: lanes 2 i and 2 i + 1 return the total of v[i].  (A warp flushes 42
-// sums per block pair: 420 32-bit shuffles with one butterfly per value was a quarter of the accumulate phase.)
-template <int N>
-__device__ __forceinline__ double warp_reduce_scatter(double* v, int lane) {
-    int off = 16;
-#pragma unroll
-    for (int n = N / 2; n >= 1; n >>= 1, off >>= 1) {
-        const bool up = (lane & off) != 0;
-#pragma unroll
-        for (int i = 0; i < n; ++i) {
-            const double keep = up ? v[i + n] : v[i];
-            const double send = up ? v[i] : v[i + n];
-            v[i] = keep + __shfl_xor_sync(0xFFFFFFFFu, send, off);
-        }
-    }
-#pragma unroll
-    for (; off >= 1; off >>= 1) v[0] += __shfl_xor_sync(0xFFFFFFFFu, v[0], off);
-    return v[0];
-}
-
 __device__ void block_sum2(double& v0, double& v1, double* s_tmp) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     v0 = warp_sum(v0);
@@ -717,11 +695,11 @@ __global__ void __launch_bounds__(kT) local_ba2_kernel(const BA2Args a) {
                 const double* R1 = s_Rlin[s_kfof[f1]];
                 const double* R2 = s_Rlin[s_kfof[f2]];
                 const int e_lo = st.ent ? s_estart[task] : 0, e_hi = st.ent ? s_estart[task + 1] : 0;
-                double acc[48];   // [0, 36) the 6 x 6 block, [36, 42) the right-hand side (diagonal pairs), the rest stays zero
+                double acc[kPairW];   // [0, 36) the 6 x 6 block, [36, 42) the right-hand side (diagonal pairs)
                 double* accS = acc;
                 double* accb = acc + 36;
 #pragma unroll
-                for (int t = 0; t < 48; ++t) acc[t] = 0;
+                for (int t = 0; t < kPairW; ++t) acc[t] = 0;
                 for (int ch = c_lo; ch < c_hi; ++ch) {
                     int jj, s1, s2;
                     if (st.ent) {
@@ -762,7 +740,8 @@ __global__ void __launch_bounds__(kT) local_ba2_kernel(const BA2Args a) {
                     }
                 }
                 {
-                    const double lo = warp_reduce_scatter<32>(acc, lane), hi = warp_reduce_scatter<16>(acc + 32, lane);
+                    // (42 sums: one butterfly per value would be 420 32-bit shuffles, a quarter of the accumulate phase)
+                    const double lo = warp_reduce_scatter<32>(acc, lane), hi = warp_reduce_scatter<16, kPairW - 32>(acc + 32, lane);
                     out[lane] = lo;
                     if (!(lane & 1) && 32 + (lane >> 1) < kPairW) out[32 + (lane >> 1)] = hi;
                 }
@@ -854,13 +833,18 @@ __global__ void __launch_bounds__(kT) local_ba2_kernel(const BA2Args a) {
     }
     const bool dup = s_bc[3] > 0;   // unsupported input: reported through stats, nothing is optimised
 
-    // optional phase timing (a.debug != null): cycles of CTA 0 / thread 0 per phase, summed over the trials
-    long long tph[8] = {0, 0, 0, 0, 0, 0, 0, 0}, tlast = clock64();
+    // optional phase timing (a.debug != null): cycles of thread 0 per phase, summed over the trials; kept in shared memory, not
+    // in 18 registers that every thread would hold through the whole LM loop
+    __shared__ long long s_tph[9];   // [8]: clock of the last tick
+    if (a.debug && tid == 0) {
+        for (int k = 0; k < 8; ++k) s_tph[k] = 0;
+        s_tph[8] = clock64();
+    }
     auto tick = [&](int ph) {
-        if (a.debug) {
+        if (a.debug && tid == 0) {
             const long long now = clock64();
-            tph[ph] += now - tlast;
-            tlast = now;
+            s_tph[ph] += now - s_tph[8];
+            s_tph[8] = now;
         }
     };
     bool fresh = false;   // Hpp / bp of the accepted state are in s_x (the prologue computed them for iteration 0)
@@ -1068,7 +1052,7 @@ __global__ void __launch_bounds__(kT) local_ba2_kernel(const BA2Args a) {
             stt[0] = iters; stt[1] = trials_total; stt[2] = chi_first; stt[3] = chi_last; stt[4] = lambda; stt[5] = s_bc[0];
             stt[6] = dup ? 1.0 : 0.0; stt[7] = 0;
             if (a.debug)
-                for (int k = 0; k < 8; ++k) a.debug[8 * (size_t)prob + k] = (double)tph[k];
+                for (int k = 0; k < 8; ++k) a.debug[8 * (size_t)prob + k] = (double)s_tph[k];
         }
     }
     cluster.sync();   // no CTA may exit while another still reads its shared memory

@@ -204,4 +204,42 @@ __device__ __forceinline__ float orderable_float(unsigned o) {
     return __uint_as_float(u);
 }
 
+// c ? a : b on values, opaque to the compiler.  Written as `c ? v[i] : v[j]` on an array, the choice may be folded into a load
+// from a selected ADDRESS; as a select of two registers pose_only_kernel spills 16 bytes less (sm_90a).
+__device__ __forceinline__ double select_f64(bool c, double a, double b) {
+    double r;
+    asm("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %1, 0;\n\tselp.f64 %0, %2, %3, p;\n\t}" : "=d"(r) : "r"((unsigned)c), "d"(a), "d"(b));
+    return r;
+}
+
+// Sums of N per-lane values over the warp, all at once (a "reduce-scatter" butterfly): at every step a lane keeps one half of
+// its values and hands the other half to its partner, so N values cost N - 1 (+ log2(32 / N)) shuffles instead of 5 N.
+// N = 32: lane l returns the total of v[l]; N = 16: lanes 2 i and 2 i + 1 return the total of v[i].  Only v[0, M) is read:
+// v[M, N) count as zeros (padding that need not be kept in registers).  v is overwritten.
+// Every loop has a trip count that is a compile-time constant before any loop is unrolled (the inner loop runs to N / 2 and
+// skips i >= n): the compiler unrolls inner loops first and leaves `for (i < n)` inside `for (n = N / 2; n >= 1; n >>= 1)`
+// rolled.  A rolled loop indexes v at run time, and v -- the caller's accumulators -- then lives in local memory, not registers.
+template <int N, int M = N>
+__device__ __forceinline__ double warp_reduce_scatter(double* v, int lane) {
+    static_assert((N == 16 || N == 32) && 2 * M > N && M <= N, "warp_reduce_scatter: N = 16 or 32 values, at most N / 2 of them padding");
+#pragma unroll
+    for (int s = 0; s < 5; ++s) {
+        const int n = (N >> 1) >> s, off = 16 >> s;
+        if (n == 0) {
+            v[0] += __shfl_xor_sync(0xFFFFFFFFu, v[0], off);
+            continue;
+        }
+        const bool up = (lane & off) != 0;
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) {
+            if (i >= n) continue;
+            const double hi = i + n < M ? v[i + n] : 0.0;
+            const double keep = select_f64(up, hi, v[i]);
+            const double send = select_f64(up, v[i], hi);
+            v[i] = keep + __shfl_xor_sync(0xFFFFFFFFu, send, off);
+        }
+    }
+    return v[0];
+}
+
 }  // namespace ygzb
