@@ -415,6 +415,50 @@ int ygzb_tracker_track(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, 
 int ygzb_tracker_make_keyframes(ygzb_tracker* t, int n, const ygzb_keyframe_job* jobs, const ygzb_ba_params* ba,
                                 ygzb_keyframe_result* results);
 
+/* ---- map record: the local map of one stream, out of a tracker and back into one ----------------------------------
+ * The reference keeps its map in Memory / MapPoint objects any caller can read, and its System declares SaveMap /
+ * LoadMap (include/ygz/system.h:63-67, never defined).  A map record is the tracker's side of that: `n_keyframes` ring
+ * entries of one stream as structure-of-arrays, sized by the caller from capacities (C = grid cells):
+ *   per key-frame [n_keyframes]      entry, T_cw[12], mp0, n_features, n_obs, image (W*H bytes of level 0; may be NULL)
+ *   per feature   [n_keyframes * C]  px[2], level, depth, pw[3]    packed key-frame after key-frame (n_features each)
+ *   per observation [n_keyframes * 4 * C]  obs_id, obs_px[2]      packed the same way (n_obs each): the older map
+ *                                                                   points tracked into the key-frame
+ * The header carries the geometry the record was made under; an import checks it.  Serialising a record is the
+ * caller's business.                                                                                               */
+#define YGZB_MAP_OBS_PER_CELL 4   /* observation capacity of a key-frame per grid cell */
+typedef struct {
+    int32_t width, height, cells, n_levels;   /* image size, grid cells, pyramid levels                             */
+    double K[4];                              /* fx, fy, cx, cy of the tracker (ygzb_tracker_create)                */
+    int32_t n_keyframes, pad;
+    int32_t* entry;        /* [n_keyframes] ring entry the key-frame was exported from                                */
+    double* T_cw;          /* [n_keyframes][12]                                                                      */
+    int64_t* mp0;          /* [n_keyframes] id of its first map point; ids are [mp0, mp0 + n_features)               */
+    int32_t* n_features;   /* [n_keyframes]                                                                          */
+    int32_t* n_obs;        /* [n_keyframes]                                                                          */
+    uint8_t* image;        /* [n_keyframes][height][width] or NULL                                                   */
+    double* px;            /* [n_keyframes * C][2] full-resolution pixel (Feature::_pixel)                            */
+    uint8_t* level;        /* [n_keyframes * C]                                                                      */
+    double* depth;         /* [n_keyframes * C]                                                                      */
+    double* pw;            /* [n_keyframes * C][3] MapPoint::_pos_world                                              */
+    int64_t* obs_id;       /* [n_keyframes * 4 * C] map point id                                                     */
+    double* obs_px;        /* [n_keyframes * 4 * C][2] measured pixel                                                */
+} ygzb_map_record;
+
+/* asynchronous like ygzb_tracker_track, and ordered behind every key-frame insertion and local BA already enqueued (it
+ * sees the BA's write-back): one kernel packs the live rows of ring entries entries[0 .. n_entries) of `stream` (and
+ * their level-0 images when out->image != NULL) into a staging buffer, one copy per array moves them to `out`.  The
+ * header, out->entry and out->n_keyframes are written before the call returns; everything else is valid after
+ * ygzb_synchronize(ctx).  The per-feature and per-observation arrays are copied at their full capacity: the rows past
+ * the live ones are zero.  Entries must be distinct and in [0, YGZB_TRACK_RING).                                     */
+int ygzb_tracker_export(ygzb_tracker* t, int stream, int n_entries, const int32_t* entries, ygzb_map_record* out);
+/* writes record `in` into ring entries entries[0 .. in->n_keyframes) of `stream` (any stream of any tracker with the same
+ * geometry and K), uploads image k into frame slot kf_slots[k] and builds its pyramid (ygzb_frames_upload); the
+ * entries' key-frame slots become kf_slots.  Asynchronous on the context's stream; the record is read before the call
+ * returns unless its arrays are page-locked, then it must stay valid until ygzb_synchronize(ctx).  The whole record is
+ * checked on the host first: a different geometry or K, a count over capacity, an entry or slot out of range or twice,
+ * a level >= the pyramid depth or a missing image returns YGZB_ERR_INVALID with the tracker untouched.             */
+int ygzb_tracker_import(ygzb_tracker* t, int stream, const int32_t* entries, const int32_t* kf_slots, const ygzb_map_record* in);
+
 #ifdef __cplusplus
 }
 #endif

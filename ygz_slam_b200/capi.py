@@ -43,6 +43,7 @@ EXPORTS = [
     "ygzb_project_align", "ygzb_sparse_align", "ygzb_default_ba_params", "ygzb_local_ba", "ygzb_local_ba_ceres", "ygzb_two_view_ba", "ygzb_pose_only",
     "ygzb_default_klt_params", "ygzb_klt",
     "ygzb_tracker_create", "ygzb_tracker_destroy", "ygzb_tracker_set_depth", "ygzb_tracker_upload", "ygzb_tracker_track", "ygzb_tracker_make_keyframes",
+    "ygzb_tracker_export", "ygzb_tracker_import",
 ]
 
 
@@ -675,3 +676,107 @@ def _klt(self, ref_slot, cur_slot, offsets, ref_xy, cur_xy, **overrides):
 
 
 Frames.klt = _klt
+
+
+# ---- map records of the device-resident tracker (ygzb_tracker_export / _import) ------------------------------------------
+TRACK_RING = 4          # YGZB_TRACK_RING
+MAP_OBS_PER_CELL = 4    # YGZB_MAP_OBS_PER_CELL
+_MAP_ARRAYS = ("entry", "T_cw", "mp0", "n_features", "n_obs", "image", "px", "level", "depth", "pw", "obs_id", "obs_px")
+
+
+class MapRecord(C.Structure):
+    _fields_ = ([("width", C.c_int32), ("height", C.c_int32), ("cells", C.c_int32), ("n_levels", C.c_int32), ("K", C.c_double * 4),
+                 ("n_keyframes", C.c_int32), ("pad", C.c_int32)] + [(k, C.c_void_p) for k in _MAP_ARRAYS])
+
+
+class MapBuffers:
+    """A ygzb_map_record with numpy arrays behind it, sized for `capacity` key-frames of a `width` x `height` image with
+    `cells` grid cells.  `rec` may be an existing MapRecord (e.g. an element of a ctypes array) to point at the arrays."""
+
+    def __init__(self, capacity, width, height, cells, images=True, rec=None):
+        F, O = capacity * cells, capacity * MAP_OBS_PER_CELL * cells
+        self.a = dict(entry=np.zeros(capacity, np.int32), T_cw=np.zeros((capacity, 12)), mp0=np.zeros(capacity, np.int64),
+                      n_features=np.zeros(capacity, np.int32), n_obs=np.zeros(capacity, np.int32),
+                      image=np.zeros((capacity, height, width), np.uint8) if images else None, px=np.zeros((F, 2)),
+                      level=np.zeros(F, np.uint8), depth=np.zeros(F), pw=np.zeros((F, 3)), obs_id=np.zeros(O, np.int64),
+                      obs_px=np.zeros((O, 2)))
+        self.rec = MapRecord() if rec is None else rec
+        for k in _MAP_ARRAYS:
+            setattr(self.rec, k, None if self.a[k] is None else self.a[k].ctypes.data)
+
+    @property
+    def header(self):
+        r = self.rec
+        return dict(width=r.width, height=r.height, cells=r.cells, n_levels=r.n_levels, K=tuple(r.K), n_keyframes=r.n_keyframes)
+
+    def keyframes(self):
+        """Per key-frame dict of its live rows (copies): entry, T_cw (3x4), mp0, px, level, depth, pw, obs_id, obs_px, image."""
+        a, out, f0, o0 = self.a, [], 0, 0
+        for k in range(self.rec.n_keyframes):
+            nf, no = int(a["n_features"][k]), int(a["n_obs"][k])
+            out.append(dict(entry=int(a["entry"][k]), T_cw=a["T_cw"][k].reshape(3, 4).copy(), mp0=int(a["mp0"][k]), px=a["px"][f0:f0 + nf].copy(),
+                            level=a["level"][f0:f0 + nf].copy(), depth=a["depth"][f0:f0 + nf].copy(), pw=a["pw"][f0:f0 + nf].copy(),
+                            obs_id=a["obs_id"][o0:o0 + no].copy(), obs_px=a["obs_px"][o0:o0 + no].copy(),
+                            image=None if a["image"] is None else a["image"][k].copy()))
+            f0 += nf
+            o0 += no
+        return out
+
+    def copy(self):
+        """An independent record with the same header and array contents."""
+        cap = len(self.a["entry"])
+        other = MapBuffers(cap, self.rec.width, self.rec.height, self.a["level"].shape[0] // cap, images=self.a["image"] is not None)
+        for k in _MAP_ARRAYS:
+            if self.a[k] is not None:
+                other.a[k][...] = self.a[k]
+        for k in ("width", "height", "cells", "n_levels", "n_keyframes", "pad"):
+            setattr(other.rec, k, getattr(self.rec, k))
+        other.rec.K[:] = list(self.rec.K)
+        return other
+
+
+class Tracker:
+    """The device-resident tracker (ygzb_tracker) on a frame pool; here for its map records (export / import)."""
+
+    def __init__(self, frames: Frames, n_streams: int, max_jobs: int, K):
+        self.frames, self.ctx, self.lib = frames, frames.ctx, frames.lib
+        self.lib.ygzb_tracker_create.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+        self.lib.ygzb_tracker_destroy.argtypes = [C.c_void_p]
+        self.lib.ygzb_tracker_destroy.restype = None
+        self.lib.ygzb_tracker_export.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+        self.lib.ygzb_tracker_import.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        Kd = np.ascontiguousarray(K, np.float64)
+        h = C.c_void_p()
+        self.ctx.check(self.lib.ygzb_tracker_create(frames.h, n_streams, max_jobs, _p(Kd), C.byref(h)), "ygzb_tracker_create")
+        self.h = h
+        self.n_streams = n_streams
+
+    def close(self):
+        if getattr(self, "h", None) and getattr(self.ctx, "h", None):
+            self.lib.ygzb_tracker_destroy(self.h)
+        self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def export(self, stream: int, entries, images: bool = True, out: MapBuffers | None = None) -> MapBuffers:
+        """Map record of ring entries `entries` of `stream`, complete (the call synchronises the context)."""
+        entries = np.ascontiguousarray(entries, np.int32)
+        if out is None:
+            f = self.frames
+            out = MapBuffers(TRACK_RING, f.lw[0], f.lh[0], self.ctx.n_cells, images=images)
+        self.ctx.check(self.lib.ygzb_tracker_export(self.h, int(stream), len(entries), _p(entries), C.byref(out.rec)), "ygzb_tracker_export")
+        self.ctx.synchronize()
+        return out
+
+    def import_(self, stream: int, entries, kf_slots, rec: MapBuffers):
+        entries = np.ascontiguousarray(entries, np.int32)
+        kf_slots = np.ascontiguousarray(kf_slots, np.int32)
+        self.ctx.check(self.lib.ygzb_tracker_import(self.h, int(stream), _p(entries), _p(kf_slots), C.byref(rec.rec)), "ygzb_tracker_import")
+        self.ctx.synchronize()
+
+
+Frames.tracker = lambda self, n_streams, max_jobs, K: Tracker(self, n_streams, max_jobs, K)

@@ -51,6 +51,7 @@ struct ygzb_tracker {
     cudaEvent_t e_main;    // recorded on the main stream after a tracking chain: the front stream must not overwrite its arrays earlier
     int cluster;           // CTAs per tracking problem (sparse alignment, pose-only): fixed, so that a frame's result does not
                            // depend on how many other frames share its batch (the summation order follows the cluster size)
+    void* d_xfer;          // staging of a map record (ygzb_tracker_export / _import), allocated on first use
 };
 
 namespace {
@@ -350,6 +351,150 @@ size_t babuild_carve(Carver& c, BABuild& B, size_t P, int cells, int n_jobs) {
     return c.bytes();
 }
 
+// ---- map records (ygzb_tracker_export / _import) -----------------------------------------------------------------------
+static_assert(YGZB_MAP_OBS_PER_CELL == kTrackMaxLocal, "a key-frame's observation capacity is kTrackMaxLocal * cells");
+constexpr int kXferChunks = 16;   // CTAs per key-frame of the pack / unpack kernels
+
+struct MapXfer {   // device staging of one record: at most YGZB_TRACK_RING key-frames, packed like ygzb_map_record
+    double* T;
+    long long* mp0;
+    int32_t *n_feat, *n_obs;
+    double *px, *depth, *pw, *obs_px;
+    uint8_t *level, *image;
+    long long* obs_id;
+};
+
+struct MapXferJob {   // kernel argument: the ring entries of a record and, for an import, its packed offsets and slots
+    int n, stream, with_image;
+    int entry[YGZB_TRACK_RING], slot[YGZB_TRACK_RING];
+    int foff[YGZB_TRACK_RING + 1], ooff[YGZB_TRACK_RING + 1];
+};
+
+size_t xfer_carve(Carver& c, MapXfer& X, size_t cells, size_t cap_obs, size_t WH) {
+    const size_t R = YGZB_TRACK_RING;
+    X.T = c.take<double>(R * 12); X.mp0 = c.take<long long>(R); X.n_feat = c.take<int32_t>(R); X.n_obs = c.take<int32_t>(R);
+    X.px = c.take<double>(R * cells * 2); X.level = c.take<uint8_t>(R * cells); X.depth = c.take<double>(R * cells);
+    X.pw = c.take<double>(R * cells * 3); X.obs_id = c.take<long long>(R * cap_obs); X.obs_px = c.take<double>(R * cap_obs * 2);
+    X.image = c.take<uint8_t>(R * WH);
+    return c.bytes();
+}
+
+// export: CTA (k, y) fills rows [k * cells, (k + 1) * cells) of the packed feature arrays and [k * cap_obs, (k + 1) * cap_obs)
+// of the observation arrays -- the live rows of all requested entries, back to back, then zeros up to the record's capacity
+// -- and the level-0 image of key-frame k
+__global__ void __launch_bounds__(256) map_pack_kernel(TrackStore st, MapXfer X, MapXferJob job, int cap_obs, const uint8_t* __restrict__ pyr,
+                                                       size_t slot_stride, unsigned lv0_off, int lv0_pitch) {
+    const int k = blockIdx.x, tid = threadIdx.x, n = job.n;
+    int foff[YGZB_TRACK_RING + 1], ooff[YGZB_TRACK_RING + 1];
+    foff[0] = ooff[0] = 0;
+    for (int q = 0; q < YGZB_TRACK_RING; ++q) {
+        const int e = job.stream * st.R + job.entry[q < n ? q : 0];
+        foff[q + 1] = foff[q] + (q < n ? st.kf_n[e] : 0);
+        ooff[q + 1] = ooff[q] + (q < n ? st.kf_nobs[e] : 0);
+    }
+    const int e = job.stream * st.R + job.entry[k];
+    if (blockIdx.y == 0) {
+        if (tid < 12) X.T[12 * k + tid] = st.kf_T[12 * (size_t)e + tid];
+        if (tid == 0) {
+            X.mp0[k] = st.kf_mp0[e];
+            X.n_feat[k] = foff[k + 1] - foff[k];
+            X.n_obs[k] = ooff[k + 1] - ooff[k];
+        }
+    }
+    const int step = gridDim.y * blockDim.x, first = blockIdx.y * blockDim.x + tid;
+    for (int i = k * st.cells + first; i < (k + 1) * st.cells; i += step) {
+        double p0 = 0, p1 = 0, d = 0, w0 = 0, w1 = 0, w2 = 0;
+        uint8_t L = 0;
+        if (i < foff[n]) {
+            int kk = 0;
+            while (i >= foff[kk + 1]) ++kk;
+            const size_t fe = (size_t)(job.stream * st.R + job.entry[kk]) * st.cells + (i - foff[kk]);
+            p0 = st.kf_px[2 * fe]; p1 = st.kf_px[2 * fe + 1];
+            L = st.kf_level[fe];
+            d = st.kf_depth[fe];
+            w0 = st.kf_pw[3 * fe]; w1 = st.kf_pw[3 * fe + 1]; w2 = st.kf_pw[3 * fe + 2];
+        }
+        X.px[2 * (size_t)i] = p0; X.px[2 * (size_t)i + 1] = p1;
+        X.level[i] = L;
+        X.depth[i] = d;
+        X.pw[3 * (size_t)i] = w0; X.pw[3 * (size_t)i + 1] = w1; X.pw[3 * (size_t)i + 2] = w2;
+    }
+    for (int i = k * cap_obs + first; i < (k + 1) * cap_obs; i += step) {
+        long long id = 0;
+        double u = 0, v = 0;
+        if (i < ooff[n]) {
+            int kk = 0;
+            while (i >= ooff[kk + 1]) ++kk;
+            const size_t q = (size_t)(job.stream * st.R + job.entry[kk]) * cap_obs + (i - ooff[kk]);
+            id = st.kf_obs_id[q];
+            u = st.kf_obs_px[2 * q]; v = st.kf_obs_px[2 * q + 1];
+        }
+        X.obs_id[i] = id;
+        X.obs_px[2 * (size_t)i] = u; X.obs_px[2 * (size_t)i + 1] = v;
+    }
+    if (job.with_image) {
+        const uint8_t* src = pyr + (size_t)st.kf_slot[e] * slot_stride + lv0_off;
+        uint8_t* dst = X.image + (size_t)k * st.W * st.H;
+        for (int i = first; i < st.W * st.H; i += step) {
+            const int y = i / st.W, x = i - y * st.W;
+            dst[i] = src[(size_t)y * lv0_pitch + x];
+        }
+    }
+}
+
+// import: CTA (k, y) scatters key-frame k of the packed record into its ring entry (live rows only)
+__global__ void __launch_bounds__(256) map_unpack_kernel(TrackStore st, MapXfer X, MapXferJob job, int cap_obs) {
+    const int k = blockIdx.x, tid = threadIdx.x;
+    const int e = job.stream * st.R + job.entry[k];
+    const int nf = job.foff[k + 1] - job.foff[k], no = job.ooff[k + 1] - job.ooff[k];
+    if (blockIdx.y == 0) {
+        if (tid < 12) st.kf_T[12 * (size_t)e + tid] = X.T[12 * k + tid];
+        if (tid == 0) {
+            st.kf_n[e] = nf;
+            st.kf_nobs[e] = no;
+            st.kf_slot[e] = job.slot[k];
+            st.kf_mp0[e] = X.mp0[k];
+        }
+    }
+    const int step = gridDim.y * blockDim.x, first = blockIdx.y * blockDim.x + tid;
+    for (int g = first; g < nf; g += step) {
+        const size_t s = (size_t)job.foff[k] + g, fe = (size_t)e * st.cells + g;
+        st.kf_px[2 * fe] = X.px[2 * s]; st.kf_px[2 * fe + 1] = X.px[2 * s + 1];
+        st.kf_level[fe] = X.level[s];
+        st.kf_depth[fe] = X.depth[s];
+        st.kf_pw[3 * fe] = X.pw[3 * s]; st.kf_pw[3 * fe + 1] = X.pw[3 * s + 1]; st.kf_pw[3 * fe + 2] = X.pw[3 * s + 2];
+    }
+    for (int q = first; q < no; q += step) {
+        const size_t s = (size_t)job.ooff[k] + q, d = (size_t)e * cap_obs + q;
+        st.kf_obs_id[d] = X.obs_id[s];
+        st.kf_obs_px[2 * d] = X.obs_px[2 * s]; st.kf_obs_px[2 * d + 1] = X.obs_px[2 * s + 1];
+    }
+}
+
+int tracker_xfer(ygzb_tracker* t, MapXfer& X) {
+    const TrackStore& st = t->st;
+    Carver c(nullptr);
+    const size_t bytes = xfer_carve(c, X, (size_t)st.cells, (size_t)t->b.cap, (size_t)st.W * st.H);
+    if (!t->d_xfer) YGZB_CUDA(t->ctx, cudaMalloc(&t->d_xfer, bytes));
+    Carver d(t->d_xfer);
+    xfer_carve(d, X, (size_t)st.cells, (size_t)t->b.cap, (size_t)st.W * st.H);
+    return YGZB_OK;
+}
+
+// distinct ring entries in range (and distinct frame slots in range when `slots` is given)
+int check_entries(ygzb_tracker* t, int n, const int32_t* entries, const int32_t* slots, const char* what) {
+    ygzb_ctx* ctx = t->ctx;
+    for (int k = 0; k < n; ++k) {
+        if (entries[k] < 0 || entries[k] >= YGZB_TRACK_RING) return set_error(ctx, YGZB_ERR_INVALID, "%s: ring entry %d out of range", what, entries[k]);
+        if (slots && (slots[k] < 0 || slots[k] >= t->f->capacity)) return set_error(ctx, YGZB_ERR_INVALID, "%s: frame slot %d out of range", what, slots[k]);
+        for (int k2 = 0; k2 < k; ++k2) {
+            if (entries[k2] == entries[k]) return set_error(ctx, YGZB_ERR_INVALID, "%s: ring entry %d given twice", what, entries[k]);
+            if (slots && slots[k2] == slots[k]) return set_error(ctx, YGZB_ERR_INVALID, "%s: frame slot %d given twice", what, slots[k]);
+        }
+    }
+    return YGZB_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -472,6 +617,7 @@ void ygzb_tracker_destroy(ygzb_tracker* t) {
     if (t->d_kfjobs) cudaFree(t->d_kfjobs);
     if (t->d_kfres) cudaFree(t->d_kfres);
     if (t->d_ba) cudaFree(t->d_ba);
+    if (t->d_xfer) cudaFree(t->d_xfer);
     if (t->staged) cudaEventDestroy(t->staged);
     if (t->front) {
         cudaStreamSynchronize(t->front);
@@ -643,6 +789,131 @@ int ygzb_tracker_make_keyframes(ygzb_tracker* t, int n, const ygzb_keyframe_job*
     }
     YGZB_CUDA(ctx, cudaMemcpyAsync(results, t->d_kfres, sizeof(ygzb_keyframe_result) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
     return YGZB_OK;
+}
+
+int ygzb_tracker_export(ygzb_tracker* t, int stream, int n_entries, const int32_t* entries, ygzb_map_record* out) {
+    if (!t || !out) return YGZB_ERR_INVALID;
+    ygzb_ctx* ctx = t->ctx;
+    const TrackStore& st = t->st;
+    if (stream < 0 || stream >= st.S) return set_error(ctx, YGZB_ERR_INVALID, "export: stream %d out of range", stream);
+    if (n_entries < 0 || n_entries > YGZB_TRACK_RING || (n_entries && !entries))
+        return set_error(ctx, YGZB_ERR_INVALID, "export: %d entries (at most %d)", n_entries, YGZB_TRACK_RING);
+    if (n_entries && (!out->entry || !out->T_cw || !out->mp0 || !out->n_features || !out->n_obs || !out->px || !out->level || !out->depth ||
+                      !out->pw || !out->obs_id || !out->obs_px))
+        return set_error(ctx, YGZB_ERR_INVALID, "export: null array in the record");
+    int rc = check_entries(t, n_entries, entries, nullptr, "export");
+    if (rc != YGZB_OK) return rc;
+    cudaSetDevice(ctx->device);
+    out->width = st.W; out->height = st.H; out->cells = st.cells; out->n_levels = ctx->geo.n_levels;
+    out->K[0] = st.fx; out->K[1] = st.fy; out->K[2] = st.cx; out->K[3] = st.cy;
+    out->n_keyframes = n_entries;
+    out->pad = 0;
+    for (int k = 0; k < n_entries; ++k) out->entry[k] = entries[k];
+    if (n_entries == 0) return YGZB_OK;
+    MapXfer X;
+    rc = tracker_xfer(t, X);
+    if (rc != YGZB_OK) return rc;
+    MapXferJob job{};
+    job.n = n_entries;
+    job.stream = stream;
+    job.with_image = out->image != nullptr;
+    for (int k = 0; k < n_entries; ++k) job.entry[k] = entries[k];
+    // on the context's stream: behind every key-frame insertion and local BA enqueued so far; behind the front stream's
+    // uploads as well, in case a caller uploads into a key-frame's slot
+    YGZB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, t->e_up, 0));
+    {
+        ProfScope ps(ctx, kStageOther);
+        const LevelGeom& lv = ctx->geo.lv[0];
+        map_pack_kernel<<<dim3((unsigned)n_entries, kXferChunks), 256, 0, ctx->stream>>>(st, X, job, t->b.cap, t->f->d_pyr, ctx->slot_stride,
+                                                                                          lv.off, lv.pitch);
+        YGZB_LAUNCHED(ctx);
+    }
+    const size_t n = (size_t)n_entries, F = n * st.cells, O = n * t->b.cap;
+    auto d2h = [&](void* dst, const void* src, size_t bytes) {
+        return check_cuda(ctx, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, ctx->stream), "D2H(map record)");
+    };
+    if (rc == YGZB_OK) rc = d2h(out->T_cw, X.T, n * 12 * sizeof(double));
+    if (rc == YGZB_OK) rc = d2h(out->mp0, X.mp0, n * sizeof(int64_t));
+    if (rc == YGZB_OK) rc = d2h(out->n_features, X.n_feat, n * sizeof(int32_t));
+    if (rc == YGZB_OK) rc = d2h(out->n_obs, X.n_obs, n * sizeof(int32_t));
+    if (rc == YGZB_OK) rc = d2h(out->px, X.px, F * 2 * sizeof(double));
+    if (rc == YGZB_OK) rc = d2h(out->level, X.level, F);
+    if (rc == YGZB_OK) rc = d2h(out->depth, X.depth, F * sizeof(double));
+    if (rc == YGZB_OK) rc = d2h(out->pw, X.pw, F * 3 * sizeof(double));
+    if (rc == YGZB_OK) rc = d2h(out->obs_id, X.obs_id, O * sizeof(int64_t));
+    if (rc == YGZB_OK) rc = d2h(out->obs_px, X.obs_px, O * 2 * sizeof(double));
+    if (rc == YGZB_OK && out->image) rc = d2h(out->image, X.image, n * st.W * st.H);
+    return rc;
+}
+
+int ygzb_tracker_import(ygzb_tracker* t, int stream, const int32_t* entries, const int32_t* kf_slots, const ygzb_map_record* in) {
+    if (!t || !in) return YGZB_ERR_INVALID;
+    ygzb_ctx* ctx = t->ctx;
+    const TrackStore& st = t->st;
+    // ---- the whole record is checked before anything is enqueued
+    if (stream < 0 || stream >= st.S) return set_error(ctx, YGZB_ERR_INVALID, "import: stream %d out of range", stream);
+    if (in->width != st.W || in->height != st.H || in->cells != st.cells || in->n_levels != ctx->geo.n_levels)
+        return set_error(ctx, YGZB_ERR_INVALID, "import: record geometry %dx%d, %d cells, %d levels; tracker %dx%d, %d cells, %d levels", in->width,
+                         in->height, in->cells, in->n_levels, st.W, st.H, st.cells, ctx->geo.n_levels);
+    if (!(in->K[0] == st.fx && in->K[1] == st.fy && in->K[2] == st.cx && in->K[3] == st.cy))
+        return set_error(ctx, YGZB_ERR_INVALID, "import: record intrinsics differ from the tracker's");
+    const int n = in->n_keyframes;
+    if (n < 0 || n > YGZB_TRACK_RING) return set_error(ctx, YGZB_ERR_INVALID, "import: %d key-frames (at most %d)", n, YGZB_TRACK_RING);
+    if (n == 0) return YGZB_OK;
+    if (!entries || !kf_slots || !in->T_cw || !in->mp0 || !in->n_features || !in->n_obs)
+        return set_error(ctx, YGZB_ERR_INVALID, "import: null array in the record");
+    if (!in->image) return set_error(ctx, YGZB_ERR_INVALID, "import: the record has no images");
+    int rc = check_entries(t, n, entries, kf_slots, "import");
+    if (rc != YGZB_OK) return rc;
+    MapXferJob job{};
+    job.n = n;
+    job.stream = stream;
+    for (int k = 0; k < n; ++k) {
+        if (in->n_features[k] < 0 || in->n_features[k] > st.cells)
+            return set_error(ctx, YGZB_ERR_INVALID, "import: key-frame %d has %d features (capacity %d)", k, in->n_features[k], st.cells);
+        if (in->n_obs[k] < 0 || in->n_obs[k] > t->b.cap)
+            return set_error(ctx, YGZB_ERR_INVALID, "import: key-frame %d has %d observations (capacity %d)", k, in->n_obs[k], t->b.cap);
+        job.entry[k] = entries[k];
+        job.slot[k] = kf_slots[k];
+        job.foff[k + 1] = job.foff[k] + in->n_features[k];
+        job.ooff[k + 1] = job.ooff[k] + in->n_obs[k];
+    }
+    const size_t F = (size_t)job.foff[n], O = (size_t)job.ooff[n];
+    if ((F && (!in->px || !in->level || !in->depth || !in->pw)) || (O && (!in->obs_id || !in->obs_px)))
+        return set_error(ctx, YGZB_ERR_INVALID, "import: null array in the record");
+    for (size_t i = 0; i < F; ++i)
+        if (in->level[i] >= ctx->geo.n_levels)
+            return set_error(ctx, YGZB_ERR_INVALID, "import: feature %zu on level %d of a %d-level pyramid", i, (int)in->level[i], ctx->geo.n_levels);
+    // ---- enqueue on the context's stream, behind the front stream's uploads and sparse alignment (they read the ring and
+    //      the key-frame slots); the next upload or tracking chain waits for e_fill
+    cudaSetDevice(ctx->device);
+    MapXfer X;
+    rc = tracker_xfer(t, X);
+    if (rc != YGZB_OK) return rc;
+    YGZB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, t->e_up, 0));
+    YGZB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, t->e_front, 0));
+    auto h2d = [&](void* dst, const void* src, size_t bytes) {
+        return bytes ? check_cuda(ctx, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, ctx->stream), "H2D(map record)") : YGZB_OK;
+    };
+    const size_t nk = (size_t)n;
+    if (rc == YGZB_OK) rc = h2d(X.T, in->T_cw, nk * 12 * sizeof(double));
+    if (rc == YGZB_OK) rc = h2d(X.mp0, in->mp0, nk * sizeof(int64_t));
+    if (rc == YGZB_OK) rc = h2d(X.px, in->px, F * 2 * sizeof(double));
+    if (rc == YGZB_OK) rc = h2d(X.level, in->level, F);
+    if (rc == YGZB_OK) rc = h2d(X.depth, in->depth, F * sizeof(double));
+    if (rc == YGZB_OK) rc = h2d(X.pw, in->pw, F * 3 * sizeof(double));
+    if (rc == YGZB_OK) rc = h2d(X.obs_id, in->obs_id, O * sizeof(int64_t));
+    if (rc == YGZB_OK) rc = h2d(X.obs_px, in->obs_px, O * 2 * sizeof(double));
+    if (rc != YGZB_OK) return rc;
+    {
+        ProfScope ps(ctx, kStageOther);
+        map_unpack_kernel<<<dim3((unsigned)n, kXferChunks), 256, 0, ctx->stream>>>(st, X, job, t->b.cap);
+        YGZB_LAUNCHED(ctx);
+    }
+    const size_t WH = (size_t)st.W * st.H;
+    for (int k = 0; k < n && rc == YGZB_OK; ++k) rc = ygzb_frames_upload(t->f, kf_slots[k], 1, in->image + k * WH, 1, WH);
+    if (rc == YGZB_OK) rc = check_cuda(ctx, cudaEventRecord(t->e_fill, ctx->stream), "cudaEventRecord");
+    return rc;
 }
 
 }  // extern "C"

@@ -23,6 +23,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <deque>
+#include <memory>
 #include <string>
 #include <thread>
 #include <vector>
@@ -542,6 +543,7 @@ class Engine {
     struct Win { int stream, first, count, job0; };   // a window in flight: frames [first, first + count) of a stream (job0 < 0: first frame)
   public:
     Engine(ygzb_ctx* ctx, int n_streams, int window, const Params& p) : ctx_(ctx), S_(n_streams), F_(std::max(1, window)), prm_(p), st_(n_streams) {
+        for (int i = 0; i < S_; ++i) order_.push_back(i);
         // YGZ_VO_BLOCKING_SYNC=1: sleep instead of spinning in the one synchronisation per round (hosts with fewer CPUs than
         // engine threads; bench.py sets it when the threads of all ranks outnumber the CPUs it may use)
         const char* e = std::getenv("YGZ_VO_BLOCKING_SYNC");
@@ -553,11 +555,14 @@ class Engine {
         if (h_res_) ygzb_host_free(h_res_);
         if (h_kres_) ygzb_host_free(h_kres_);
     }
+    // order[i] = the caller's index of tracker stream i (images, depth maps, trajectory rows); identity unless set
+    void set_order(const std::vector<int>& order) { order_ = order; }
+    const std::vector<int>& order() const { return order_; }
     int init(const double* const* depth) {
         CHK(ygzb_frames_create(ctx_, S_ * F_ + S_ * YGZB_TRACK_RING, &fr_));
         const double K[4] = {FX, FY, CX, CY};
         CHK(ygzb_tracker_create(fr_, S_, S_ * F_, K, &tr_));
-        for (int i = 0; i < S_; ++i) CHK(ygzb_tracker_set_depth(tr_, i, depth[i]));
+        for (int i = 0; i < S_; ++i) CHK(ygzb_tracker_set_depth(tr_, i, depth[order_[i]]));
         void* p = nullptr;
         CHK(ygzb_host_alloc(&p, sizeof(ygzb_track_result) * (size_t)S_ * F_));
         h_res_ = static_cast<ygzb_track_result*>(p);
@@ -672,7 +677,7 @@ class Engine {
                     w = sure >= 1 ? std::min(F_, sure) : std::min(F_, kSpeculativeFrames);
                 }
                 w = std::min(w, limit - s.next_frame);
-                CHK(ygzb_tracker_upload(tr_, i * F_, w, images[i] + (size_t)s.next_frame * W * H, (size_t)W * H));
+                CHK(ygzb_tracker_upload(tr_, i * F_, w, images[order_[i]] + (size_t)s.next_frame * W * H, (size_t)W * H));
                 h2d_image_bytes += (long long)w * W * H;
                 if (s.kfs.empty()) {
                     wins_.push_back({i, s.next_frame, 1, -1});
@@ -720,10 +725,31 @@ class Engine {
         }
     }
 
+    // local map of stream i (every key-frame still in its ring, oldest first) into `rec`: asynchronous, valid after
+    // ygzb_synchronize; call with nothing in flight (after run_until)
+    int export_map(int i, ygzb_map_record* rec) const {
+        std::vector<int32_t> entries;
+        for (const KfInfo& kf : st_[i].kfs) entries.push_back(kf.entry);
+        return ygzb_tracker_export(tr_, i, (int)entries.size(), entries.data(), rec);
+    }
+    // stream i continues a stream of another engine: its map (exported by export_map) goes into the same ring entries, its
+    // key-frame images into this engine's key-frame slots of stream i, and its host bookkeeping is taken over as it is
+    int adopt(int i, const EStream& s, const ygzb_map_record* rec) {
+        std::vector<int32_t> entries, slots;
+        for (const KfInfo& kf : s.kfs) {
+            entries.push_back(kf.entry);
+            slots.push_back(S_ * F_ + i * YGZB_TRACK_RING + kf.entry);
+        }
+        if (rec->n_keyframes != (int)entries.size()) return YGZB_ERR_INVALID;
+        CHK(ygzb_tracker_import(tr_, i, entries.data(), slots.data(), rec));
+        st_[i] = s;
+        return YGZB_OK;
+    }
+
   private:
     void put_pose(double* traj, int stream, int n_frames, int frame, const EStream& s) const {
         if (!traj) return;
-        double* out = traj + ((size_t)stream * n_frames + frame) * 12;
+        double* out = traj + ((size_t)order_[stream] * n_frames + frame) * 12;
         for (int c = 0; c < 12; ++c) out[c] = s.has_pose ? s.T.m[c] : NAN;
     }
     ygzb_keyframe_job make_kf_job(int stream, int frame_slot, int track_job) const {
@@ -762,8 +788,154 @@ class Engine {
     ygzb_keyframe_result* h_kres_ = nullptr;
     ygzb_ba_params ba_;
     std::vector<Win> wins_;
+    std::vector<int> order_;
     bool blocking_sync_ = false;
 };
+
+// host arrays behind a map record of up to YGZB_TRACK_RING key-frames (ygzb_map_record capacities)
+struct MapBuf {
+    std::vector<int32_t> entry, n_features, n_obs;
+    std::vector<int64_t> mp0, obs_id;
+    std::vector<double> T, px, depth, pw, obs_px;
+    std::vector<uint8_t> level, image;
+    ygzb_map_record rec{};
+    explicit MapBuf(int cells) {
+        const size_t R = YGZB_TRACK_RING, F = R * cells, O = R * YGZB_MAP_OBS_PER_CELL * cells;
+        entry.resize(R); n_features.resize(R); n_obs.resize(R); mp0.resize(R); T.resize(12 * R); image.resize(R * W * H);
+        px.resize(2 * F); level.resize(F); depth.resize(F); pw.resize(3 * F); obs_id.resize(O); obs_px.resize(2 * O);
+        rec.entry = entry.data(); rec.T_cw = T.data(); rec.mp0 = mp0.data(); rec.n_features = n_features.data(); rec.n_obs = n_obs.data();
+        rec.image = image.data(); rec.px = px.data(); rec.level = level.data(); rec.depth = depth.data(); rec.pw = pw.data();
+        rec.obs_id = obs_id.data(); rec.obs_px = obs_px.data();
+    }
+};
+
+// Device-resident engine over the streams of one host thread; with handoff >= 0 the streams move to a new tracker at frame
+// `handoff` (see ygz_vo_run_handoff).  Shared by ygz_vo_run (handoff < 0) and ygz_vo_run_handoff.
+int run_engine(ygzb_ctx* ctx, int device, const ygzb_params* params, int n_threads, int n_streams, int n_frames,
+               const uint8_t* const* images, const double* const* depth, int kf_min_frames, double kf_min_rot, double kf_min_trans,
+               int warm, int window, int handoff, ygzb_map_record* maps, double* traj, int64_t* stats, double* seconds, double* device_ms,
+               int64_t* totals) {
+    if (!ctx || !params || n_streams < 1 || n_frames < 1 || !images || !depth || !traj || !stats || !seconds) return YGZB_ERR_INVALID;
+    n_threads = std::max(1, std::min(n_threads, n_streams));
+    warm = std::max(0, std::min(warm, n_frames - 1));
+    if (handoff >= 0) handoff = std::min(handoff, n_frames);
+    for (auto& v : g_stage_ns) v.store(0);
+    std::vector<int> rcs(n_threads, YGZB_OK);
+    std::vector<std::vector<long long>> tot(n_threads, std::vector<long long>(4, 0));
+    std::barrier sync_point(n_threads);
+    std::chrono::steady_clock::time_point t_begin, t_end;
+    auto worker = [&](int t) {
+        const int s0 = (int)((long)n_streams * t / n_threads), s1 = (int)((long)n_streams * (t + 1) / n_threads), ns = s1 - s0;
+        const Params prm{kf_min_frames, kf_min_rot, kf_min_trans};
+        ygzb_ctx* my = ctx;
+        bool own_ctx = t > 0;   // this thread created `my`
+        int rc = YGZB_OK;
+        if (t > 0) rc = ygzb_create(device, params, &my);
+        {
+            auto eng = std::make_unique<Engine>(my, ns, window, prm);
+            if (rc == YGZB_OK) rc = eng->init(depth + s0);
+            double* my_traj = traj + (size_t)s0 * n_frames * 12;
+            bool timed = false, handed = false;
+            long long launch_base = 0;
+            // run to frame `handoff`, export every stream's map, tear the tracker, its frame pool and (but for the caller's)
+            // the context down, and carry the streams over to a fresh engine on a new context in reverse order
+            auto hand_over = [&]() -> int {
+                CHK(eng->run_until(images + s0, n_frames, handoff, my_traj));
+                int cells_r = 0, cells_c = 0;
+                ygzb_grid_dims(my, &cells_r, &cells_c);
+                std::vector<MapBuf> own;
+                std::vector<ygzb_map_record*> recs(ns);
+                if (!maps) own.reserve(ns);
+                for (int i = 0; i < ns; ++i) {
+                    if (maps) {
+                        recs[i] = maps + s0 + eng->order()[i];
+                    } else {
+                        own.emplace_back(cells_r * cells_c);
+                        recs[i] = &own.back().rec;
+                    }
+                    CHK(eng->export_map(i, recs[i]));
+                }
+                CHK(ygzb_synchronize(my));
+                const std::vector<EStream> carried = eng->streams();
+                const std::vector<int> order = eng->order();
+                if (timed) {
+                    tot[t][0] += ygzb_launch_count(my) - launch_base;
+                    tot[t][1] += eng->h2d_image_bytes; tot[t][2] += eng->h2d_other_bytes; tot[t][3] += eng->d2h_bytes;
+                }
+                eng.reset();
+                if (own_ctx) ygzb_destroy(my);
+                my = nullptr;
+                own_ctx = true;
+                const int created = ygzb_create(device, params, &my);
+                eng = std::make_unique<Engine>(my, ns, window, prm);
+                std::vector<int> reversed(ns);
+                for (int j = 0; j < ns; ++j) reversed[j] = order[ns - 1 - j];
+                eng->set_order(reversed);
+                CHK(created);
+                launch_base = ygzb_launch_count(my);
+                CHK(eng->init(depth + s0));
+                for (int j = 0; j < ns; ++j) CHK(eng->adopt(j, carried[ns - 1 - j], recs[ns - 1 - j]));
+                return YGZB_OK;
+            };
+            auto advance = [&](int limit) {
+                if (rc == YGZB_OK && handoff >= 0 && !handed && (handoff < limit || limit == n_frames)) {
+                    handed = true;
+                    rc = hand_over();
+                }
+                if (rc == YGZB_OK) rc = eng->run_until(images + s0, n_frames, limit, my_traj);
+            };
+            advance(warm);
+                if (rc == YGZB_OK) ygzb_synchronize(my);
+            launch_base = my ? ygzb_launch_count(my) : 0;
+            eng->h2d_image_bytes = eng->h2d_other_bytes = eng->d2h_bytes = 0;
+            timed = true;
+            sync_point.arrive_and_wait();
+            if (t == 0) {
+                t_begin = std::chrono::steady_clock::now();
+                for (auto& v : g_stage_ns) v.store(0);
+                ygzb_timer_start(ctx);
+            }
+            advance(n_frames);
+            if (rc == YGZB_OK) ygzb_synchronize(my);
+            tot[t][0] += my ? ygzb_launch_count(my) - launch_base : 0;
+            tot[t][1] += eng->h2d_image_bytes; tot[t][2] += eng->h2d_other_bytes; tot[t][3] += eng->d2h_bytes;
+            sync_point.arrive_and_wait();
+            if (t == 0) {
+                double ms = 0;
+                if (ygzb_timer_stop(ctx, &ms) == YGZB_OK && device_ms) *device_ms = ms;
+                t_end = std::chrono::steady_clock::now();
+            }
+            for (int s = 0; s < ns; ++s) {
+                const EStream& st = eng->streams()[s];
+                int64_t* o = stats + 16 * (size_t)(s0 + eng->order()[s]);
+                for (int c = 0; c < 16; ++c) o[c] = 0;
+                o[0] = st.lost; o[1] = st.n_keyframes; o[2] = st.n_ba; o[3] = st.n_candidates; o[4] = st.n_projected; o[5] = st.n_inliers;
+                o[6] = st.ba_obs; o[7] = st.ba_pts; o[8] = st.ba_kfs; o[9] = st.ba_trials; o[10] = st.ba_iters; o[11] = (int64_t)st.ba_flops;
+            }
+        }   // (the engine releases its tracker and frame slots before the context goes)
+        if (own_ctx && my) ygzb_destroy(my);
+        rcs[t] = rc;
+    };
+    std::vector<std::thread> pool;
+    for (int t = 1; t < n_threads; ++t) pool.emplace_back(worker, t);
+    worker(0);
+    for (auto& th : pool) th.join();
+    *seconds = std::chrono::duration<double>(t_end - t_begin).count();
+    if (totals) {
+        for (int c = 0; c < 8; ++c) totals[c] = 0;
+        for (int t = 0; t < n_threads; ++t)
+            for (int c = 0; c < 4; ++c) totals[c] += tot[t][c];
+    }
+    if (getenv("YGZ_VO_TIMING")) {
+        const int timed = n_frames - warm;
+        fprintf(stderr, "[ygz_vo engine] %d streams on %d host threads, window %d, %d timed frames: %.3f ms per frame index; track rounds %.3f ms, "
+                        "key-frame rounds %.3f ms (host wall, summed over threads)\n",
+                n_streams, n_threads, window, timed, 1e3 * *seconds / timed, 1e-6 * g_stage_ns[kTSparse].load(), 1e-6 * g_stage_ns[kTLocalBA].load());
+    }
+    for (int rc : rcs)
+        if (rc != YGZB_OK) return rc;
+    return YGZB_OK;
+}
 
 }  // namespace
 
@@ -877,73 +1049,26 @@ int ygz_vo_run_stages(ygzb_ctx* ctx, int device, const ygzb_params* params, int 
 int ygz_vo_run(ygzb_ctx* ctx, int device, const ygzb_params* params, int n_threads, int n_streams, int n_frames,
                const uint8_t* const* images, const double* const* depth, int kf_min_frames, double kf_min_rot, double kf_min_trans,
                int warm, int window, double* traj, int64_t* stats, double* seconds, double* device_ms, int64_t* totals) {
-    if (!ctx || !params || n_streams < 1 || n_frames < 1 || !images || !depth || !traj || !stats || !seconds) return YGZB_ERR_INVALID;
-    n_threads = std::max(1, std::min(n_threads, n_streams));
-    warm = std::max(0, std::min(warm, n_frames - 1));
-    for (auto& v : g_stage_ns) v.store(0);
-    std::vector<int> rcs(n_threads, YGZB_OK);
-    std::vector<std::vector<long long>> tot(n_threads, std::vector<long long>(4, 0));
-    std::barrier sync_point(n_threads);
-    std::chrono::steady_clock::time_point t_begin, t_end;
-    auto worker = [&](int t) {
-        const int s0 = (int)((long)n_streams * t / n_threads), s1 = (int)((long)n_streams * (t + 1) / n_threads), ns = s1 - s0;
-        ygzb_ctx* my = ctx;
-        int rc = YGZB_OK;
-        if (t > 0) rc = ygzb_create(device, params, &my);
-        {
-            Engine eng(my, ns, window, Params{kf_min_frames, kf_min_rot, kf_min_trans});
-            if (rc == YGZB_OK) rc = eng.init(depth + s0);
-            double* my_traj = traj + (size_t)s0 * n_frames * 12;
-            if (rc == YGZB_OK) rc = eng.run_until(images + s0, n_frames, warm, my_traj);
-            if (rc == YGZB_OK) ygzb_synchronize(my);
-            tot[t][0] = -ygzb_launch_count(my);
-            eng.h2d_image_bytes = eng.h2d_other_bytes = eng.d2h_bytes = 0;
-            sync_point.arrive_and_wait();
-            if (t == 0) {
-                t_begin = std::chrono::steady_clock::now();
-                for (auto& v : g_stage_ns) v.store(0);
-                ygzb_timer_start(ctx);
-            }
-            if (rc == YGZB_OK) rc = eng.run_until(images + s0, n_frames, n_frames, my_traj);
-            if (rc == YGZB_OK) ygzb_synchronize(my);
-            tot[t][0] += ygzb_launch_count(my);
-            tot[t][1] = eng.h2d_image_bytes; tot[t][2] = eng.h2d_other_bytes; tot[t][3] = eng.d2h_bytes;
-            sync_point.arrive_and_wait();
-            if (t == 0) {
-                double ms = 0;
-                if (ygzb_timer_stop(ctx, &ms) == YGZB_OK && device_ms) *device_ms = ms;
-                t_end = std::chrono::steady_clock::now();
-            }
-            for (int s = 0; s < ns; ++s) {
-                const EStream& st = eng.streams()[s];
-                int64_t* o = stats + 16 * (size_t)(s0 + s);
-                for (int c = 0; c < 16; ++c) o[c] = 0;
-                o[0] = st.lost; o[1] = st.n_keyframes; o[2] = st.n_ba; o[3] = st.n_candidates; o[4] = st.n_projected; o[5] = st.n_inliers;
-                o[6] = st.ba_obs; o[7] = st.ba_pts; o[8] = st.ba_kfs; o[9] = st.ba_trials; o[10] = st.ba_iters; o[11] = (int64_t)st.ba_flops;
-            }
-        }   // (the engine releases its tracker and frame slots before the context goes)
-        if (t > 0 && my) ygzb_destroy(my);
-        rcs[t] = rc;
-    };
-    std::vector<std::thread> pool;
-    for (int t = 1; t < n_threads; ++t) pool.emplace_back(worker, t);
-    worker(0);
-    for (auto& th : pool) th.join();
-    *seconds = std::chrono::duration<double>(t_end - t_begin).count();
-    if (totals) {
-        for (int c = 0; c < 8; ++c) totals[c] = 0;
-        for (int t = 0; t < n_threads; ++t)
-            for (int c = 0; c < 4; ++c) totals[c] += tot[t][c];
-    }
-    if (getenv("YGZ_VO_TIMING")) {
-        const int timed = n_frames - warm;
-        fprintf(stderr, "[ygz_vo engine] %d streams on %d host threads, window %d, %d timed frames: %.3f ms per frame index; track rounds %.3f ms, "
-                        "key-frame rounds %.3f ms (host wall, summed over threads)\n",
-                n_streams, n_threads, window, timed, 1e3 * *seconds / timed, 1e-6 * g_stage_ns[kTSparse].load(), 1e-6 * g_stage_ns[kTLocalBA].load());
-    }
-    for (int rc : rcs)
-        if (rc != YGZB_OK) return rc;
-    return YGZB_OK;
+    return run_engine(ctx, device, params, n_threads, n_streams, n_frames, images, depth, kf_min_frames, kf_min_rot, kf_min_trans, warm, window,
+                      -1, nullptr, traj, stats, seconds, device_ms, totals);
+}
+
+// The device-resident engine with a hand-over of every stream to a new tracker: ygz_vo_run's arguments plus
+//   handoff : every host thread runs its streams to frame `handoff` (nothing in flight), exports each stream's key-frames
+//             (ygzb_tracker_export), destroys its tracker and frame pool, creates a fresh tracker on a new context of the
+//             same device with the stream order reversed (a stream changes its index), imports the maps
+//             (ygzb_tracker_import), takes the host-side bookkeeping over and runs on to the last frame;
+//   maps    : NULL, or n_streams records (one per stream, each sized for YGZB_TRACK_RING key-frames, images included) that
+//             receive the exported maps and are what the new tracker imports.
+// Results equal those of ygz_vo_run with warm = handoff, which splits the run at the same frame.  The hand-over's own
+// record copies are not counted in `totals`.
+int ygz_vo_run_handoff(ygzb_ctx* ctx, int device, const ygzb_params* params, int n_threads, int n_streams, int n_frames,
+                       const uint8_t* const* images, const double* const* depth, int kf_min_frames, double kf_min_rot, double kf_min_trans,
+                       int warm, int window, int handoff, ygzb_map_record* maps, double* traj, int64_t* stats, double* seconds,
+                       double* device_ms, int64_t* totals) {
+    if (handoff < 0) return YGZB_ERR_INVALID;
+    return run_engine(ctx, device, params, n_threads, n_streams, n_frames, images, depth, kf_min_frames, kf_min_rot, kf_min_trans, warm, window,
+                      handoff, maps, traj, stats, seconds, device_ms, totals);
 }
 
 }  // extern "C"

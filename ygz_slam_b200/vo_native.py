@@ -22,6 +22,10 @@ def _lib():
         _LIB.ygz_vo_run.restype = C.c_int
         _LIB.ygz_vo_run.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                     C.c_double, C.c_double, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        _LIB.ygz_vo_run_handoff.restype = C.c_int
+        _LIB.ygz_vo_run_handoff.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                            C.c_double, C.c_double, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p]
         _LIB.ygz_vo_run_stages.restype = C.c_int
         _LIB.ygz_vo_run_stages.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                            C.c_double, C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -40,14 +44,17 @@ def stack_pinned(frames):
 
 
 def run(ctx, frames, depths, kf_min_frames=10, kf_min_rot=0.1, kf_min_trans=0.1, warm=0, threads=1, device_frames=None,
-        return_device_ms=False, details=False, window=1, engine="resident"):
+        return_device_ms=False, details=False, window=1, engine="resident", handoff=None, return_maps=False):
     """frames: list of (n_frames, 480, 640) uint8 arrays or one stacked (S, n, 480, 640) array (ideally from stack_pinned);
     depths[s]: (480, 640) float64.  device_frames = (device pointer, S, n): the same stacked layout already resident in
     HBM (the "value" leg of bench.py) -- the driver then copies device-to-device.  The context must use the 3-level pyramid.
     threads > 1 splits the streams over that many host threads, each with its own context (CUDA stream) on the device.
     engine = "resident": the device-resident engine (ygzb_tracker_*; `window` = frames of one stream in flight per round);
     engine = "stages": the per-stage C-ABI path (one blocking call per stage and lock-step frame).
-    Returns (trajectory (S, n_frames, 3, 4), stats list of dicts, seconds of frames [warm, n_frames)[, device ms])."""
+    handoff = frame h (resident engine only): at h every stream's local map is exported, the tracker torn down and the
+    streams carried over to a fresh tracker on a new context in reverse order (ygz_vo_run_handoff); the results equal a
+    run with warm = h.  return_maps (with handoff): also return the maps exported at h, one capi.MapBuffers per stream.
+    Returns (trajectory (S, n_frames, 3, 4), stats list of dicts, seconds of frames [warm, n_frames)[, device ms][, maps])."""
     if device_frames is not None:
         base, S, n = device_frames
         ptrs = [base + s * n * 480 * 640 for s in range(S)]
@@ -67,11 +74,25 @@ def run(ctx, frames, depths, kf_min_frames=10, kf_min_rot=0.1, kf_min_trans=0.1,
         rc = _lib().ygz_vo_run_stages(ctx.h, ctx.device_index, C.byref(ctx.params), threads, S, n, C.cast(ip, C.c_void_p),
                                       C.cast(dp, C.c_void_p), kf_min_frames, kf_min_rot, kf_min_trans, warm, traj.ctypes.data,
                                       stats.ctypes.data, C.byref(sec), C.byref(dev_ms), totals.ctypes.data)
+    elif handoff is not None:
+        from .capi import TRACK_RING, MapBuffers, MapRecord
+        recs = (MapRecord * S)() if return_maps else None
+        maps = [MapBuffers(TRACK_RING, 640, 480, ctx.n_cells, rec=recs[s_]) for s_ in range(S)] if return_maps else None
+        rc = _lib().ygz_vo_run_handoff(ctx.h, ctx.device_index, C.byref(ctx.params), threads, S, n, C.cast(ip, C.c_void_p),
+                                       C.cast(dp, C.c_void_p), kf_min_frames, kf_min_rot, kf_min_trans, warm, int(window), int(handoff),
+                                       C.cast(recs, C.c_void_p) if return_maps else None, traj.ctypes.data, stats.ctypes.data,
+                                       C.byref(sec), C.byref(dev_ms), totals.ctypes.data)
     else:
         rc = _lib().ygz_vo_run(ctx.h, ctx.device_index, C.byref(ctx.params), threads, S, n, C.cast(ip, C.c_void_p), C.cast(dp, C.c_void_p),
                                kf_min_frames, kf_min_rot, kf_min_trans, warm, int(window), traj.ctypes.data, stats.ctypes.data,
                                C.byref(sec), C.byref(dev_ms), totals.ctypes.data)
     ctx.check(rc, "ygz_vo_run")
+    if handoff is not None and return_maps:
+        return _result(traj, stats, totals, sec, dev_ms, S, n, details, return_device_ms) + (maps,)
+    return _result(traj, stats, totals, sec, dev_ms, S, n, details, return_device_ms)
+
+
+def _result(traj, stats, totals, sec, dev_ms, S, n, details, return_device_ms):
     keys = ("lost", "keyframes", "ba", "candidates", "projected", "inliers", "ba_obs", "ba_pts", "ba_kfs", "ba_trials", "ba_iters", "ba_flops")
     out = (traj.reshape(S, n, 3, 4), [dict(zip(keys, map(int, row[:12]))) for row in stats], sec.value)
     if details:   # timed region only: device ms (CUDA events), kernel launches, bytes through the C ABI
