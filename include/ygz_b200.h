@@ -459,6 +459,28 @@ int ygzb_tracker_export(ygzb_tracker* t, int stream, int n_entries, const int32_
  * a level >= the pyramid depth or a missing image returns YGZB_ERR_INVALID with the tracker untouched.             */
 int ygzb_tracker_import(ygzb_tracker* t, int stream, const int32_t* entries, const int32_t* kf_slots, const ygzb_map_record* in);
 
+/* ---- parity / debug view of the last tracking batch (tests; not part of the tracking path, like ygzb_fast_debug) ------
+ * Synchronous: waits for the context's stream, then copies out the intermediate state of job `job` of the most recent
+ * ygzb_tracker_track batch (valid until the next ygzb_tracker_track).  The caller sizes every array for
+ * YGZB_MAP_OBS_PER_CELL * C entries (C = grid cells): the dense arrays are indexed by local key-frame k * C + feature, the
+ * compacted ones by the candidate order; entries of cand_px are only written for candidates, entries past n_projected
+ * of the compacted arrays are left over from earlier batches.                                                      */
+typedef struct {
+    double T_aligned[12];               /* T_cw after the sparse alignment and the key-frame pose (pose-only's start) */
+    double rel[YGZB_TRACK_RING][12];    /* T_aligned * T_cw(local key-frame k)^-1, first n_local rows               */
+    int32_t n_local, n_meas, aligned;
+    int32_t n_candidates;               /* FindCandidates: z > 0 and inside the border of 20 px                      */
+    int32_t n_projected;                /* FindDirectProjection succeeded: the compacted count                       */
+    int32_t n_inliers;                  /* pose-only's count (also when aligned == 0)                                */
+    uint8_t* cand_ok;                   /* [4 C] direct projection succeeded                                         */
+    double* cand_px;                    /* [4 C][2] its result                                                       */
+    int32_t* c_src;                     /* [4 C] dense index of compacted candidate i                                */
+    double* c_px;                       /* [4 C][2]                                                                  */
+    double* c_pw;                       /* [4 C][3] the map point                                                    */
+    uint8_t* inlier;                    /* [4 C] pose-only's inlier flag                                             */
+} ygzb_track_debug;
+int ygzb_tracker_debug_job(ygzb_tracker* t, int job, ygzb_track_debug* out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -43,7 +43,7 @@ EXPORTS = [
     "ygzb_project_align", "ygzb_sparse_align", "ygzb_default_ba_params", "ygzb_local_ba", "ygzb_local_ba_ceres", "ygzb_two_view_ba", "ygzb_pose_only",
     "ygzb_default_klt_params", "ygzb_klt",
     "ygzb_tracker_create", "ygzb_tracker_destroy", "ygzb_tracker_set_depth", "ygzb_tracker_upload", "ygzb_tracker_track", "ygzb_tracker_make_keyframes",
-    "ygzb_tracker_export", "ygzb_tracker_import",
+    "ygzb_tracker_export", "ygzb_tracker_import", "ygzb_tracker_debug_job",
 ]
 
 
@@ -735,8 +735,43 @@ class MapBuffers:
         return other
 
 
+class TrackJob(C.Structure):
+    _fields_ = [("stream", C.c_int32), ("cur_slot", C.c_int32), ("n_local", C.c_int32), ("entry", C.c_int32 * TRACK_RING), ("pad", C.c_int32)]
+
+
+class TrackResult(C.Structure):
+    _fields_ = [("T_cw", C.c_double * 12), ("n_meas", C.c_int32), ("aligned", C.c_int32), ("n_candidates", C.c_int32),
+                ("n_projected", C.c_int32), ("n_inliers", C.c_int32), ("pad", C.c_int32 * 3)]
+
+
+class KeyframeJob(C.Structure):
+    _fields_ = [("stream", C.c_int32), ("frame_slot", C.c_int32), ("kf_slot", C.c_int32), ("entry", C.c_int32), ("track_job", C.c_int32),
+                ("n_local", C.c_int32), ("local_entry", C.c_int32 * TRACK_RING), ("run_ba", C.c_int32), ("pad", C.c_int32), ("mp0", C.c_int64)]
+
+
+class KeyframeResult(C.Structure):
+    _fields_ = [("n_features", C.c_int32), ("ba_points", C.c_int32), ("ba_observations", C.c_int32), ("ba_iters", C.c_int32),
+                ("ba_trials", C.c_int32), ("pad", C.c_int32), ("chi2_initial", C.c_double), ("chi2_final", C.c_double),
+                ("T_cw", C.c_double * (12 * TRACK_RING))]
+
+
+_DEBUG_ARRAYS = ("cand_ok", "cand_px", "c_src", "c_px", "c_pw", "inlier")
+
+
+class TrackDebug(C.Structure):
+    _fields_ = ([("T_aligned", C.c_double * 12), ("rel", C.c_double * (12 * TRACK_RING)), ("n_local", C.c_int32), ("n_meas", C.c_int32),
+                 ("aligned", C.c_int32), ("n_candidates", C.c_int32), ("n_projected", C.c_int32), ("n_inliers", C.c_int32)]
+                + [(k, C.c_void_p) for k in _DEBUG_ARRAYS])
+
+
+def _record(s):
+    """dict of a ctypes record without its padding; array fields as float64 numpy arrays."""
+    return {k: (np.array(getattr(s, k)[:]) if isinstance(getattr(s, k), C.Array) else getattr(s, k)) for k, _ in s._fields_ if k != "pad"}
+
+
 class Tracker:
-    """The device-resident tracker (ygzb_tracker) on a frame pool; here for its map records (export / import)."""
+    """The device-resident tracker (ygzb_tracker) on a frame pool: its map records (export / import) and thin wrappers of the
+    tracking entry points, each followed by a synchronisation."""
 
     def __init__(self, frames: Frames, n_streams: int, max_jobs: int, K):
         self.frames, self.ctx, self.lib = frames, frames.ctx, frames.lib
@@ -745,6 +780,11 @@ class Tracker:
         self.lib.ygzb_tracker_destroy.restype = None
         self.lib.ygzb_tracker_export.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
         self.lib.ygzb_tracker_import.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        self.lib.ygzb_tracker_set_depth.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        self.lib.ygzb_tracker_upload.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
+        self.lib.ygzb_tracker_track.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+        self.lib.ygzb_tracker_make_keyframes.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        self.lib.ygzb_tracker_debug_job.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         Kd = np.ascontiguousarray(K, np.float64)
         h = C.c_void_p()
         self.ctx.check(self.lib.ygzb_tracker_create(frames.h, n_streams, max_jobs, _p(Kd), C.byref(h)), "ygzb_tracker_create")
@@ -777,6 +817,74 @@ class Tracker:
         kf_slots = np.ascontiguousarray(kf_slots, np.int32)
         self.ctx.check(self.lib.ygzb_tracker_import(self.h, int(stream), _p(entries), _p(kf_slots), C.byref(rec.rec)), "ygzb_tracker_import")
         self.ctx.synchronize()
+
+    def set_depth(self, stream: int, depth):
+        """Depth image (H, W) that initialises the map points of `stream`'s next key-frame."""
+        depth = np.ascontiguousarray(depth, np.float64)
+        self.ctx.check(self.lib.ygzb_tracker_set_depth(self.h, int(stream), _p(depth)), "ygzb_tracker_set_depth")
+        self.ctx.synchronize()
+
+    def upload(self, first: int, images):
+        """Grey frames (n, H, W) into slots [first, first + n)."""
+        images = np.ascontiguousarray(images, np.uint8)
+        if images.ndim == 2:
+            images = images[None]
+        self.ctx.check(self.lib.ygzb_tracker_upload(self.h, int(first), len(images), _p(images), C.c_size_t(images[0].size)),
+                       "ygzb_tracker_upload")
+        self.ctx.synchronize()
+
+    def track(self, jobs):
+        """jobs: (stream, cur_slot, ring entries of the local key-frames, oldest first).  One result dict per job: T_cw (3, 4),
+        n_meas, aligned, n_candidates, n_projected, n_inliers."""
+        arr = (TrackJob * len(jobs))()
+        for q, (stream, slot, entries) in zip(arr, jobs):
+            q.stream, q.cur_slot, q.n_local = int(stream), int(slot), len(entries)
+            q.entry[:len(entries)] = [int(e) for e in entries]
+        res = (TrackResult * len(jobs))()
+        self.ctx.check(self.lib.ygzb_tracker_track(self.h, len(jobs), arr, res), "ygzb_tracker_track")
+        self.ctx.synchronize()
+        out = [_record(r) for r in res]
+        for r in out:
+            r["T_cw"] = r["T_cw"].reshape(3, 4)
+        return out
+
+    def make_keyframes(self, jobs, ba: BAParams | None = None):
+        """jobs: dicts with the fields of ygzb_keyframe_job (local_entry: a list, oldest first; run_ba and mp0 default to 0).
+        One result dict per job: n_features, ba_points, ba_observations, ba_iters, ba_trials, chi2_initial, chi2_final and
+        T_cw (n_local, 3, 4)."""
+        arr = (KeyframeJob * len(jobs))()
+        for q, j in zip(arr, jobs):
+            q.stream, q.frame_slot, q.kf_slot, q.entry, q.track_job = (int(j[k]) for k in ("stream", "frame_slot", "kf_slot", "entry", "track_job"))
+            q.n_local = len(j["local_entry"])
+            q.local_entry[:q.n_local] = [int(e) for e in j["local_entry"]]
+            q.run_ba, q.mp0 = int(j.get("run_ba", 0)), int(j.get("mp0", 0))
+        if ba is None:
+            ba = BAParams()
+            self.lib.ygzb_default_ba_params(C.byref(ba))
+        res = (KeyframeResult * len(jobs))()
+        self.ctx.check(self.lib.ygzb_tracker_make_keyframes(self.h, len(jobs), arr, C.byref(ba), res), "ygzb_tracker_make_keyframes")
+        self.ctx.synchronize()
+        out = [_record(r) for r in res]
+        for r, q in zip(out, arr):
+            r["T_cw"] = r["T_cw"].reshape(TRACK_RING, 3, 4)[:q.n_local]
+        return out
+
+    def debug_job(self, job: int):
+        """ygzb_tracker_debug_job: the intermediate state of job `job` of the last track() batch.  The dense arrays (cand_ok,
+        cand_px) cover MAP_OBS_PER_CELL * cells entries; the compacted ones (c_src, c_px, c_pw, inlier) are cut to
+        n_projected; rel to n_local."""
+        cap = MAP_OBS_PER_CELL * self.ctx.n_cells
+        a = dict(cand_ok=np.zeros(cap, np.uint8), cand_px=np.zeros((cap, 2)), c_src=np.zeros(cap, np.int32), c_px=np.zeros((cap, 2)),
+                 c_pw=np.zeros((cap, 3)), inlier=np.zeros(cap, np.uint8))
+        d = TrackDebug()
+        for k in _DEBUG_ARRAYS:
+            setattr(d, k, a[k].ctypes.data)
+        self.ctx.check(self.lib.ygzb_tracker_debug_job(self.h, int(job), C.byref(d)), "ygzb_tracker_debug_job")
+        out = _record(d)
+        n = d.n_projected
+        out.update(T_aligned=out["T_aligned"].reshape(3, 4), rel=out["rel"].reshape(TRACK_RING, 3, 4)[:d.n_local], cand_ok=a["cand_ok"].astype(bool),
+                   cand_px=a["cand_px"], c_src=a["c_src"][:n], c_px=a["c_px"][:n], c_pw=a["c_pw"][:n], inlier=a["inlier"][:n].astype(bool))
+        return out
 
 
 Frames.tracker = lambda self, n_streams, max_jobs, K: Tracker(self, n_streams, max_jobs, K)

@@ -930,7 +930,10 @@ __global__ void track_compose_kernel(TrackStore st, TrackBatch b) {
     const double* Tk = st.kf_T + 12 * (size_t)(job.stream * st.R + job.entry[job.n_local - 1]);
     const SE3d Trel = se3_from_mat(b.T_cur + 12 * (size_t)j), Tref = se3_from_mat(Tk);
     se3_to_mat(se3_mul(Trel, Tref), b.T_cur + 12 * (size_t)j);
-    for (int c = 0; c < 12; ++c) b.T_ref[12 * (size_t)j + c] = Tk[c];
+    for (int c = 0; c < 12; ++c) {
+        b.T_ref[12 * (size_t)j + c] = Tk[c];
+        b.T_aligned[12 * (size_t)j + c] = b.T_cur[12 * (size_t)j + c];
+    }
 }
 
 // per job: Matcher::SparseImageAlignment's motion check (Matcher.cpp:482-488) and the current pose relative to every

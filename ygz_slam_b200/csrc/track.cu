@@ -548,7 +548,7 @@ int ygzb_tracker_create(ygzb_frames* f, int n_streams, int max_jobs, const doubl
             b.jobs = c.take<ygzb_track_job>(J);
             b.ref_slot = c.take<int32_t>(J); b.cur_slot = c.take<int32_t>(J); b.offsets = c.take<int32_t>(J + 1); b.in_off = c.take<int32_t>(J);
             b.n_feat = c.take<int32_t>(J); b.n_meas = c.take<int32_t>(J);
-            b.T_ref = c.take<double>(J * 12); b.T_cur = c.take<double>(J * 12);
+            b.T_ref = c.take<double>(J * 12); b.T_cur = c.take<double>(J * 12); b.T_aligned = c.take<double>(J * 12);
             b.ref_patch = c.take<float>(F * 16); b.gdx = c.take<float>(F * 16); b.gdy = c.take<float>(F * 16);
             b.frame_jac = c.take<double>(F * 12); b.visible = c.take<uint8_t>(F);
             b.sparse_ws = c.take<double>(sparse_align_ws_doubles((int)J));
@@ -913,6 +913,36 @@ int ygzb_tracker_import(ygzb_tracker* t, int stream, const int32_t* entries, con
     const size_t WH = (size_t)st.W * st.H;
     for (int k = 0; k < n && rc == YGZB_OK; ++k) rc = ygzb_frames_upload(t->f, kf_slots[k], 1, in->image + k * WH, 1, WH);
     if (rc == YGZB_OK) rc = check_cuda(ctx, cudaEventRecord(t->e_fill, ctx->stream), "cudaEventRecord");
+    return rc;
+}
+
+int ygzb_tracker_debug_job(ygzb_tracker* t, int job, ygzb_track_debug* out) {
+    if (!t || !out) return YGZB_ERR_INVALID;
+    ygzb_ctx* ctx = t->ctx;
+    if (job < 0 || job >= t->last_J) return set_error(ctx, YGZB_ERR_INVALID, "debug: job %d is not in the last batch (%d jobs)", job, t->last_J);
+    if (!out->cand_ok || !out->cand_px || !out->c_src || !out->c_px || !out->c_pw || !out->inlier)
+        return set_error(ctx, YGZB_ERR_INVALID, "debug: null array");
+    cudaSetDevice(ctx->device);
+    const TrackBatch& b = t->b;
+    const size_t j = (size_t)job, cap = (size_t)b.cap;
+    auto d2h = [&](void* dst, const void* src, size_t bytes) {
+        return check_cuda(ctx, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, ctx->stream), "D2H(track debug)");
+    };
+    int rc = d2h(out->T_aligned, b.T_aligned + 12 * j, 12 * sizeof(double));
+    if (rc == YGZB_OK) rc = d2h(out->rel, b.rel + 12 * kTrackMaxLocal * j, 12 * kTrackMaxLocal * sizeof(double));
+    if (rc == YGZB_OK) rc = d2h(&out->n_meas, b.n_meas + j, sizeof(int32_t));
+    if (rc == YGZB_OK) rc = d2h(&out->aligned, b.aligned + j, sizeof(int32_t));
+    if (rc == YGZB_OK) rc = d2h(&out->n_candidates, b.n_cand + j, sizeof(int32_t));
+    if (rc == YGZB_OK) rc = d2h(&out->n_projected, b.c_cnt + j, sizeof(int32_t));
+    if (rc == YGZB_OK) rc = d2h(&out->n_inliers, b.n_inl + j, sizeof(int32_t));
+    if (rc == YGZB_OK) rc = d2h(out->cand_ok, b.cand_ok + cap * j, cap);
+    if (rc == YGZB_OK) rc = d2h(out->cand_px, b.cand_px + 2 * cap * j, 2 * cap * sizeof(double));
+    if (rc == YGZB_OK) rc = d2h(out->c_src, b.c_src + cap * j, cap * sizeof(int32_t));
+    if (rc == YGZB_OK) rc = d2h(out->c_px, b.c_px + 2 * cap * j, 2 * cap * sizeof(double));
+    if (rc == YGZB_OK) rc = d2h(out->c_pw, b.c_pw + 3 * cap * j, 3 * cap * sizeof(double));
+    if (rc == YGZB_OK) rc = d2h(out->inlier, b.inlier + cap * j, cap);
+    if (rc == YGZB_OK) rc = check_cuda(ctx, cudaStreamSynchronize(ctx->stream), "cudaStreamSynchronize");
+    out->n_local = t->h_jobs[job].n_local;
     return rc;
 }
 

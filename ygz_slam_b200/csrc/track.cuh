@@ -38,6 +38,7 @@ struct TrackBatch {
     // sparse alignment (SparseImgAlign::run): problem j owns scratch features [offsets[j], offsets[j] + n_feat[j])
     int32_t *ref_slot, *cur_slot, *offsets, *in_off, *n_feat, *n_meas;
     double *T_ref, *T_cur;      // [J][12]; T_cur: reference pose in, aligned pose, then pose-only result
+    double* T_aligned;          // [J][12]  the aligned pose (pose-only's start), kept for ygzb_tracker_debug_job
     float *ref_patch, *gdx, *gdy;
     double* frame_jac;
     uint8_t* visible;
