@@ -298,7 +298,12 @@ int ygzb_local_ba(ygzb_ctx* ctx, int n_problems, const int32_t* kf_off, const in
  * choice of free / fixed poses the same entry point is ba::OptimizeCurrent (BA.cpp:91-186: the current frame free, its
  * map points free, their other observers fixed, HuberLoss(0.1)) and ba::OptimizeCurrentPointOnly (:266-322: every pose
  * fixed, no loss); a problem without free poses is a pure point refinement.
- * termination: 0 max_iters reached, 1 gradient, 2 parameter, 3 function tolerance, 4 trust region collapsed.    */
+ * termination: 0 max_iters reached, 1 gradient, 2 parameter, 3 function tolerance, 4 trust region collapsed.
+ * The statistics follow the solver restated in oracle/ba.cpp, which may differ from ceres::Solver::Summary: the gradient
+ * test runs before the iteration limit (max_iters = 0 evaluates once and reports 1 if the gradient is already below
+ * 1e-10; a step accepted on the last allowed trial is still followed by the gradient test), and after a gradient exit
+ * radius_final is the radius before the last step's update.  A landmark observed twice by one free pose returns
+ * YGZB_ERR_INVALID, as in ygzb_local_ba.                                                                        */
 typedef struct {
     int iters, successful_steps;
     double cost_initial, cost_final, radius_final;

@@ -372,7 +372,7 @@ __global__ void __launch_bounds__(kBAThreads) local_ba_kernel(const BAArgs a, Cl
         }
     };
     // Ceres twin: LM damping of one parameter from its Hessian diagonal and Jacobi scale
-    double radius = 1e4, decrease_factor = 2.0;
+    double radius = 1e4, radius_next = 1e4, decrease_factor = 2.0;
     auto damp = [&](double hkk, double sk) { return fmin(fmax(sk * sk * hkk, 1e-6), 1e32) / radius / (sk * sk); };
     int term = 0, n_success = 0;   // Ceres twin: termination code (see ygz_b200.h), accepted steps
 
@@ -380,7 +380,9 @@ __global__ void __launch_bounds__(kBAThreads) local_ba_kernel(const BAArgs a, Cl
     int iters = 0, trials_total = 0;
     double chi_first = 0, chi_last = 0, lambda = 0, ni = 2, rho = 0, currentChi = 0;
 
-    for (int iteration = 0; iteration < a.max_iters; ++iteration) {
+    // Ceres twin: the trial budget is checked after the linearisation, so that max_iters = 0 still reports the initial cost
+    // and gradient test, and a step accepted on the last trial is still followed by the gradient test at its point
+    for (int iteration = 0; kCeres || iteration < a.max_iters; ++iteration) {
         // ---- computeActiveErrors + buildSystem -------------------------------------------------------------------
         for (int i = ct; i < np * 36; i += CT) ws.Hpp[i] = 0.0;
         for (int i = ct; i < dimp; i += CT) ws.bp[i] = 0.0;
@@ -519,6 +521,7 @@ __global__ void __launch_bounds__(kBAThreads) local_ba_kernel(const BAArgs a, Cl
                     __syncthreads();
                 }
                 if (m0 <= 1e-10) term = 1;   // gradient tolerance
+                else radius = radius_next;   // the previous accepted step's radius update, taken once it did not converge
             } else if (iteration == 0) {  // computeLambdaInit = tau * max |diag H|
                 for (int i = 0; i < dimp; ++i) m0 = fmax(m0, fabs(__ldcg(&ws.Hpp[(i / 6) * 36 + (i % 6) * 7])));
                 lambda = a.tau * m0;
@@ -526,7 +529,7 @@ __global__ void __launch_bounds__(kBAThreads) local_ba_kernel(const BAArgs a, Cl
             }
             (void)m1;
         }
-        if (kCeres && term) break;
+        if (kCeres && (term || trials_total >= a.max_iters)) break;
 
         int qmax = 0;
         do {
@@ -781,11 +784,8 @@ __global__ void __launch_bounds__(kBAThreads) local_ba_kernel(const BAArgs a, Cl
                         if (fabs(cost - new_cost) <= 1e-6 * cost) {
                             term = 3;   // function tolerance
                         } else {
-                            {
                             const double t3 = 2.0 * relative_decrease - 1.0;
-                            radius = radius / fmax(1.0 / 3.0, 1.0 - t3 * t3 * t3);
-                        }
-                            radius = fmin(1e16, radius);
+                            radius_next = fmin(1e16, radius / fmax(1.0 / 3.0, 1.0 - t3 * t3 * t3));
                             decrease_factor = 2.0;
                         }
                     }
@@ -838,7 +838,7 @@ __global__ void __launch_bounds__(kBAThreads) local_ba_kernel(const BAArgs a, Cl
         ++iters;
         chi_last = currentChi;
         if constexpr (kCeres) {
-            if (term || trials_total >= a.max_iters) break;
+            if (term || (trials_total >= a.max_iters && rho < 0)) break;   // (accepted: linearise once more for the gradient test)
         } else {
             if (qmax == a.max_trials || rho == 0) break;
         }
@@ -861,7 +861,7 @@ __global__ void __launch_bounds__(kBAThreads) local_ba_kernel(const BAArgs a, Cl
         if (tid == 0) {
             double* st = a.stats + 8 * (size_t)prob;
             if constexpr (kCeres) {
-                st[0] = trials_total; st[1] = n_success; st[2] = 0.5 * chi_first; st[3] = 0.5 * chi_last; st[4] = radius; st[5] = term;
+                st[0] = trials_total; st[1] = n_success; st[2] = 0.5 * chi_first; st[3] = 0.5 * currentChi; st[4] = radius; st[5] = term;
             } else {
                 st[0] = iters; st[1] = trials_total; st[2] = chi_first; st[3] = chi_last; st[4] = lambda; st[5] = n_out_tot;
             }
@@ -1488,6 +1488,16 @@ int run_local_ba(ygzb_ctx* ctx, bool ceres, int n_problems, const int32_t* kf_of
                 ps_obs[pc[kf_off[p] + kf_idx[o]]++] = o;
             }
     }
+    // a landmark observed twice by one free pose is rejected, as ygzb_local_ba does: the pair lists below hold one entry per
+    // (landmark, free pose), so the Schur complement would miss the cross terms of the two observations
+    for (size_t p = 0; p < P; ++p)
+        for (int j = pt_off[p]; j < pt_off[p + 1]; ++j)
+            for (int q1 = lm_start[j]; q1 < lm_start[j + 1]; ++q1)
+                for (int q2 = q1 + 1; q2 < lm_start[j + 1]; ++q2) {
+                    const int k = kf_idx[lm_obs[q1]];
+                    if (kf_idx[lm_obs[q2]] == k && !fixed[kf_off[p] + k])
+                        return set_error(ctx, YGZB_ERR_INVALID, "problem %zu: a point is observed twice by one key-frame (not a SLAM graph)", p);
+                }
     // landmark-sharing observation pairs per (free pose f1 <= f2) block pair, as CSR: two passes (count, fill), no
     // per-problem allocations.  pair_start holds n_pairs + 1 entries per problem.
     std::vector<int32_t> free_of(NK, -1), nfree(P, 0);
@@ -1717,23 +1727,30 @@ int ygzb_local_ba_ceres(ygzb_ctx* ctx, int n_problems, const int32_t* kf_off, co
 // ba::TwoViewBACeres (reference src/Algorithm/BA.cpp:11-89) for a batch of two-view problems, on the Ceres-flavoured
 // cluster kernel: reference pose fixed (point-only blocks), current pose and points free, HuberLoss(0.1) on the blocks of the
 // non-inlier points, then the reference's inlier test (classification kernel below)
-__global__ void two_view_classify_kernel(int n, const int32_t* __restrict__ prob_of, const double* __restrict__ T_ref,
-                                         const double* __restrict__ poses, const double* __restrict__ pts, const double* __restrict__ px_ref,
-                                         const double* __restrict__ px_cur, float fx, float fy, float cx, float cy, uint8_t* __restrict__ inlier,
-                                         double* __restrict__ T_cur_out) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int p = prob_of[i];
-    const double* Tr = T_ref + 12 * (size_t)p;
+__device__ __forceinline__ void two_view_cur_pose(const double* __restrict__ poses, int p, double Tm[12]) {
     const double* pc = poses + 12 * (size_t)p + 6;   // [t; angle-axis] of the current frame
     double th;
     SE3d Tc;
     Tc.q = so3_exp(V3d{pc[3], pc[4], pc[5]}, &th);
     Tc.t = V3d{pc[0], pc[1], pc[2]};
-    double Tm[12];
     se3_to_mat(Tc, Tm);
-    if (i == 0 || prob_of[i - 1] != p)
-        for (int c = 0; c < 12; ++c) T_cur_out[12 * (size_t)p + c] = Tm[c];
+}
+
+// thread i < n_problems writes the pose of problem i (a pair without points included), thread i < n classifies point i
+__global__ void two_view_classify_kernel(int n, int n_problems, const int32_t* __restrict__ prob_of, const double* __restrict__ T_ref,
+                                         const double* __restrict__ poses, const double* __restrict__ pts, const double* __restrict__ px_ref,
+                                         const double* __restrict__ px_cur, float fx, float fy, float cx, float cy, uint8_t* __restrict__ inlier,
+                                         double* __restrict__ T_cur_out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    double Tm[12];
+    if (i < n_problems) {
+        two_view_cur_pose(poses, i, Tm);
+        for (int c = 0; c < 12; ++c) T_cur_out[12 * (size_t)i + c] = Tm[c];
+    }
+    if (i >= n) return;
+    const int p = prob_of[i];
+    const double* Tr = T_ref + 12 * (size_t)p;
+    two_view_cur_pose(poses, p, Tm);
     const double X = pts[3 * (size_t)i], Y = pts[3 * (size_t)i + 1], Z = pts[3 * (size_t)i + 2];
     const double x1 = Tr[0] * X + Tr[1] * Y + Tr[2] * Z + Tr[3], y1 = Tr[4] * X + Tr[5] * Y + Tr[6] * Z + Tr[7], z1 = Tr[8] * X + Tr[9] * Y + Tr[10] * Z + Tr[11];
     const double x2 = Tm[0] * X + Tm[1] * Y + Tm[2] * Z + Tm[3], y2 = Tm[4] * X + Tm[5] * Y + Tm[6] * Z + Tm[7], z2 = Tm[8] * X + Tm[9] * Y + Tm[10] * Z + Tm[11];
@@ -1820,9 +1837,11 @@ int ygzb_two_view_ba(ygzb_ctx* ctx, int n_problems, const int32_t* offsets, cons
         TRY(h2d(ctx, d_pts, X.data(), 3 * N));
         TRY(h2d(ctx, d_pr, px_ref, 2 * N));
         TRY(h2d(ctx, d_pc, px_cur, 2 * N));
-        if (N) {
-            two_view_classify_kernel<<<(unsigned)((N + 127) / 128), 128, 0, ctx->stream>>>((int)N, d_prob, d_Tref, d_poses, d_pts, d_pr, d_pc, ctx->prm.fx,
-                                                                                       ctx->prm.fy, ctx->prm.cx, ctx->prm.cy, d_in, d_Tcur);
+        {
+            const size_t threads = std::max(N, P);
+            two_view_classify_kernel<<<(unsigned)((threads + 127) / 128), 128, 0, ctx->stream>>>((int)N, (int)P, d_prob, d_Tref, d_poses, d_pts, d_pr,
+                                                                                                 d_pc, ctx->prm.fx, ctx->prm.fy, ctx->prm.cx,
+                                                                                                 ctx->prm.cy, d_in, d_Tcur);
             YGZB_LAUNCHED(ctx);
             TRY(d2h(ctx, inlier, d_in, N));
             TRY(d2h(ctx, T_cw_cur, d_Tcur, 12 * P));
