@@ -112,5 +112,5 @@ def test_gpu_depth_from_triangulation(ctx3, oracle):
         sel = pose_of == k
         w1, w2, wok = oracle.depth_from_triangulation(Ts[k], f_ref[sel], f_cur[sel])
         assert np.array_equal(ok[sel], wok)
-        assert np.abs(d1[sel] - w1).max() < 1e-12 and np.abs(d2[sel] - w2).max() < 1e-12
+        assert np.array_equal(d1[sel], w1) and np.array_equal(d2[sel], w2)
     assert ok[pose_of == 0].all() and not ok[pose_of == 1].any()

@@ -21,7 +21,8 @@ NVCC_FLAGS = [
 
 
 # per-file extra flags: the f32/f64 parity kernels must not contract a*b+c into FMA
-PER_FILE_FLAGS = {"align.cu": ["-fmad=false"], "track.cu": ["-fmad=false"], "initializer.cu": ["-fmad=false"]}
+PER_FILE_FLAGS = {"align.cu": ["-fmad=false"], "track.cu": ["-fmad=false"], "initializer.cu": ["-fmad=false"],
+                  "triangulate.cu": ["-fmad=false"]}
 
 
 def nvcc() -> str:

@@ -9,7 +9,10 @@
 // DBoW3 feature vector's index lists -- so the reference's tie rule (a later candidate of EQUAL distance replaces the
 // earlier one, `dist > bestDist` skips) is kept and the result is index-exact.  The descriptors of key-frame 2 are staged
 // through shared memory in chunks like the brute-force matcher (match.cu); the distance is 8 x POPC per candidate of the
-// same node only.  f32 steps of the epipolar test use explicit round-to-nearest intrinsics (no FMA contraction).
+// same node only.  Compiled with -fmad=false: the double sums behind the epipolar line and its distance, and the normal
+// matrix, determinant and right-hand side of DepthFromTriangulation, are rounded after every operation as in the oracle.
+// A fused multiply-add changes them in their last bits, which moves the `dsqr < th` and `det < det_th` decisions on
+// boundary cases and the depths themselves.  The f32 steps also use explicit round-to-nearest intrinsics.
 #include <exception>
 #include <vector>
 
