@@ -43,7 +43,7 @@ EXPORTS = [
     "ygzb_project_align", "ygzb_sparse_align", "ygzb_default_ba_params", "ygzb_local_ba", "ygzb_local_ba_ceres", "ygzb_two_view_ba", "ygzb_pose_only",
     "ygzb_default_klt_params", "ygzb_klt",
     "ygzb_tracker_create", "ygzb_tracker_destroy", "ygzb_tracker_set_depth", "ygzb_tracker_upload", "ygzb_tracker_track", "ygzb_tracker_make_keyframes",
-    "ygzb_tracker_export", "ygzb_tracker_import", "ygzb_tracker_debug_job",
+    "ygzb_tracker_export", "ygzb_tracker_import", "ygzb_tracker_debug_job", "ygzb_tracker_set_reference_mode", "ygzb_tracker_debug_reference",
 ]
 
 
@@ -785,6 +785,8 @@ class Tracker:
         self.lib.ygzb_tracker_track.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         self.lib.ygzb_tracker_make_keyframes.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         self.lib.ygzb_tracker_debug_job.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        self.lib.ygzb_tracker_set_reference_mode.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        self.lib.ygzb_tracker_debug_reference.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         Kd = np.ascontiguousarray(K, np.float64)
         h = C.c_void_p()
         self.ctx.check(self.lib.ygzb_tracker_create(frames.h, n_streams, max_jobs, _p(Kd), C.byref(h)), "ygzb_tracker_create")
@@ -885,6 +887,27 @@ class Tracker:
         out.update(T_aligned=out["T_aligned"].reshape(3, 4), rel=out["rel"].reshape(TRACK_RING, 3, 4)[:d.n_local], cand_ok=a["cand_ok"].astype(bool),
                    cand_px=a["cand_px"], c_src=a["c_src"][:n], c_px=a["c_px"][:n], c_pw=a["c_pw"][:n], inlier=a["inlier"][:n].astype(bool))
         return out
+
+    def set_reference_mode(self, mode: str, ref_slots=None):
+        """ygzb_tracker_set_reference_mode: "keyframe" or "previous" (ref_slots: one frame slot per stream)."""
+        slots = None if ref_slots is None else np.ascontiguousarray(ref_slots, np.int32)
+        self.ctx.check(self.lib.ygzb_tracker_set_reference_mode(self.h, {"keyframe": 0, "previous": 1}.get(mode, -1),
+                                                                 None if slots is None else _p(slots)), "ygzb_tracker_set_reference_mode")
+
+    def debug_reference(self, stream: int):
+        """ygzb_tracker_debug_reference: the stream's current reference -- dict(slot, T_cw (3, 4), px (n, 2), depth (n,))."""
+        cap = (TRACK_RING + 1) * self.ctx.n_cells
+        px, depth = np.zeros((cap, 2)), np.zeros(cap)
+        r = TrackReference()
+        r.capacity = cap
+        r.px, r.depth = px.ctypes.data, depth.ctypes.data
+        self.ctx.check(self.lib.ygzb_tracker_debug_reference(self.h, int(stream), C.byref(r)), "ygzb_tracker_debug_reference")
+        return dict(slot=r.slot, T_cw=np.array(r.T_cw).reshape(3, 4), px=px[:r.n].copy(), depth=depth[:r.n].copy())
+
+
+class TrackReference(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("n", C.c_int32), ("capacity", C.c_int32), ("pad", C.c_int32), ("T_cw", C.c_double * 12),
+                ("px", C.c_void_p), ("depth", C.c_void_p)]
 
 
 Frames.tracker = lambda self, n_streams, max_jobs, K: Tracker(self, n_streams, max_jobs, K)

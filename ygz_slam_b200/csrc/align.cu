@@ -906,9 +906,22 @@ __global__ void track_prep_kernel(TrackStore st, TrackBatch b) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= b.J) return;
     const ygzb_track_job job = b.jobs[j];
+    b.cur_slot[j] = job.cur_slot;
+    b.n_cand[j] = 0;
+    b.c_off[j] = j * b.cap;
+    if (j == 0) b.c_off[b.J] = b.J * b.cap;
+    if (b.prev) {   // the stream's current reference (previous frame or key-frame): absolute start pose, as VisualOdometry.cpp:66
+        const int r = 2 * job.stream + st.ref_cur[job.stream];
+        b.ref_slot[j] = b.job_ref_slot[j];
+        b.offsets[j] = j * st.ref_cap;
+        if (j == 0) b.offsets[b.J] = b.J * st.ref_cap;
+        b.in_off[j] = r * st.ref_cap;
+        b.n_feat[j] = st.ref_n[r];
+        for (int c = 0; c < 12; ++c) b.T_ref[12 * (size_t)j + c] = b.T_cur[12 * (size_t)j + c] = st.ref_T[12 * (size_t)r + c];
+        return;
+    }
     const int e = job.stream * st.R + job.entry[job.n_local - 1];
     b.ref_slot[j] = st.kf_slot[e];
-    b.cur_slot[j] = job.cur_slot;
     b.offsets[j] = j * st.cells;
     if (j == 0) b.offsets[b.J] = b.J * st.cells;
     b.in_off[j] = e * st.cells;
@@ -917,9 +930,6 @@ __global__ void track_prep_kernel(TrackStore st, TrackBatch b) {
     // identity in the key-frame's frame); track_compose_kernel applies the key-frame's pose afterwards, so this part of the
     // chain does not depend on a local BA that may still be refining that pose
     for (int c = 0; c < 12; ++c) b.T_ref[12 * (size_t)j + c] = b.T_cur[12 * (size_t)j + c] = (c == 0 || c == 5 || c == 10) ? 1.0 : 0.0;
-    b.n_cand[j] = 0;
-    b.c_off[j] = j * b.cap;
-    if (j == 0) b.c_off[b.J] = b.J * b.cap;
 }
 
 // per job: T_cw of the aligned frame = (pose relative to the reference key-frame) * (pose of the key-frame, after its BA)
@@ -927,6 +937,10 @@ __global__ void track_compose_kernel(TrackStore st, TrackBatch b) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= b.J) return;
     const ygzb_track_job job = b.jobs[j];
+    if (b.prev) {   // the alignment ran in world coordinates from the reference's pose: T_ref is that pose already
+        for (int c = 0; c < 12; ++c) b.T_aligned[12 * (size_t)j + c] = b.T_cur[12 * (size_t)j + c];
+        return;
+    }
     const double* Tk = st.kf_T + 12 * (size_t)(job.stream * st.R + job.entry[job.n_local - 1]);
     const SE3d Trel = se3_from_mat(b.T_cur + 12 * (size_t)j), Tref = se3_from_mat(Tk);
     se3_to_mat(se3_mul(Trel, Tref), b.T_cur + 12 * (size_t)j);
@@ -1206,8 +1220,9 @@ int launch_track_chain_front(ygzb_frames* f, const TrackStore& st, const TrackBa
         YGZB_LAUNCHED(ctx);
     }
     const bool gen1 = sparse_align_gen1();
+    const int feat_cap = b.prev ? st.ref_cap : st.cells;   // scratch features per problem (the tracker sizes the scratch)
     if (gen1)   // (the second-generation kernel keeps its patches in shared memory)
-        YGZB_CUDA(ctx, cudaMemsetAsync(b.ref_patch, 0, (size_t)b.J * st.cells * 16 * sizeof(float), ctx->stream));
+        YGZB_CUDA(ctx, cudaMemsetAsync(b.ref_patch, 0, (size_t)b.J * feat_cap * 16 * sizeof(float), ctx->stream));
     SparseArgs a;
     a.pyr = f->d_pyr;
     a.slot_stride = ctx->slot_stride;
@@ -1218,9 +1233,9 @@ int launch_track_chain_front(ygzb_frames* f, const TrackStore& st, const TrackBa
     a.offsets = b.offsets;
     a.in_off = b.in_off;
     a.n_feat = b.n_feat;
-    a.px = st.kf_px;
-    a.depth = st.kf_depth;
-    a.has_mp = nullptr;            // every feature of a key-frame has its map point (depth-initialised)
+    a.px = b.prev ? st.ref_px : st.kf_px;
+    a.depth = b.prev ? st.ref_depth : st.kf_depth;
+    a.has_mp = nullptr;            // every feature of a key-frame or a reference frame has its map point
     a.T_ref = b.T_ref;
     a.T_cur = b.T_cur;
     a.max_level = 2;               // Matcher's SparseImgAlign(2, 0, 30, GaussNewton) (Matcher.cpp:18)
@@ -1238,7 +1253,7 @@ int launch_track_chain_front(ygzb_frames* f, const TrackStore& st, const TrackBa
     a.feat_scratch = nullptr;
     a.feat_stride = 0;
     if (gen1) return launch_sparse_align1(ctx, a, b.J, sparse_cluster);
-    return launch_sparse_align2(ctx, a, b.J, sparse_cluster, b.sa2_scratch, sparse_align2_scratch_bytes(1, st.cells));
+    return launch_sparse_align2(ctx, a, b.J, sparse_cluster, b.sa2_scratch, sparse_align2_scratch_bytes(1, feat_cap));
 }
 
 // part 2 (main stream, behind a local BA in flight): key-frame pose applied -> motion check / relative poses -> candidate

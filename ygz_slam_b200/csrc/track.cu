@@ -52,6 +52,15 @@ struct ygzb_tracker {
     int cluster;           // CTAs per tracking problem (sparse alignment, pose-only): fixed, so that a frame's result does not
                            // depend on how many other frames share its batch (the summation order follows the cluster size)
     void* d_xfer;          // staging of a map record (ygzb_tracker_export / _import), allocated on first use
+    // previous-frame reference (ygzb_tracker_set_reference_mode)
+    int ref_mode;
+    bool kf_inserted;              // a key-frame insertion has been enqueued: the mode is fixed from then on
+    std::vector<int32_t> ref_slots; // the caller's reference slot of every stream (pyramid of the last tracked frame)
+    std::vector<int32_t> cur_ref;   // slot the stream's reference pyramid is in now (ref_slots[s] or a key-frame's slot), -1: none
+    std::vector<int32_t> pos_of;    // caller's job index -> position in the wave-ordered batch
+    void* d_ref;                   // reference store + the wave scratch of the sparse alignment (ref_cap features per problem)
+    int32_t* h_aux;                // pinned [2][max_jobs]: job_ref_slot, orig
+    int32_t* d_aux;
 };
 
 namespace {
@@ -79,7 +88,7 @@ __global__ void track_finish_kernel(TrackBatch b) {
     r.n_projected = b.c_cnt[j];
     r.n_inliers = b.aligned[j] ? b.n_inl[j] : 0;
     r.pad[0] = r.pad[1] = r.pad[2] = 0;
-    b.results[j] = r;
+    b.results[b.orig ? b.orig[j] : j] = r;
 }
 
 // inclusive scan of one int per thread over a 1024-thread CTA: shuffles inside the warps, the 32 warp totals scanned by warp 0
@@ -175,6 +184,86 @@ __global__ void __launch_bounds__(1024) kf_fill_kernel(TrackStore st, TrackBatch
         total = s_carry;
     }
     if (tid == 0) st.kf_nobs[e] = total;
+}
+
+// previous-frame reference of job blockIdx.x after its pose-only refinement, into the stream's other buffer: its pose and its
+// projected candidates in candidate order; an inlier at the depth of its map point under that pose (OptimizeCurrent,
+// LocalMapping.cpp:130-134), an outlier at the depth pose-only left it (its last inlier round's, or -1).  Outliers stay:
+// SparseImgAlign tests only _mappoint and the border, not _bad.
+__global__ void __launch_bounds__(256) track_ref_write_kernel(TrackStore st, TrackBatch b) {
+    __shared__ double s_T[12];
+    const int j = blockIdx.x, tid = threadIdx.x;
+    const int s = b.jobs[j].stream, nb = 1 - st.ref_cur[s], r = 2 * s + nb;
+    const int n = b.aligned[j] ? b.c_cnt[j] : 0;
+    if (tid < 12) s_T[tid] = b.T_cur[12 * (size_t)j + tid];
+    __syncthreads();
+    for (int i = tid; i < n; i += blockDim.x) {
+        const size_t at = (size_t)j * b.cap + i, o = (size_t)r * st.ref_cap + i;
+        const double* X = b.c_pw + 3 * at;
+        st.ref_px[2 * o] = b.c_px[2 * at];
+        st.ref_px[2 * o + 1] = b.c_px[2 * at + 1];
+        st.ref_depth[o] = b.inlier[at] ? s_T[8] * X[0] + s_T[9] * X[1] + s_T[10] * X[2] + s_T[11] : b.c_depth[at];
+    }
+    if (tid < 12) st.ref_T[12 * (size_t)r + tid] = s_T[tid];
+    __syncthreads();
+    if (tid == 0) {
+        st.ref_n[r] = n;
+        st.ref_cur[s] = nb;
+    }
+}
+
+// previous-frame reference after key-frame job blockIdx.x (SetKeyframe + LocalBA, VisualOdometry.cpp:182-218,
+// LocalMapping.cpp:192-206), over the stream's current buffer: the key-frame's pose after the BA write-back; its tracked
+// features, inliers at the depth of their map point after the BA, outliers unchanged; then its new features with their
+// depth-image depth
+__global__ void __launch_bounds__(256) kf_ref_kernel(TrackStore st, TrackBatch b, const ygzb_keyframe_job* __restrict__ jobs) {
+    __shared__ double s_T[12];
+    const ygzb_keyframe_job kj = jobs[blockIdx.x];
+    const int tid = threadIdx.x, e = kj.stream * st.R + kj.entry, r = 2 * kj.stream + st.ref_cur[kj.stream];
+    if (tid < 12) s_T[tid] = st.kf_T[12 * (size_t)e + tid];
+    __syncthreads();
+    int n_tr = 0;
+    if (kj.track_job >= 0) {
+        const int tj = kj.track_job;
+        const ygzb_track_job job = b.jobs[tj];
+        n_tr = b.aligned[tj] ? b.c_cnt[tj] : 0;
+        for (int i = tid; i < n_tr; i += blockDim.x) {
+            const size_t at = (size_t)tj * b.cap + i, o = (size_t)r * st.ref_cap + i;
+            st.ref_px[2 * o] = b.c_px[2 * at];
+            st.ref_px[2 * o + 1] = b.c_px[2 * at + 1];
+            double d = b.c_depth[at];
+            if (b.inlier[at]) {
+                const int c = b.c_src[at], k = c / st.cells, f = c - k * st.cells;
+                const double* X = st.kf_pw + 3 * ((size_t)(job.stream * st.R + job.entry[k]) * st.cells + f);
+                d = s_T[8] * X[0] + s_T[9] * X[1] + s_T[10] * X[2] + s_T[11];
+            }
+            st.ref_depth[o] = d;
+        }
+    }
+    const int n_new = st.kf_n[e];
+    for (int g = tid; g < n_new; g += blockDim.x) {
+        const size_t fe = (size_t)e * st.cells + g, o = (size_t)r * st.ref_cap + n_tr + g;
+        st.ref_px[2 * o] = st.kf_px[2 * fe];
+        st.ref_px[2 * o + 1] = st.kf_px[2 * fe + 1];
+        st.ref_depth[o] = st.kf_depth[fe];
+    }
+    if (tid < 12) st.ref_T[12 * (size_t)r + tid] = s_T[tid];
+    if (tid == 0) st.ref_n[r] = n_tr + n_new;
+}
+
+// the batch arrays of wave jobs [j0, j0 + J): every per-job array shifted to job j0; the workspaces of the solvers and the
+// sparse alignment's per-feature scratch (wave-local, sized for the stream count) are not
+TrackBatch wave_batch(const TrackBatch& b, int j0, int J) {
+    TrackBatch w = b;
+    const size_t c = (size_t)j0 * b.cap;
+    w.J = J;
+    w.jobs += j0; w.ref_slot += j0; w.cur_slot += j0; w.offsets += j0; w.in_off += j0; w.n_feat += j0; w.n_meas += j0;
+    w.T_ref += 12 * (size_t)j0; w.T_cur += 12 * (size_t)j0; w.T_aligned += 12 * (size_t)j0;
+    w.aligned += j0; w.rel += 12 * (size_t)kTrackMaxLocal * j0;
+    w.cand_ok += c; w.cand_px += 2 * c; w.n_cand += j0; w.c_cnt += j0; w.c_off += j0; w.c_src += c;
+    w.c_pw += 3 * c; w.c_px += 2 * c; w.c_depth += c; w.inlier += c; w.enable += c; w.n_inl += j0;
+    w.results += j0; w.job_ref_slot += j0; w.orig += j0;
+    return w;
 }
 
 struct BABuild {   // device arrays of the batch of local-BA problems (capacity based: problem p owns fixed ranges)
@@ -497,6 +586,97 @@ int check_entries(ygzb_tracker* t, int n, const int32_t* entries, const int32_t*
 
 }  // namespace
 
+size_t ref_store_bytes(const TrackStore& st) {
+    const size_t R2 = 2 * (size_t)st.S, cap = st.ref_cap;
+    Carver c(nullptr);
+    c.take<double>(R2 * cap * 2); c.take<double>(R2 * cap); c.take<int32_t>(R2); c.take<double>(R2 * 12); c.take<int32_t>(st.S);
+    return (c.bytes() + 255) & ~(size_t)255;
+}
+
+void wave_scratch(Carver& c, TrackBatch& b, size_t F, int S, int ref_cap) {
+    b.ref_patch = c.take<float>(F * 16); b.gdx = c.take<float>(F * 16); b.gdy = c.take<float>(F * 16);
+    b.frame_jac = c.take<double>(F * 12); b.visible = c.take<uint8_t>(F);
+    b.sa2_scratch = c.take<double>(sparse_align2_scratch_bytes(S, ref_cap) / 8 + 1);
+}
+
+// ygzb_tracker_track in YGZB_TRACK_REF_PREVIOUS mode.  A stream's jobs are tracked in batch order, each against the one
+// before it (its first against the stream's reference).  The batch runs in waves (wave w = the w-th job of every stream),
+// each wave the whole chain -- sparse alignment, candidates, direct projection, pose-only -- followed by the kernel that
+// makes every job the next reference of its stream; all on the context's stream, without a host synchronisation.  Behind
+// the last wave the last job's pyramid is copied into the stream's reference slot.  The alignment needs the refined pose
+// and depths of a key-frame, so nothing overlaps a local BA here.
+int track_previous(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, ygzb_track_result* results) {
+    ygzb_ctx* ctx = t->ctx;
+    const int S = t->st.S;
+    std::vector<int> wave_of(n_jobs), count(S, 0), last(S, -1);
+    int n_waves = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const int s = jobs[j].stream;
+        if (t->cur_ref[s] < 0) return set_error(ctx, YGZB_ERR_INVALID, "track job %d: stream %d has no reference frame yet", j, s);
+        wave_of[j] = count[s]++;
+        n_waves = std::max(n_waves, wave_of[j] + 1);
+    }
+    YGZB_CUDA(ctx, cudaEventSynchronize(t->staged));
+    std::vector<int> wave_start(n_waves + 1, 0);
+    for (int j = 0; j < n_jobs; ++j) wave_start[wave_of[j] + 1] += 1;
+    for (int w = 0; w < n_waves; ++w) wave_start[w + 1] += wave_start[w];
+    std::vector<int> fill(wave_start.begin(), wave_start.end() - 1);
+    t->pos_of.assign(n_jobs, 0);
+    int32_t* h_ref_slot = t->h_aux;
+    int32_t* h_orig = t->h_aux + t->max_jobs;
+    for (int j = 0; j < n_jobs; ++j) {   // wave-major order, batch order inside a wave
+        const int p = fill[wave_of[j]]++, s = jobs[j].stream;
+        t->pos_of[j] = p;
+        t->h_jobs[p] = jobs[j];
+        h_orig[p] = j;
+        h_ref_slot[p] = last[s] < 0 ? t->cur_ref[s] : jobs[last[s]].cur_slot;
+        last[s] = j;
+    }
+    TrackBatch b = t->b;
+    b.J = n_jobs;
+    b.prev = 1;
+    b.job_ref_slot = t->d_aux;
+    b.orig = t->d_aux + t->max_jobs;
+    {   // the sparse alignment's per-feature scratch, for ref_cap features per problem (a wave has at most one job per stream)
+        Carver c(static_cast<uint8_t*>(t->d_ref) + ref_store_bytes(t->st));
+        wave_scratch(c, b, (size_t)S * t->st.ref_cap, S, t->st.ref_cap);
+    }
+    t->last_J = n_jobs;
+    const int cl = t->cluster;
+    // uploads ran on the front stream; a key-frame insertion (and its BA) is on this stream already
+    YGZB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, t->e_up, 0));
+    YGZB_CUDA(ctx, cudaMemcpyAsync(const_cast<ygzb_track_job*>(t->b.jobs), t->h_jobs, sizeof(ygzb_track_job) * (size_t)n_jobs,
+                                   cudaMemcpyHostToDevice, ctx->stream));
+    YGZB_CUDA(ctx, cudaMemcpyAsync(t->d_aux, t->h_aux, sizeof(int32_t) * 2 * (size_t)t->max_jobs, cudaMemcpyHostToDevice, ctx->stream));
+    YGZB_CUDA(ctx, cudaEventRecord(t->staged, ctx->stream));
+    for (int w = 0; w < n_waves; ++w) {
+        TrackBatch wb = wave_batch(b, wave_start[w], wave_start[w + 1] - wave_start[w]);
+        int rc = launch_track_chain_front(t->f, t->st, wb, cl);
+        if (rc == YGZB_OK) rc = launch_track_chain_mid(t->f, t->st, wb);
+        if (rc == YGZB_OK)
+            rc = launch_pose_only_dev(ctx, wb.J, wb.c_off, wb.c_cnt, wb.c_pw, wb.c_px, wb.T_cur, wb.inlier, wb.c_depth, wb.n_inl, wb.enable,
+                                      wb.pose_ws, cl, wb.cap);
+        if (rc != YGZB_OK) return rc;
+        ProfScope ps(ctx, kStageOther);
+        track_ref_write_kernel<<<(unsigned)wb.J, 256, 0, ctx->stream>>>(t->st, wb);
+        YGZB_LAUNCHED(ctx);
+    }
+    {
+        ProfScope ps(ctx, kStageOther);
+        track_finish_kernel<<<(n_jobs + 63) / 64, 64, 0, ctx->stream>>>(b);
+        YGZB_LAUNCHED(ctx);
+    }
+    for (int s = 0; s < S; ++s)
+        if (last[s] >= 0) {
+            const int rc = ygzb_frames_copy(t->f, jobs[last[s]].cur_slot, t->ref_slots[s]);
+            if (rc != YGZB_OK) return rc;
+            t->cur_ref[s] = t->ref_slots[s];
+        }
+    YGZB_CUDA(ctx, cudaMemcpyAsync(results, b.results, sizeof(ygzb_track_result) * (size_t)n_jobs, cudaMemcpyDeviceToHost, ctx->stream));
+    YGZB_CUDA(ctx, cudaEventRecord(t->e_main, ctx->stream));
+    return YGZB_OK;
+}
+
 extern "C" {
 
 int ygzb_tracker_create(ygzb_frames* f, int n_streams, int max_jobs, const double K[4], ygzb_tracker** out) {
@@ -507,7 +687,6 @@ int ygzb_tracker_create(ygzb_frames* f, int n_streams, int max_jobs, const doubl
     if (ctx->geo.n_cells > 4096) return set_error(ctx, YGZB_ERR_CAPACITY, "tracker: %d grid cells (the BA assembly handles up to 4096)", ctx->geo.n_cells);
     ygzb_tracker* t = new (std::nothrow) ygzb_tracker();
     if (!t) return YGZB_ERR_INVALID;
-    memset(t, 0, sizeof(*t));
     t->f = f;
     t->ctx = ctx;
     t->max_jobs = max_jobs;
@@ -618,6 +797,9 @@ void ygzb_tracker_destroy(ygzb_tracker* t) {
     if (t->d_kfres) cudaFree(t->d_kfres);
     if (t->d_ba) cudaFree(t->d_ba);
     if (t->d_xfer) cudaFree(t->d_xfer);
+    if (t->d_ref) cudaFree(t->d_ref);
+    if (t->h_aux) cudaFreeHost(t->h_aux);
+    if (t->d_aux) cudaFree(t->d_aux);
     if (t->staged) cudaEventDestroy(t->staged);
     if (t->front) {
         cudaStreamSynchronize(t->front);
@@ -626,6 +808,72 @@ void ygzb_tracker_destroy(ygzb_tracker* t) {
     for (cudaEvent_t e : {t->e_fill, t->e_front, t->e_main, t->e_up})
         if (e) cudaEventDestroy(e);
     delete t;
+}
+
+int ygzb_tracker_set_reference_mode(ygzb_tracker* t, int mode, const int32_t* ref_slots) {
+    if (!t) return YGZB_ERR_INVALID;
+    ygzb_ctx* ctx = t->ctx;
+    if (mode != YGZB_TRACK_REF_KEYFRAME && mode != YGZB_TRACK_REF_PREVIOUS) return set_error(ctx, YGZB_ERR_INVALID, "reference mode %d", mode);
+    if (t->kf_inserted) return set_error(ctx, YGZB_ERR_INVALID, "the reference mode is fixed once a key-frame has been inserted");
+    const int S = t->st.S;
+    if (mode == YGZB_TRACK_REF_PREVIOUS) {
+        if (!ref_slots) return set_error(ctx, YGZB_ERR_INVALID, "previous-frame reference: no reference slots");
+        for (int s = 0; s < S; ++s) {
+            if (ref_slots[s] < 0 || ref_slots[s] >= t->f->capacity) return set_error(ctx, YGZB_ERR_INVALID, "reference slot of stream %d out of range", s);
+            for (int q = 0; q < s; ++q)
+                if (ref_slots[q] == ref_slots[s]) return set_error(ctx, YGZB_ERR_INVALID, "streams %d and %d share reference slot %d", q, s, ref_slots[s]);
+        }
+    }
+    cudaSetDevice(ctx->device);
+    if (mode == YGZB_TRACK_REF_PREVIOUS && !t->d_ref) {
+        TrackStore st = t->st;
+        st.ref_cap = (kTrackMaxLocal + 1) * st.cells;
+        Carver sz(nullptr);
+        TrackBatch tmp{};
+        wave_scratch(sz, tmp, (size_t)S * st.ref_cap, S, st.ref_cap);
+        const size_t head = ref_store_bytes(st);
+        int rc = check_cuda(ctx, cudaMalloc(&t->d_ref, head + sz.bytes() + 256), "cudaMalloc(reference store)");
+        if (rc == YGZB_OK) rc = check_cuda(ctx, cudaMemsetAsync(t->d_ref, 0, head, ctx->stream), "memset");
+        if (rc == YGZB_OK) rc = check_cuda(ctx, cudaMallocHost((void**)&t->h_aux, sizeof(int32_t) * 2 * (size_t)t->max_jobs), "cudaMallocHost");
+        if (rc == YGZB_OK) rc = dalloc(ctx, &t->d_aux, 2 * (size_t)t->max_jobs);
+        if (rc != YGZB_OK) {
+            if (t->d_ref) cudaFree(t->d_ref);
+            if (t->h_aux) cudaFreeHost(t->h_aux);
+            t->d_ref = nullptr;
+            t->h_aux = nullptr;
+            return rc;
+        }
+        Carver c(t->d_ref);
+        const size_t R2 = 2 * (size_t)S, cap = st.ref_cap;
+        st.ref_px = c.take<double>(R2 * cap * 2); st.ref_depth = c.take<double>(R2 * cap); st.ref_n = c.take<int32_t>(R2);
+        st.ref_T = c.take<double>(R2 * 12); st.ref_cur = c.take<int32_t>(S);
+        t->st = st;
+    }
+    t->ref_mode = mode;
+    t->ref_slots.assign(ref_slots && mode == YGZB_TRACK_REF_PREVIOUS ? ref_slots : nullptr, ref_slots && mode == YGZB_TRACK_REF_PREVIOUS ? ref_slots + S : nullptr);
+    t->cur_ref.assign(S, -1);
+    return YGZB_OK;
+}
+
+int ygzb_tracker_debug_reference(ygzb_tracker* t, int stream, ygzb_track_reference* out) {
+    if (!t || !out) return YGZB_ERR_INVALID;
+    ygzb_ctx* ctx = t->ctx;
+    if (t->ref_mode != YGZB_TRACK_REF_PREVIOUS) return set_error(ctx, YGZB_ERR_INVALID, "debug_reference: not in previous-frame reference mode");
+    if (stream < 0 || stream >= t->st.S) return set_error(ctx, YGZB_ERR_INVALID, "debug_reference: stream %d out of range", stream);
+    if (!out->px || !out->depth) return set_error(ctx, YGZB_ERR_INVALID, "debug_reference: null array");
+    cudaSetDevice(ctx->device);
+    YGZB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    int32_t cur = 0, n = 0;
+    YGZB_CUDA(ctx, cudaMemcpy(&cur, t->st.ref_cur + stream, sizeof(int32_t), cudaMemcpyDeviceToHost));
+    const size_t r = 2 * (size_t)stream + cur;
+    YGZB_CUDA(ctx, cudaMemcpy(&n, t->st.ref_n + r, sizeof(int32_t), cudaMemcpyDeviceToHost));
+    if (n > out->capacity) return set_error(ctx, YGZB_ERR_CAPACITY, "debug_reference: %d features exceed the capacity %d", n, out->capacity);
+    out->slot = t->cur_ref[stream];
+    out->n = n;
+    YGZB_CUDA(ctx, cudaMemcpy(out->T_cw, t->st.ref_T + 12 * r, 12 * sizeof(double), cudaMemcpyDeviceToHost));
+    YGZB_CUDA(ctx, cudaMemcpy(out->px, t->st.ref_px + 2 * r * t->st.ref_cap, 2 * (size_t)n * sizeof(double), cudaMemcpyDeviceToHost));
+    YGZB_CUDA(ctx, cudaMemcpy(out->depth, t->st.ref_depth + r * t->st.ref_cap, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost));
+    return YGZB_OK;
 }
 
 int ygzb_tracker_set_depth(ygzb_tracker* t, int stream, const double* depth) {
@@ -666,11 +914,13 @@ int ygzb_tracker_track(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, 
         for (int k = 0; k < q.n_local; ++k)
             if (q.entry[k] < 0 || q.entry[k] >= YGZB_TRACK_RING) return set_error(ctx, YGZB_ERR_INVALID, "track job %d: ring entry out of range", j);
     }
+    if (t->ref_mode == YGZB_TRACK_REF_PREVIOUS) return track_previous(t, n_jobs, jobs, results);
     YGZB_CUDA(ctx, cudaEventSynchronize(t->staged));   // the previous copy out of the staging buffer has finished
     memcpy(t->h_jobs, jobs, sizeof(ygzb_track_job) * (size_t)n_jobs);
     TrackBatch b = t->b;
     b.J = n_jobs;
     t->last_J = n_jobs;
+    t->pos_of.clear();
     const int cl = t->cluster;
     int rc;
     {   // part 1 on the front stream: behind the key-frame insertion (new reference features, and the batch arrays it still
@@ -737,6 +987,10 @@ int ygzb_tracker_make_keyframes(ygzb_tracker* t, int n, const ygzb_keyframe_job*
         }
     YGZB_CUDA(ctx, cudaEventSynchronize(t->staged));
     memcpy(t->h_kfjobs, jobs, sizeof(ygzb_keyframe_job) * (size_t)n);
+    const bool prev = t->ref_mode == YGZB_TRACK_REF_PREVIOUS;
+    for (int i = 0; i < n; ++i)   // (previous-frame mode keeps the batch in wave order)
+        if (jobs[i].track_job >= 0 && !t->pos_of.empty()) t->h_kfjobs[i].track_job = t->pos_of[jobs[i].track_job];
+    t->kf_inserted = true;
     YGZB_CUDA(ctx, cudaMemcpyAsync(t->d_kfjobs, t->h_kfjobs, sizeof(ygzb_keyframe_job) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
     BABuild B{};
     B.pcap = t->pcap;
@@ -756,7 +1010,9 @@ int ygzb_tracker_make_keyframes(ygzb_tracker* t, int n, const ygzb_keyframe_job*
                                                              t->d_kfres);
         YGZB_LAUNCHED(ctx);
     }
-    YGZB_CUDA(ctx, cudaEventRecord(t->e_fill, ctx->stream));   // from here on only the BA runs: the next batch's front part may start
+    // from here on only the BA runs: the next batch's front part may start (key-frame mode: the alignment is relative to the
+    // key-frame and needs its features only; previous-frame mode records this behind the reference, below)
+    if (!prev) YGZB_CUDA(ctx, cudaEventRecord(t->e_fill, ctx->stream));
     double* d_ba_stats = nullptr;
     if (P > 0) {
         {
@@ -786,6 +1042,15 @@ int ygzb_tracker_make_keyframes(ygzb_tracker* t, int n, const ygzb_keyframe_job*
         ProfScope ps(ctx, kStageOther);
         ba_writeback_kernel<<<(unsigned)n, 256, 0, ctx->stream>>>(t->st, t->d_kfjobs, B, d_ba_stats, t->d_kfres);
         YGZB_LAUNCHED(ctx);
+    }
+    if (prev) {   // the key-frame becomes its stream's reference, with the BA's pose and points
+        {
+            ProfScope ps(ctx, kStageOther);
+            kf_ref_kernel<<<(unsigned)n, 256, 0, ctx->stream>>>(t->st, b, t->d_kfjobs);
+            YGZB_LAUNCHED(ctx);
+        }
+        for (int i = 0; i < n; ++i) t->cur_ref[jobs[i].stream] = jobs[i].kf_slot;
+        YGZB_CUDA(ctx, cudaEventRecord(t->e_fill, ctx->stream));
     }
     YGZB_CUDA(ctx, cudaMemcpyAsync(results, t->d_kfres, sizeof(ygzb_keyframe_result) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
     return YGZB_OK;
@@ -924,6 +1189,7 @@ int ygzb_tracker_debug_job(ygzb_tracker* t, int job, ygzb_track_debug* out) {
         return set_error(ctx, YGZB_ERR_INVALID, "debug: null array");
     cudaSetDevice(ctx->device);
     const TrackBatch& b = t->b;
+    if (!t->pos_of.empty()) job = t->pos_of[job];   // previous-frame mode keeps the batch in wave order
     const size_t j = (size_t)job, cap = (size_t)b.cap;
     auto d2h = [&](void* dst, const void* src, size_t bytes) {
         return check_cuda(ctx, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, ctx->stream), "D2H(track debug)");

@@ -29,6 +29,14 @@ struct TrackStore {
     long long* kf_obs_id;       // [S*R][kTrackMaxLocal*cells]
     double* kf_obs_px;          // [S*R][kTrackMaxLocal*cells][2]
     const double* depth_map;    // [S][W*H]    depth image of the frame that becomes a key-frame (stand-in for the TUM depth)
+    // previous-frame reference (YGZB_TRACK_REF_PREVIOUS): per stream two buffers r = 2 * stream + b of ref_cap features;
+    // ref_cur[stream] is the one the stream's next job aligns against
+    int ref_cap;                // kTrackMaxLocal * cells tracked + cells new features
+    double* ref_px;             // [2S][ref_cap][2]
+    double* ref_depth;          // [2S][ref_cap]
+    int32_t* ref_n;             // [2S]
+    double* ref_T;              // [2S][12]
+    int32_t* ref_cur;           // [S]
 };
 
 struct TrackBatch {
@@ -59,6 +67,11 @@ struct TrackBatch {
     int32_t* n_inl;
     double* pose_ws;
     ygzb_track_result* results; // [J]
+    // previous-frame reference: the jobs are reordered into waves (wave w = the w-th job of every stream) and a wave runs as
+    // a batch of its own (pointers shifted to its first job); prev = 0 in key-frame mode
+    int prev;
+    const int32_t* job_ref_slot; // [J] slot of the pyramid the job aligns against
+    const int32_t* orig;         // [J] the caller's index of the job (results order)
 };
 
 // align.cu

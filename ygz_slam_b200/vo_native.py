@@ -22,6 +22,8 @@ def _lib():
         _LIB.ygz_vo_run.restype = C.c_int
         _LIB.ygz_vo_run.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                     C.c_double, C.c_double, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        _LIB.ygz_vo_run_ex.restype = C.c_int
+        _LIB.ygz_vo_run_ex.argtypes = _LIB.ygz_vo_run.argtypes + [C.c_int]
         _LIB.ygz_vo_run_handoff.restype = C.c_int
         _LIB.ygz_vo_run_handoff.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                             C.c_double, C.c_double, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -43,8 +45,11 @@ def stack_pinned(frames):
     return stacked
 
 
+_REF_MODES = {"keyframe": 0, "previous": 1}   # YGZB_TRACK_REF_KEYFRAME / _PREVIOUS
+
+
 def run(ctx, frames, depths, kf_min_frames=10, kf_min_rot=0.1, kf_min_trans=0.1, warm=0, threads=1, device_frames=None,
-        return_device_ms=False, details=False, window=1, engine="resident", handoff=None, return_maps=False):
+        return_device_ms=False, details=False, window=1, engine="resident", handoff=None, return_maps=False, ref_mode="keyframe"):
     """frames: list of (n_frames, 480, 640) uint8 arrays or one stacked (S, n, 480, 640) array (ideally from stack_pinned);
     depths[s]: (480, 640) float64.  device_frames = (device pointer, S, n): the same stacked layout already resident in
     HBM (the "value" leg of bench.py) -- the driver then copies device-to-device.  The context must use the 3-level pyramid.
@@ -54,7 +59,13 @@ def run(ctx, frames, depths, kf_min_frames=10, kf_min_rot=0.1, kf_min_trans=0.1,
     handoff = frame h (resident engine only): at h every stream's local map is exported, the tracker torn down and the
     streams carried over to a fresh tracker on a new context in reverse order (ygz_vo_run_handoff); the results equal a
     run with warm = h.  return_maps (with handoff): also return the maps exported at h, one capi.MapBuffers per stream.
+    ref_mode (resident engine without handoff): "keyframe" aligns every frame against the newest key-frame; "previous"
+    against the previous frame, the reference's rule (ygz_vo_run_ex, YGZB_TRACK_REF_PREVIOUS).
     Returns (trajectory (S, n_frames, 3, 4), stats list of dicts, seconds of frames [warm, n_frames)[, device ms][, maps])."""
+    if ref_mode not in _REF_MODES:
+        raise ValueError(f"ref_mode must be 'keyframe' or 'previous', not {ref_mode!r}")
+    if ref_mode != "keyframe" and (engine != "resident" or handoff is not None):
+        raise ValueError("the previous-frame reference is only offered by the resident engine without handoff")
     if device_frames is not None:
         base, S, n = device_frames
         ptrs = [base + s * n * 480 * 640 for s in range(S)]
@@ -83,9 +94,9 @@ def run(ctx, frames, depths, kf_min_frames=10, kf_min_rot=0.1, kf_min_trans=0.1,
                                        C.cast(recs, C.c_void_p) if return_maps else None, traj.ctypes.data, stats.ctypes.data,
                                        C.byref(sec), C.byref(dev_ms), totals.ctypes.data)
     else:
-        rc = _lib().ygz_vo_run(ctx.h, ctx.device_index, C.byref(ctx.params), threads, S, n, C.cast(ip, C.c_void_p), C.cast(dp, C.c_void_p),
-                               kf_min_frames, kf_min_rot, kf_min_trans, warm, int(window), traj.ctypes.data, stats.ctypes.data,
-                               C.byref(sec), C.byref(dev_ms), totals.ctypes.data)
+        rc = _lib().ygz_vo_run_ex(ctx.h, ctx.device_index, C.byref(ctx.params), threads, S, n, C.cast(ip, C.c_void_p), C.cast(dp, C.c_void_p),
+                                  kf_min_frames, kf_min_rot, kf_min_trans, warm, int(window), traj.ctypes.data, stats.ctypes.data,
+                                  C.byref(sec), C.byref(dev_ms), totals.ctypes.data, _REF_MODES[ref_mode])
     ctx.check(rc, "ygz_vo_run")
     if handoff is not None and return_maps:
         return _result(traj, stats, totals, sec, dev_ms, S, n, details, return_device_ms) + (maps,)
