@@ -465,6 +465,45 @@ int ygzb_tracker_export(ygzb_tracker* t, int stream, int n_entries, const int32_
  * a level >= the pyramid depth or a missing image returns YGZB_ERR_INVALID with the tracker untouched.             */
 int ygzb_tracker_import(ygzb_tracker* t, int stream, const int32_t* entries, const int32_t* kf_slots, const ygzb_map_record* in);
 
+/* ---- reference record: what a stream in YGZB_TRACK_REF_PREVIOUS mode aligns its next frame against ------------------
+ * In previous-frame mode (ygzb_tracker_set_reference_mode, below) a stream's state is its ring plus its current
+ * reference: the pose, projected pixels and depths of the previous tracked frame or key-frame, and the pyramid of that
+ * frame.  A reference record carries both out of a tracker and into another; together with the map record of the
+ * stream's ring it is everything a stream tracked the reference's way needs to continue bit for bit.  The pyramid
+ * travels as its level-0 image, from which the destination rebuilds it.  Capacity: at most
+ * YGZB_TRACK_REF_FEATURES_PER_CELL * C features (C = grid cells), every tracked candidate of the local key-frames plus
+ * the new features of a key-frame.                                                                                     */
+#define YGZB_TRACK_REF_FEATURES_PER_CELL (YGZB_TRACK_RING + 1)
+typedef struct {
+    int32_t width, height, cells, n_levels;   /* as in ygzb_map_record                                              */
+    double K[4];
+    int32_t capacity;      /* in: rows px / depth hold; at least YGZB_TRACK_REF_FEATURES_PER_CELL * cells              */
+    int32_t n;             /* features of the reference                                                              */
+    double T_cw[12];       /* its pose                                                                               */
+    double* px;            /* [capacity][2] full-resolution pixels, in the order the alignment reads them             */
+    double* depth;         /* [capacity]                                                                             */
+    uint8_t* image;        /* [height][width] level 0 of the pyramid the stream aligns its next frame against         */
+} ygzb_reference_record;
+
+/* asynchronous like ygzb_tracker_export, on the context's stream: ordered behind every tracking batch already enqueued
+ * (including the copy of its last frame into the stream's reference slot) and every key-frame insertion (including the
+ * key-frame's reference, written after its local BA).  One kernel packs the reference's rows, zeros up to the store's
+ * capacity and level 0 of its pyramid into a staging buffer; one copy per field moves them to `out`.  The header is
+ * written before the call returns; n, T_cw, px, depth and image are valid after ygzb_synchronize(ctx).  Rows past n are
+ * zero.  YGZB_ERR_INVALID for a tracker in key-frame mode, a stream out of range or without a reference yet, a capacity
+ * below YGZB_TRACK_REF_FEATURES_PER_CELL * cells, or a missing px, depth or image.                                    */
+int ygzb_tracker_export_reference(ygzb_tracker* t, int stream, ygzb_reference_record* out);
+/* writes record `in` as the current reference of `stream` (any stream of a previous-mode tracker with the same geometry
+ * and K): pose, pixels and depths into the stream's reference store, the image into its reference slot with the pyramid
+ * rebuilt (ygzb_frames_upload).  A reference that was a key-frame in the source lives in the reference slot here; the
+ * pixels are the same, and so are the results.  Like a key-frame insertion, it fixes the reference mode.  Asynchronous
+ * on the context's stream like ygzb_tracker_import.  The whole record is checked first: a tracker in key-frame mode, a
+ * stream out of range, a capacity below the store's, n < 0 or above it, a different geometry or K, or a missing px,
+ * depth or image returns YGZB_ERR_INVALID with the tracker untouched.
+ * A stream moves to another tracker in this order: ygzb_tracker_set_reference_mode(YGZB_TRACK_REF_PREVIOUS, ref_slots),
+ * ygzb_tracker_import (its map), ygzb_tracker_import_reference.                                                     */
+int ygzb_tracker_import_reference(ygzb_tracker* t, int stream, const ygzb_reference_record* in);
+
 /* ---- parity / debug view of the last tracking batch (tests; not part of the tracking path, like ygzb_fast_debug) ------
  * Synchronous: waits for the context's stream, then copies out the intermediate state of job `job` of the most recent
  * ygzb_tracker_track batch (valid until the next ygzb_tracker_track).  The caller sizes every array for
@@ -507,7 +546,8 @@ int ygzb_tracker_set_reference_mode(ygzb_tracker* t, int mode, const int32_t* re
 
 /* synchronous, for tests (like ygzb_tracker_debug_job): the current reference of a stream in YGZB_TRACK_REF_PREVIOUS
  * mode.  The caller sets capacity and sizes px [capacity][2] and depth [capacity]; a larger reference returns
- * YGZB_ERR_CAPACITY.  At most (YGZB_TRACK_RING + 1) * grid cells features.                                             */
+ * YGZB_ERR_CAPACITY.  At most YGZB_TRACK_REF_FEATURES_PER_CELL * grid cells features.  ygzb_tracker_export_reference
+ * reads the same reference asynchronously, with its image.                                                           */
 typedef struct {
     int32_t slot;          /* slot of its pyramid */
     int32_t n;             /* features */

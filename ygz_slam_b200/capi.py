@@ -44,6 +44,7 @@ EXPORTS = [
     "ygzb_default_klt_params", "ygzb_klt",
     "ygzb_tracker_create", "ygzb_tracker_destroy", "ygzb_tracker_set_depth", "ygzb_tracker_upload", "ygzb_tracker_track", "ygzb_tracker_make_keyframes",
     "ygzb_tracker_export", "ygzb_tracker_import", "ygzb_tracker_debug_job", "ygzb_tracker_set_reference_mode", "ygzb_tracker_debug_reference",
+    "ygzb_tracker_export_reference", "ygzb_tracker_import_reference",
 ]
 
 
@@ -735,6 +736,50 @@ class MapBuffers:
         return other
 
 
+# ---- reference records of the previous-frame mode (ygzb_tracker_export_reference / _import_reference) ----------------------
+REF_FEATURES_PER_CELL = TRACK_RING + 1   # YGZB_TRACK_REF_FEATURES_PER_CELL
+_REF_ARRAYS = ("px", "depth", "image")
+
+
+class ReferenceRecord(C.Structure):
+    _fields_ = ([("width", C.c_int32), ("height", C.c_int32), ("cells", C.c_int32), ("n_levels", C.c_int32), ("K", C.c_double * 4),
+                 ("capacity", C.c_int32), ("n", C.c_int32), ("T_cw", C.c_double * 12)] + [(k, C.c_void_p) for k in _REF_ARRAYS])
+
+
+class ReferenceBuffers:
+    """A ygzb_reference_record with numpy arrays behind it, sized for a `width` x `height` image with `cells` grid cells
+    (capacity REF_FEATURES_PER_CELL * cells).  `rec` may be an existing ReferenceRecord to point at the arrays."""
+
+    def __init__(self, width, height, cells, rec=None):
+        cap = REF_FEATURES_PER_CELL * cells
+        self.a = dict(px=np.zeros((cap, 2)), depth=np.zeros(cap), image=np.zeros((height, width), np.uint8))
+        self.rec = ReferenceRecord() if rec is None else rec
+        self.rec.capacity = cap
+        for k in _REF_ARRAYS:
+            setattr(self.rec, k, self.a[k].ctypes.data)
+
+    @property
+    def header(self):
+        r = self.rec
+        return dict(width=r.width, height=r.height, cells=r.cells, n_levels=r.n_levels, K=tuple(r.K), capacity=r.capacity, n=r.n)
+
+    @property
+    def T_cw(self):
+        return np.array(self.rec.T_cw).reshape(3, 4)
+
+    def copy(self):
+        """An independent record with the same header, pose and array contents."""
+        h, w = self.a["image"].shape
+        other = ReferenceBuffers(w, h, self.a["depth"].shape[0] // REF_FEATURES_PER_CELL)
+        for k in _REF_ARRAYS:
+            other.a[k][...] = self.a[k]
+        for k in ("width", "height", "cells", "n_levels", "capacity", "n"):
+            setattr(other.rec, k, getattr(self.rec, k))
+        other.rec.K[:] = list(self.rec.K)
+        other.rec.T_cw[:] = list(self.rec.T_cw)
+        return other
+
+
 class TrackJob(C.Structure):
     _fields_ = [("stream", C.c_int32), ("cur_slot", C.c_int32), ("n_local", C.c_int32), ("entry", C.c_int32 * TRACK_RING), ("pad", C.c_int32)]
 
@@ -787,6 +832,8 @@ class Tracker:
         self.lib.ygzb_tracker_debug_job.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         self.lib.ygzb_tracker_set_reference_mode.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         self.lib.ygzb_tracker_debug_reference.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        self.lib.ygzb_tracker_export_reference.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        self.lib.ygzb_tracker_import_reference.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         Kd = np.ascontiguousarray(K, np.float64)
         h = C.c_void_p()
         self.ctx.check(self.lib.ygzb_tracker_create(frames.h, n_streams, max_jobs, _p(Kd), C.byref(h)), "ygzb_tracker_create")
@@ -818,6 +865,20 @@ class Tracker:
         entries = np.ascontiguousarray(entries, np.int32)
         kf_slots = np.ascontiguousarray(kf_slots, np.int32)
         self.ctx.check(self.lib.ygzb_tracker_import(self.h, int(stream), _p(entries), _p(kf_slots), C.byref(rec.rec)), "ygzb_tracker_import")
+        self.ctx.synchronize()
+
+    def export_reference(self, stream: int, out: ReferenceBuffers | None = None) -> ReferenceBuffers:
+        """Reference record of `stream` (previous-frame mode), complete (the call synchronises the context)."""
+        if out is None:
+            f = self.frames
+            out = ReferenceBuffers(f.lw[0], f.lh[0], self.ctx.n_cells)
+        self.ctx.check(self.lib.ygzb_tracker_export_reference(self.h, int(stream), C.byref(out.rec)), "ygzb_tracker_export_reference")
+        self.ctx.synchronize()
+        return out
+
+    def import_reference(self, stream: int, rec: ReferenceBuffers):
+        """`rec` becomes the current reference of `stream`; import the stream's map first."""
+        self.ctx.check(self.lib.ygzb_tracker_import_reference(self.h, int(stream), C.byref(rec.rec)), "ygzb_tracker_import_reference")
         self.ctx.synchronize()
 
     def set_depth(self, stream: int, depth):

@@ -442,7 +442,8 @@ size_t babuild_carve(Carver& c, BABuild& B, size_t P, int cells, int n_jobs) {
 
 // ---- map records (ygzb_tracker_export / _import) -----------------------------------------------------------------------
 static_assert(YGZB_MAP_OBS_PER_CELL == kTrackMaxLocal, "a key-frame's observation capacity is kTrackMaxLocal * cells");
-constexpr int kXferChunks = 16;   // CTAs per key-frame of the pack / unpack kernels
+static_assert(YGZB_TRACK_REF_FEATURES_PER_CELL == kTrackMaxLocal + 1, "the reference store holds (kTrackMaxLocal + 1) * cells features");
+constexpr int kXferChunks = 16;   // CTAs per key-frame of the pack / unpack kernels (per reference record of theirs)
 
 struct MapXfer {   // device staging of one record: at most YGZB_TRACK_RING key-frames, packed like ygzb_map_record
     double* T;
@@ -451,6 +452,10 @@ struct MapXfer {   // device staging of one record: at most YGZB_TRACK_RING key-
     double *px, *depth, *pw, *obs_px;
     uint8_t *level, *image;
     long long* obs_id;
+    // and of one reference record (ygzb_tracker_export_reference / _import_reference): ref_cap rows and one image
+    double *ref_T, *ref_px, *ref_depth;
+    int32_t* ref_n;
+    uint8_t* ref_image;
 };
 
 struct MapXferJob {   // kernel argument: the ring entries of a record and, for an import, its packed offsets and slots
@@ -465,6 +470,9 @@ size_t xfer_carve(Carver& c, MapXfer& X, size_t cells, size_t cap_obs, size_t WH
     X.px = c.take<double>(R * cells * 2); X.level = c.take<uint8_t>(R * cells); X.depth = c.take<double>(R * cells);
     X.pw = c.take<double>(R * cells * 3); X.obs_id = c.take<long long>(R * cap_obs); X.obs_px = c.take<double>(R * cap_obs * 2);
     X.image = c.take<uint8_t>(R * WH);
+    const size_t ref_cap = YGZB_TRACK_REF_FEATURES_PER_CELL * cells;
+    X.ref_T = c.take<double>(12); X.ref_n = c.take<int32_t>(1); X.ref_px = c.take<double>(ref_cap * 2); X.ref_depth = c.take<double>(ref_cap);
+    X.ref_image = c.take<uint8_t>(WH);
     return c.bytes();
 }
 
@@ -560,6 +568,45 @@ __global__ void __launch_bounds__(256) map_unpack_kernel(TrackStore st, MapXfer 
     }
 }
 
+// reference export: the live rows of stream s's current reference buffer, zeros up to ref_cap, and level 0 of the slot its
+// pyramid is in (`lv0`, the host knows the slot when it enqueues); kXferChunks CTAs stride over rows and pixels
+__global__ void __launch_bounds__(256) ref_pack_kernel(TrackStore st, MapXfer X, int s, const uint8_t* __restrict__ lv0, int lv0_pitch) {
+    const int r = 2 * s + st.ref_cur[s], n = st.ref_n[r], tid = threadIdx.x;
+    if (blockIdx.x == 0) {
+        if (tid < 12) X.ref_T[tid] = st.ref_T[12 * (size_t)r + tid];
+        if (tid == 0) X.ref_n[0] = n;
+    }
+    const int step = gridDim.x * blockDim.x, first = blockIdx.x * blockDim.x + tid;
+    for (int i = first; i < st.ref_cap; i += step) {
+        double u = 0, v = 0, d = 0;
+        if (i < n) {
+            const size_t o = (size_t)r * st.ref_cap + i;
+            u = st.ref_px[2 * o]; v = st.ref_px[2 * o + 1];
+            d = st.ref_depth[o];
+        }
+        X.ref_px[2 * (size_t)i] = u; X.ref_px[2 * (size_t)i + 1] = v;
+        X.ref_depth[i] = d;
+    }
+    for (int i = first; i < st.W * st.H; i += step) {
+        const int y = i / st.W, x = i - y * st.W;
+        X.ref_image[i] = lv0[(size_t)y * lv0_pitch + x];
+    }
+}
+
+// reference import: the first n rows of an uploaded record, its pose and count into stream s's current reference buffer
+__global__ void __launch_bounds__(256) ref_unpack_kernel(TrackStore st, MapXfer X, int s, int n) {
+    const int r = 2 * s + st.ref_cur[s], tid = threadIdx.x;
+    if (blockIdx.x == 0) {
+        if (tid < 12) st.ref_T[12 * (size_t)r + tid] = X.ref_T[tid];
+        if (tid == 0) st.ref_n[r] = n;
+    }
+    for (int i = blockIdx.x * blockDim.x + tid; i < n; i += gridDim.x * blockDim.x) {
+        const size_t o = (size_t)r * st.ref_cap + i;
+        st.ref_px[2 * o] = X.ref_px[2 * (size_t)i]; st.ref_px[2 * o + 1] = X.ref_px[2 * (size_t)i + 1];
+        st.ref_depth[o] = X.ref_depth[i];
+    }
+}
+
 int tracker_xfer(ygzb_tracker* t, MapXfer& X) {
     const TrackStore& st = t->st;
     Carver c(nullptr);
@@ -581,6 +628,17 @@ int check_entries(ygzb_tracker* t, int n, const int32_t* entries, const int32_t*
             if (slots && slots[k2] == slots[k]) return set_error(ctx, YGZB_ERR_INVALID, "%s: frame slot %d given twice", what, slots[k]);
         }
     }
+    return YGZB_OK;
+}
+
+// the checks an export and an import of a reference record share: the mode, the stream, the capacity and the arrays
+int check_reference_call(ygzb_tracker* t, int stream, const ygzb_reference_record* rec, const char* what) {
+    ygzb_ctx* ctx = t->ctx;
+    if (t->ref_mode != YGZB_TRACK_REF_PREVIOUS) return set_error(ctx, YGZB_ERR_INVALID, "%s: not in previous-frame reference mode", what);
+    if (stream < 0 || stream >= t->st.S) return set_error(ctx, YGZB_ERR_INVALID, "%s: stream %d out of range", what, stream);
+    if (rec->capacity < t->st.ref_cap)
+        return set_error(ctx, YGZB_ERR_INVALID, "%s: capacity %d below the reference store's %d", what, rec->capacity, t->st.ref_cap);
+    if (!rec->px || !rec->depth || !rec->image) return set_error(ctx, YGZB_ERR_INVALID, "%s: null array in the record", what);
     return YGZB_OK;
 }
 
@@ -1179,6 +1237,88 @@ int ygzb_tracker_import(ygzb_tracker* t, int stream, const int32_t* entries, con
     for (int k = 0; k < n && rc == YGZB_OK; ++k) rc = ygzb_frames_upload(t->f, kf_slots[k], 1, in->image + k * WH, 1, WH);
     if (rc == YGZB_OK) rc = check_cuda(ctx, cudaEventRecord(t->e_fill, ctx->stream), "cudaEventRecord");
     return rc;
+}
+
+int ygzb_tracker_export_reference(ygzb_tracker* t, int stream, ygzb_reference_record* out) {
+    if (!t || !out) return YGZB_ERR_INVALID;
+    ygzb_ctx* ctx = t->ctx;
+    const TrackStore& st = t->st;
+    int rc = check_reference_call(t, stream, out, "export_reference");
+    if (rc != YGZB_OK) return rc;
+    const int slot = t->cur_ref[stream];
+    if (slot < 0) return set_error(ctx, YGZB_ERR_INVALID, "export_reference: stream %d has no reference yet", stream);
+    cudaSetDevice(ctx->device);
+    out->width = st.W; out->height = st.H; out->cells = st.cells; out->n_levels = ctx->geo.n_levels;
+    out->K[0] = st.fx; out->K[1] = st.fy; out->K[2] = st.cx; out->K[3] = st.cy;
+    MapXfer X;
+    rc = tracker_xfer(t, X);
+    if (rc != YGZB_OK) return rc;
+    // on the context's stream, where previous-frame tracking (its copy into the reference slot included) and key-frame
+    // insertion (kf_ref_kernel included) run; behind the front stream's uploads, in case a caller uploads into the slot
+    YGZB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, t->e_up, 0));
+    {
+        ProfScope ps(ctx, kStageOther);
+        const LevelGeom& lv = ctx->geo.lv[0];
+        ref_pack_kernel<<<kXferChunks, 256, 0, ctx->stream>>>(st, X, stream, t->f->d_pyr + (size_t)slot * ctx->slot_stride + lv.off, lv.pitch);
+        YGZB_LAUNCHED(ctx);
+    }
+    const size_t cap = st.ref_cap;
+    auto d2h = [&](void* dst, const void* src, size_t bytes) {
+        return check_cuda(ctx, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, ctx->stream), "D2H(reference record)");
+    };
+    if (rc == YGZB_OK) rc = d2h(&out->n, X.ref_n, sizeof(int32_t));
+    if (rc == YGZB_OK) rc = d2h(out->T_cw, X.ref_T, 12 * sizeof(double));
+    if (rc == YGZB_OK) rc = d2h(out->px, X.ref_px, cap * 2 * sizeof(double));
+    if (rc == YGZB_OK) rc = d2h(out->depth, X.ref_depth, cap * sizeof(double));
+    if (rc == YGZB_OK) rc = d2h(out->image, X.ref_image, (size_t)st.W * st.H);
+    if (rc == YGZB_OK && (size_t)out->capacity > cap) {   // rows the store cannot hold: zero, like the store's rows past n
+        memset(out->px + 2 * cap, 0, ((size_t)out->capacity - cap) * 2 * sizeof(double));
+        memset(out->depth + cap, 0, ((size_t)out->capacity - cap) * sizeof(double));
+    }
+    return rc;
+}
+
+int ygzb_tracker_import_reference(ygzb_tracker* t, int stream, const ygzb_reference_record* in) {
+    if (!t || !in) return YGZB_ERR_INVALID;
+    ygzb_ctx* ctx = t->ctx;
+    const TrackStore& st = t->st;
+    // ---- the whole record is checked before anything is enqueued
+    int rc = check_reference_call(t, stream, in, "import_reference");
+    if (rc != YGZB_OK) return rc;
+    if (in->width != st.W || in->height != st.H || in->cells != st.cells || in->n_levels != ctx->geo.n_levels)
+        return set_error(ctx, YGZB_ERR_INVALID, "import_reference: record geometry %dx%d, %d cells, %d levels; tracker %dx%d, %d cells, %d levels",
+                         in->width, in->height, in->cells, in->n_levels, st.W, st.H, st.cells, ctx->geo.n_levels);
+    if (!(in->K[0] == st.fx && in->K[1] == st.fy && in->K[2] == st.cx && in->K[3] == st.cy))
+        return set_error(ctx, YGZB_ERR_INVALID, "import_reference: record intrinsics differ from the tracker's");
+    const int n = in->n;
+    if (n < 0 || n > st.ref_cap) return set_error(ctx, YGZB_ERR_INVALID, "import_reference: %d features (capacity %d)", n, st.ref_cap);
+    // ---- enqueue on the context's stream, behind the front stream's uploads and sparse alignment, like an import of a map;
+    //      the next upload waits for e_fill
+    cudaSetDevice(ctx->device);
+    MapXfer X;
+    rc = tracker_xfer(t, X);
+    if (rc != YGZB_OK) return rc;
+    YGZB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, t->e_up, 0));
+    YGZB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, t->e_front, 0));
+    auto h2d = [&](void* dst, const void* src, size_t bytes) {
+        return bytes ? check_cuda(ctx, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, ctx->stream), "H2D(reference record)") : YGZB_OK;
+    };
+    if (rc == YGZB_OK) rc = h2d(X.ref_T, in->T_cw, 12 * sizeof(double));
+    if (rc == YGZB_OK) rc = h2d(X.ref_px, in->px, (size_t)n * 2 * sizeof(double));
+    if (rc == YGZB_OK) rc = h2d(X.ref_depth, in->depth, (size_t)n * sizeof(double));
+    if (rc != YGZB_OK) return rc;
+    {
+        ProfScope ps(ctx, kStageOther);
+        ref_unpack_kernel<<<kXferChunks, 256, 0, ctx->stream>>>(st, X, stream, n);
+        YGZB_LAUNCHED(ctx);
+    }
+    const size_t WH = (size_t)st.W * st.H;
+    rc = ygzb_frames_upload(t->f, t->ref_slots[stream], 1, in->image, 1, WH);
+    if (rc == YGZB_OK) rc = check_cuda(ctx, cudaEventRecord(t->e_fill, ctx->stream), "cudaEventRecord");
+    if (rc != YGZB_OK) return rc;
+    t->cur_ref[stream] = t->ref_slots[stream];
+    t->kf_inserted = true;   // the stream has a reference of the previous-frame mode: the mode is fixed from here on
+    return YGZB_OK;
 }
 
 int ygzb_tracker_debug_job(ygzb_tracker* t, int job, ygzb_track_debug* out) {

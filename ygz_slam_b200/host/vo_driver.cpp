@@ -741,9 +741,14 @@ class Engine {
         for (const KfInfo& kf : st_[i].kfs) entries.push_back(kf.entry);
         return ygzb_tracker_export(tr_, i, (int)entries.size(), entries.data(), rec);
     }
+    // previous-frame mode: whether stream i has a reference (its first key-frame has been inserted), and that reference
+    // into `rec` (asynchronous like export_map)
+    bool has_reference(int i) const { return prm_.ref_mode == YGZB_TRACK_REF_PREVIOUS && !st_[i].kfs.empty(); }
+    int export_reference(int i, ygzb_reference_record* rec) const { return ygzb_tracker_export_reference(tr_, i, rec); }
     // stream i continues a stream of another engine: its map (exported by export_map) goes into the same ring entries, its
-    // key-frame images into this engine's key-frame slots of stream i, and its host bookkeeping is taken over as it is
-    int adopt(int i, const EStream& s, const ygzb_map_record* rec) {
+    // key-frame images into this engine's key-frame slots of stream i, in previous-frame mode its reference (exported by
+    // export_reference; NULL if it has none) into stream i's reference slot, and its host bookkeeping is taken over as it is
+    int adopt(int i, const EStream& s, const ygzb_map_record* rec, const ygzb_reference_record* ref) {
         std::vector<int32_t> entries, slots;
         for (const KfInfo& kf : s.kfs) {
             entries.push_back(kf.entry);
@@ -751,6 +756,7 @@ class Engine {
         }
         if (rec->n_keyframes != (int)entries.size()) return YGZB_ERR_INVALID;
         CHK(ygzb_tracker_import(tr_, i, entries.data(), slots.data(), rec));
+        if (ref) CHK(ygzb_tracker_import_reference(tr_, i, ref));
         st_[i] = s;
         return YGZB_OK;
     }
@@ -818,12 +824,25 @@ struct MapBuf {
     }
 };
 
+// host arrays behind a reference record (ygzb_reference_record capacity)
+struct RefBuf {
+    std::vector<double> px, depth;
+    std::vector<uint8_t> image;
+    ygzb_reference_record rec{};
+    explicit RefBuf(int cells) {
+        const size_t cap = (size_t)YGZB_TRACK_REF_FEATURES_PER_CELL * cells;
+        px.resize(2 * cap); depth.resize(cap); image.resize((size_t)W * H);
+        rec.capacity = (int32_t)cap;
+        rec.px = px.data(); rec.depth = depth.data(); rec.image = image.data();
+    }
+};
+
 // Device-resident engine over the streams of one host thread; with handoff >= 0 the streams move to a new tracker at frame
-// `handoff` (see ygz_vo_run_handoff).  Shared by ygz_vo_run (handoff < 0) and ygz_vo_run_handoff.
+// `handoff` (see ygz_vo_run_handoff_ex).  Shared by ygz_vo_run(_ex) (handoff < 0) and ygz_vo_run_handoff(_ex).
 int run_engine(ygzb_ctx* ctx, int device, const ygzb_params* params, int n_threads, int n_streams, int n_frames,
                const uint8_t* const* images, const double* const* depth, int kf_min_frames, double kf_min_rot, double kf_min_trans,
-               int warm, int window, int handoff, ygzb_map_record* maps, double* traj, int64_t* stats, double* seconds, double* device_ms,
-               int64_t* totals, int ref_mode) {
+               int warm, int window, int handoff, ygzb_map_record* maps, ygzb_reference_record* refs, double* traj, int64_t* stats,
+               double* seconds, double* device_ms, int64_t* totals, int ref_mode) {
     if (ref_mode != YGZB_TRACK_REF_KEYFRAME && ref_mode != YGZB_TRACK_REF_PREVIOUS) return YGZB_ERR_INVALID;
     if (!ctx || !params || n_streams < 1 || n_frames < 1 || !images || !depth || !traj || !stats || !seconds) return YGZB_ERR_INVALID;
     n_threads = std::max(1, std::min(n_threads, n_streams));
@@ -847,15 +866,19 @@ int run_engine(ygzb_ctx* ctx, int device, const ygzb_params* params, int n_threa
             double* my_traj = traj + (size_t)s0 * n_frames * 12;
             bool timed = false, handed = false;
             long long launch_base = 0;
-            // run to frame `handoff`, export every stream's map, tear the tracker, its frame pool and (but for the caller's)
-            // the context down, and carry the streams over to a fresh engine on a new context in reverse order
+            // run to frame `handoff`, export every stream's map (and in previous-frame mode its reference), tear the tracker,
+            // its frame pool and (but for the caller's) the context down, and carry the streams over to a fresh engine on a
+            // new context in reverse order
             auto hand_over = [&]() -> int {
                 CHK(eng->run_until(images + s0, n_frames, handoff, my_traj));
                 int cells_r = 0, cells_c = 0;
                 ygzb_grid_dims(my, &cells_r, &cells_c);
                 std::vector<MapBuf> own;
+                std::vector<RefBuf> own_refs;
                 std::vector<ygzb_map_record*> recs(ns);
+                std::vector<ygzb_reference_record*> ref_recs(ns, nullptr);
                 if (!maps) own.reserve(ns);
+                if (!refs) own_refs.reserve(ns);
                 for (int i = 0; i < ns; ++i) {
                     if (maps) {
                         recs[i] = maps + s0 + eng->order()[i];
@@ -864,6 +887,14 @@ int run_engine(ygzb_ctx* ctx, int device, const ygzb_params* params, int n_threa
                         recs[i] = &own.back().rec;
                     }
                     CHK(eng->export_map(i, recs[i]));
+                    if (!eng->has_reference(i)) continue;
+                    if (refs) {
+                        ref_recs[i] = refs + s0 + eng->order()[i];
+                    } else {
+                        own_refs.emplace_back(cells_r * cells_c);
+                        ref_recs[i] = &own_refs.back().rec;
+                    }
+                    CHK(eng->export_reference(i, ref_recs[i]));
                 }
                 CHK(ygzb_synchronize(my));
                 const std::vector<EStream> carried = eng->streams();
@@ -884,7 +915,7 @@ int run_engine(ygzb_ctx* ctx, int device, const ygzb_params* params, int n_threa
                 CHK(created);
                 launch_base = ygzb_launch_count(my);
                 CHK(eng->init(depth + s0));
-                for (int j = 0; j < ns; ++j) CHK(eng->adopt(j, carried[ns - 1 - j], recs[ns - 1 - j]));
+                for (int j = 0; j < ns; ++j) CHK(eng->adopt(j, carried[ns - 1 - j], recs[ns - 1 - j], ref_recs[ns - 1 - j]));
                 return YGZB_OK;
             };
             auto advance = [&](int limit) {
@@ -1060,7 +1091,7 @@ int ygz_vo_run(ygzb_ctx* ctx, int device, const ygzb_params* params, int n_threa
                const uint8_t* const* images, const double* const* depth, int kf_min_frames, double kf_min_rot, double kf_min_trans,
                int warm, int window, double* traj, int64_t* stats, double* seconds, double* device_ms, int64_t* totals) {
     return run_engine(ctx, device, params, n_threads, n_streams, n_frames, images, depth, kf_min_frames, kf_min_rot, kf_min_trans, warm, window,
-                      -1, nullptr, traj, stats, seconds, device_ms, totals, YGZB_TRACK_REF_KEYFRAME);
+                      -1, nullptr, nullptr, traj, stats, seconds, device_ms, totals, YGZB_TRACK_REF_KEYFRAME);
 }
 
 // ygz_vo_run with the tracker's reference mode: YGZB_TRACK_REF_KEYFRAME (= ygz_vo_run) or YGZB_TRACK_REF_PREVIOUS, the
@@ -1070,25 +1101,39 @@ int ygz_vo_run_ex(ygzb_ctx* ctx, int device, const ygzb_params* params, int n_th
                   const uint8_t* const* images, const double* const* depth, int kf_min_frames, double kf_min_rot, double kf_min_trans,
                   int warm, int window, double* traj, int64_t* stats, double* seconds, double* device_ms, int64_t* totals, int ref_mode) {
     return run_engine(ctx, device, params, n_threads, n_streams, n_frames, images, depth, kf_min_frames, kf_min_rot, kf_min_trans, warm, window,
-                      -1, nullptr, traj, stats, seconds, device_ms, totals, ref_mode);
+                      -1, nullptr, nullptr, traj, stats, seconds, device_ms, totals, ref_mode);
 }
 
-// The device-resident engine with a hand-over of every stream to a new tracker: ygz_vo_run's arguments plus
+// The device-resident engine with a hand-over of every stream to a new tracker: ygz_vo_run_ex's arguments plus
 //   handoff : every host thread runs its streams to frame `handoff` (nothing in flight), exports each stream's key-frames
-//             (ygzb_tracker_export), destroys its tracker and frame pool, creates a fresh tracker on a new context of the
-//             same device with the stream order reversed (a stream changes its index), imports the maps
-//             (ygzb_tracker_import), takes the host-side bookkeeping over and runs on to the last frame;
+//             (ygzb_tracker_export) and, in YGZB_TRACK_REF_PREVIOUS mode, then its reference (ygzb_tracker_export_reference),
+//             destroys its tracker and frame pool, creates a fresh tracker on a new context of the same device with the
+//             stream order reversed (a stream changes its index), imports the maps (ygzb_tracker_import) and then the
+//             references (ygzb_tracker_import_reference), takes the host-side bookkeeping over and runs on to the last frame;
 //   maps    : NULL, or n_streams records (one per stream, each sized for YGZB_TRACK_RING key-frames, images included) that
-//             receive the exported maps and are what the new tracker imports.
-// Results equal those of ygz_vo_run with warm = handoff, which splits the run at the same frame.  The hand-over's own
+//             receive the exported maps and are what the new tracker imports;
+//   refs    : (previous-frame mode; unused in key-frame mode) NULL, or n_streams reference records (each with capacity >=
+//             YGZB_TRACK_REF_FEATURES_PER_CELL * grid cells, px, depth and image set) that receive the exported references
+//             and are what the new tracker imports.  A stream without a key-frame at the hand-over has no reference yet and
+//             leaves its record as it was.
+// Results equal those of ygz_vo_run_ex with warm = handoff, which splits the run at the same frame.  The hand-over's own
 // record copies are not counted in `totals`.
+int ygz_vo_run_handoff_ex(ygzb_ctx* ctx, int device, const ygzb_params* params, int n_threads, int n_streams, int n_frames,
+                          const uint8_t* const* images, const double* const* depth, int kf_min_frames, double kf_min_rot, double kf_min_trans,
+                          int warm, int window, int handoff, ygzb_map_record* maps, ygzb_reference_record* refs, double* traj, int64_t* stats,
+                          double* seconds, double* device_ms, int64_t* totals, int ref_mode) {
+    if (handoff < 0) return YGZB_ERR_INVALID;
+    return run_engine(ctx, device, params, n_threads, n_streams, n_frames, images, depth, kf_min_frames, kf_min_rot, kf_min_trans, warm, window,
+                      handoff, maps, ref_mode == YGZB_TRACK_REF_PREVIOUS ? refs : nullptr, traj, stats, seconds, device_ms, totals, ref_mode);
+}
+
+// ygz_vo_run_handoff_ex in key-frame mode, without reference records
 int ygz_vo_run_handoff(ygzb_ctx* ctx, int device, const ygzb_params* params, int n_threads, int n_streams, int n_frames,
                        const uint8_t* const* images, const double* const* depth, int kf_min_frames, double kf_min_rot, double kf_min_trans,
                        int warm, int window, int handoff, ygzb_map_record* maps, double* traj, int64_t* stats, double* seconds,
                        double* device_ms, int64_t* totals) {
-    if (handoff < 0) return YGZB_ERR_INVALID;
-    return run_engine(ctx, device, params, n_threads, n_streams, n_frames, images, depth, kf_min_frames, kf_min_rot, kf_min_trans, warm, window,
-                      handoff, maps, traj, stats, seconds, device_ms, totals, YGZB_TRACK_REF_KEYFRAME);
+    return ygz_vo_run_handoff_ex(ctx, device, params, n_threads, n_streams, n_frames, images, depth, kf_min_frames, kf_min_rot, kf_min_trans,
+                                 warm, window, handoff, maps, nullptr, traj, stats, seconds, device_ms, totals, YGZB_TRACK_REF_KEYFRAME);
 }
 
 }  // extern "C"

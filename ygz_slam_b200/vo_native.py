@@ -28,6 +28,9 @@ def _lib():
         _LIB.ygz_vo_run_handoff.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                             C.c_double, C.c_double, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.c_void_p, C.c_void_p, C.c_void_p]
+        _LIB.ygz_vo_run_handoff_ex.restype = C.c_int
+        _LIB.ygz_vo_run_handoff_ex.argtypes = (_LIB.ygz_vo_run_handoff.argtypes[:15] + [C.c_void_p] + _LIB.ygz_vo_run_handoff.argtypes[15:]
+                                               + [C.c_int])
         _LIB.ygz_vo_run_stages.restype = C.c_int
         _LIB.ygz_vo_run_stages.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                            C.c_double, C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -56,16 +59,19 @@ def run(ctx, frames, depths, kf_min_frames=10, kf_min_rot=0.1, kf_min_trans=0.1,
     threads > 1 splits the streams over that many host threads, each with its own context (CUDA stream) on the device.
     engine = "resident": the device-resident engine (ygzb_tracker_*; `window` = frames of one stream in flight per round);
     engine = "stages": the per-stage C-ABI path (one blocking call per stage and lock-step frame).
-    handoff = frame h (resident engine only): at h every stream's local map is exported, the tracker torn down and the
-    streams carried over to a fresh tracker on a new context in reverse order (ygz_vo_run_handoff); the results equal a
-    run with warm = h.  return_maps (with handoff): also return the maps exported at h, one capi.MapBuffers per stream.
-    ref_mode (resident engine without handoff): "keyframe" aligns every frame against the newest key-frame; "previous"
-    against the previous frame, the reference's rule (ygz_vo_run_ex, YGZB_TRACK_REF_PREVIOUS).
-    Returns (trajectory (S, n_frames, 3, 4), stats list of dicts, seconds of frames [warm, n_frames)[, device ms][, maps])."""
+    handoff = frame h (resident engine only): at h every stream's local map (and, with ref_mode="previous", its reference)
+    is exported, the tracker torn down and the streams carried over to a fresh tracker on a new context in reverse order
+    (ygz_vo_run_handoff_ex); the results equal a run with warm = h.  return_maps (with handoff): also return the maps
+    exported at h, one capi.MapBuffers per stream, and with ref_mode="previous" the references, one capi.ReferenceBuffers
+    per stream (n = 0 for a stream that had no key-frame yet).
+    ref_mode (resident engine): "keyframe" aligns every frame against the newest key-frame; "previous" against the previous
+    frame, the reference's rule (ygz_vo_run_ex, YGZB_TRACK_REF_PREVIOUS).
+    Returns (trajectory (S, n_frames, 3, 4), stats list of dicts, seconds of frames [warm, n_frames)[, device ms][, maps]
+    [, references])."""
     if ref_mode not in _REF_MODES:
         raise ValueError(f"ref_mode must be 'keyframe' or 'previous', not {ref_mode!r}")
-    if ref_mode != "keyframe" and (engine != "resident" or handoff is not None):
-        raise ValueError("the previous-frame reference is only offered by the resident engine without handoff")
+    if ref_mode != "keyframe" and engine != "resident":
+        raise ValueError("the previous-frame reference is only offered by the resident engine")
     if device_frames is not None:
         base, S, n = device_frames
         ptrs = [base + s * n * 480 * 640 for s in range(S)]
@@ -86,20 +92,24 @@ def run(ctx, frames, depths, kf_min_frames=10, kf_min_rot=0.1, kf_min_trans=0.1,
                                       C.cast(dp, C.c_void_p), kf_min_frames, kf_min_rot, kf_min_trans, warm, traj.ctypes.data,
                                       stats.ctypes.data, C.byref(sec), C.byref(dev_ms), totals.ctypes.data)
     elif handoff is not None:
-        from .capi import TRACK_RING, MapBuffers, MapRecord
+        from .capi import TRACK_RING, MapBuffers, MapRecord, ReferenceBuffers, ReferenceRecord
         recs = (MapRecord * S)() if return_maps else None
         maps = [MapBuffers(TRACK_RING, 640, 480, ctx.n_cells, rec=recs[s_]) for s_ in range(S)] if return_maps else None
-        rc = _lib().ygz_vo_run_handoff(ctx.h, ctx.device_index, C.byref(ctx.params), threads, S, n, C.cast(ip, C.c_void_p),
-                                       C.cast(dp, C.c_void_p), kf_min_frames, kf_min_rot, kf_min_trans, warm, int(window), int(handoff),
-                                       C.cast(recs, C.c_void_p) if return_maps else None, traj.ctypes.data, stats.ctypes.data,
-                                       C.byref(sec), C.byref(dev_ms), totals.ctypes.data)
+        with_refs = return_maps and ref_mode == "previous"
+        ref_recs = (ReferenceRecord * S)() if with_refs else None
+        refs = [ReferenceBuffers(640, 480, ctx.n_cells, rec=ref_recs[s_]) for s_ in range(S)] if with_refs else None
+        rc = _lib().ygz_vo_run_handoff_ex(ctx.h, ctx.device_index, C.byref(ctx.params), threads, S, n, C.cast(ip, C.c_void_p),
+                                          C.cast(dp, C.c_void_p), kf_min_frames, kf_min_rot, kf_min_trans, warm, int(window), int(handoff),
+                                          C.cast(recs, C.c_void_p) if return_maps else None,
+                                          C.cast(ref_recs, C.c_void_p) if with_refs else None, traj.ctypes.data, stats.ctypes.data,
+                                          C.byref(sec), C.byref(dev_ms), totals.ctypes.data, _REF_MODES[ref_mode])
     else:
         rc = _lib().ygz_vo_run_ex(ctx.h, ctx.device_index, C.byref(ctx.params), threads, S, n, C.cast(ip, C.c_void_p), C.cast(dp, C.c_void_p),
                                   kf_min_frames, kf_min_rot, kf_min_trans, warm, int(window), traj.ctypes.data, stats.ctypes.data,
                                   C.byref(sec), C.byref(dev_ms), totals.ctypes.data, _REF_MODES[ref_mode])
     ctx.check(rc, "ygz_vo_run")
     if handoff is not None and return_maps:
-        return _result(traj, stats, totals, sec, dev_ms, S, n, details, return_device_ms) + (maps,)
+        return _result(traj, stats, totals, sec, dev_ms, S, n, details, return_device_ms) + (maps,) + ((refs,) if refs else ())
     return _result(traj, stats, totals, sec, dev_ms, S, n, details, return_device_ms)
 
 
