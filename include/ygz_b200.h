@@ -100,6 +100,32 @@ void* ygzb_frames_device_ptr(ygzb_frames* f);
 /* copy one level of one slot back to the host (tests) */
 int ygzb_frames_download_level(ygzb_frames* f, int slot, int level, uint8_t* host /* lw*lh, packed */);
 
+/* ---- lens undistortion on upload ----------------------------------------------------------------------------------
+ * The reference's camera reads the radial-tangential coefficients camera.k1 k2 p1 p2 (include/ygz/Basic/Camera.h:19-22)
+ * and declares UndistortPoint (:96-104), but nothing on its path applies them.  Here a frame pool can undistort every
+ * frame on the device as it enters the pyramid: level 0 becomes cv::remap(cv::cvtColor(image), map, INTER_LINEAR,
+ * BORDER_CONSTANT, 0), bit for bit, with the maps in OpenCV's fixed-point format (cv::initUndistortRectifyMap with
+ * CV_16SC2), so a caller with OpenCV can pass the maps it already has:
+ *   map_xy [H][W][2] int16   (CV_16SC2: integer source pixel x, y)
+ *   map_a  [H][W]    uint16  (CV_16UC1: (fy << 5) | fx, the 1/32-pixel fractions, < 1024)
+ * Source pixels outside the image read as 0.
+ *
+ * Host code, no device needed: cv::initUndistortRectifyMap(K, D, R = I, newK, (width, height), CV_16SC2) restated in
+ * double precision, D = {k1, k2, p1, p2, k3} (k3 = 0 is the model of the reference's UndistortPoint).  K and newK are
+ * {fx, fy, cx, cy}; newK == NULL means newK = K (unlike OpenCV, whose empty newK centres the principal point).       */
+int ygzb_undistort_map(int width, int height, const double K[4], const double dist[5], const double newK[4], int16_t* map_xy,
+                       uint16_t* map_a);
+/* copies the maps (image_width x image_height entries, host or device memory) to the device, one set per frame pool;
+ * map_xy == map_a == NULL clears them.  While they are set, every ygzb_frames_upload (grey or BGR, host or device source)
+ * and every ygzb_tracker_upload writes level 0 undistorted before the pyramid is built; ygzb_frames_build_pyramid, which
+ * starts from the level 0 already in the slot, is unchanged.  Then the camera of everything downstream is the
+ * undistorted one: the tracker's K (ygzb_tracker_create), the context's fx..cy and every depth map passed to
+ * ygzb_tracker_set_depth belong to newK.  Images the tracker re-uploads from a map or reference record
+ * (ygzb_tracker_import, ygzb_tracker_import_reference) are undistorted already and are not remapped again.
+ * Synchronous: the call waits for the uploads in flight that read the old maps.  An entry map_a >= 1024, or only one
+ * of the two pointers, returns YGZB_ERR_INVALID with the pool's maps unchanged.                                         */
+int ygzb_frames_set_undistort(ygzb_frames* f, const int16_t* map_xy, const uint16_t* map_a);
+
 /* ---- FeatureDetector ------------------------------------------------------------------------
  * replaces FeatureDetector::Detect (src/Algorithm/FeatureDetector.cpp:345-444; header
  * include/ygz/Algorithm/FeatureDetector.h:63): grid FAST-10 over the pyramid, 3x3 non-max, best
@@ -404,7 +430,8 @@ typedef struct {
     double T_cw[YGZB_TRACK_RING][12];   /* poses of the local key-frames after the BA, order of local_entry  */
 } ygzb_keyframe_result;
 
-/* K = {fx, fy, cx, cy} of the caller (doubles: the reference's callers project with PinholeCamera in double). */
+/* K = {fx, fy, cx, cy} of the caller (doubles: the reference's callers project with PinholeCamera in double); with
+ * undistortion maps on the pool (ygzb_frames_set_undistort), the undistorted camera newK. */
 int ygzb_tracker_create(ygzb_frames* f, int n_streams, int max_jobs, const double K[4], ygzb_tracker** out);
 void ygzb_tracker_destroy(ygzb_tracker* t);
 /* depth image (image_width * image_height doubles, host or device) that initialises the map points of the next key-frame

@@ -6,4 +6,4 @@ package only holds the ctypes binding used by the tests and the benchmark, the s
 generators, and the C++ shim classes (host/) that keep the reference's call surface.
 There is no CPU fallback: loading the library or creating a context fails loudly without it / an H100 (sm_90).
 """
-from .capi import Context, Frames, YgzbError, load_library, lib_path  # noqa: F401
+from .capi import Context, Frames, YgzbError, load_library, lib_path, undistort_map  # noqa: F401

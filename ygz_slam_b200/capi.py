@@ -44,7 +44,7 @@ EXPORTS = [
     "ygzb_default_klt_params", "ygzb_klt",
     "ygzb_tracker_create", "ygzb_tracker_destroy", "ygzb_tracker_set_depth", "ygzb_tracker_upload", "ygzb_tracker_track", "ygzb_tracker_make_keyframes",
     "ygzb_tracker_export", "ygzb_tracker_import", "ygzb_tracker_debug_job", "ygzb_tracker_set_reference_mode", "ygzb_tracker_debug_reference",
-    "ygzb_tracker_export_reference", "ygzb_tracker_import_reference",
+    "ygzb_tracker_export_reference", "ygzb_tracker_import_reference", "ygzb_undistort_map", "ygzb_frames_set_undistort",
 ]
 
 
@@ -119,6 +119,24 @@ def pinned_empty(shape, dtype):
 
 
 _PINNED_OWNERS: dict = {}
+
+
+def undistort_map(width: int, height: int, K, dist, newK=None):
+    """cv2.initUndistortRectifyMap(K, dist, None, newK, (width, height), cv2.CV_16SC2) without OpenCV (ygzb_undistort_map, host
+    code): K / newK = (fx, fy, cx, cy), newK None = K; dist = (k1, k2, p1, p2[, k3]).  Returns map_xy (H, W, 2) int16 and
+    map_a (H, W) uint16 for Frames.set_undistort."""
+    lib = load_library()
+    lib.ygzb_undistort_map.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    K = np.ascontiguousarray(K, np.float64).reshape(4)
+    d = np.zeros(5)
+    d[:len(dist)] = dist
+    nk = None if newK is None else np.ascontiguousarray(newK, np.float64).reshape(4)
+    map_xy = np.empty((height, width, 2), np.int16)
+    map_a = np.empty((height, width), np.uint16)
+    rc = lib.ygzb_undistort_map(int(width), int(height), _p(K), _p(d), _p(nk), _p(map_xy), _p(map_a))
+    if rc != 0:
+        raise YgzbError(f"ygzb_undistort_map failed (rc={rc}): bad size or camera")
+    return map_xy, map_a
 
 
 class Context:
@@ -259,6 +277,20 @@ class Frames:
     def upload_raw(self, ptr: int, n: int, channels: int, frame_stride: int, first: int = 0):
         self.ctx.check(self.lib.ygzb_frames_upload(self.h, first, n, C.c_void_p(ptr), channels, C.c_size_t(frame_stride)),
                        "ygzb_frames_upload")
+
+    def set_undistort(self, map_xy=None, map_a=None):
+        """Undistort every later upload into this pool: level 0 = cv2.remap of the (grey-converted) frame through OpenCV's
+        fixed-point maps, map_xy (H, W, 2) int16 and map_a (H, W) uint16 (cv2.initUndistortRectifyMap(.., cv2.CV_16SC2) or
+        undistort_map).  No arguments clear the maps."""
+        if map_xy is None and map_a is None:
+            self.ctx.check(self.lib.ygzb_frames_set_undistort(self.h, None, None), "ygzb_frames_set_undistort")
+            return
+        H, W = self.lh[0], self.lw[0]
+        map_xy = np.ascontiguousarray(map_xy, np.int16)
+        map_a = np.ascontiguousarray(map_a, np.uint16)
+        if map_xy.shape != (H, W, 2) or map_a.shape != (H, W):
+            raise ValueError(f"maps must be ({H}, {W}, 2) int16 and ({H}, {W}) uint16, not {map_xy.shape} and {map_a.shape}")
+        self.ctx.check(self.lib.ygzb_frames_set_undistort(self.h, _p(map_xy), _p(map_a)), "ygzb_frames_set_undistort")
 
     def copy_slot(self, src: int, dst: int):
         self.ctx.check(self.lib.ygzb_frames_copy(self.h, int(src), int(dst)), "ygzb_frames_copy")

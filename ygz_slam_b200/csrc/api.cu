@@ -3,6 +3,7 @@
 #include <stdarg.h>
 
 #include <algorithm>
+#include <cmath>
 #include <new>
 
 #include "common.cuh"
@@ -388,6 +389,12 @@ void ygzb_frames_destroy(ygzb_frames* f) {
     for (void* p : ptrs)
         if (p) cudaFree(p);
     if (f->d_tile_maps) cudaFree(f->d_tile_maps);
+    if (f->e_stage) {
+        cudaEventSynchronize(f->e_stage);
+        cudaEventDestroy(f->e_stage);
+    }
+    for (void* p : {(void*)f->d_map_xy, (void*)f->d_map_a, (void*)f->d_stage})
+        if (p) cudaFree(p);
     delete f;
 }
 
@@ -409,7 +416,7 @@ void* ygzb_frames_device_ptr(ygzb_frames* f) { return f ? f->d_pyr : nullptr; }
 int ygzb_frames_build_pyramid(ygzb_frames* f, int first, int count) {
     if (!f || first < 0 || count < 0 || first + count > f->capacity) return YGZB_ERR_INVALID;
     cudaSetDevice(f->ctx->device);
-    return launch_pyramid(f, first, count, nullptr);
+    return launch_pyramid(f, first, count, nullptr, 1, false);
 }
 
 int ygzb_frames_copy(ygzb_frames* f, int src_slot, int dst_slot) {
@@ -422,7 +429,52 @@ int ygzb_frames_copy(ygzb_frames* f, int src_slot, int dst_slot) {
     return YGZB_OK;
 }
 
-int ygzb_frames_upload(ygzb_frames* f, int first, int count, const uint8_t* host, int channels, size_t frame_stride) {
+}  // extern "C"
+
+namespace {
+
+// host or device memory -> device staging of `count` raw frames, packed (one frame after the other)
+int stage_frames(ygzb_ctx* ctx, uint8_t* dst, const uint8_t* src, int count, size_t frame_bytes, size_t frame_stride) {
+    // cudaMemcpyDefault: `src` may also be a device pointer (frames already resident in HBM, unified addressing).
+    // A strided batch copy treats one image as a "row", so its pitch is limited (cudaDeviceProp::memPitch, 2^31 - 1):
+    // longer strides (a stacked [stream][frame] array of thousands of frames) fall back to one copy per image.
+    if (frame_stride <= (size_t)0x7FFFFFFF) {
+        YGZB_CUDA(ctx, cudaMemcpy2DAsync(dst, frame_bytes, src, frame_stride, frame_bytes, count, cudaMemcpyDefault, ctx->stream));
+    } else {
+        for (int i = 0; i < count; ++i)
+            YGZB_CUDA(ctx, cudaMemcpyAsync(dst + (size_t)i * frame_bytes, src + (size_t)i * frame_stride, frame_bytes, cudaMemcpyDefault,
+                                           ctx->stream));
+    }
+    return YGZB_OK;
+}
+
+// undistorting upload: the raw frames go to the pool's staging buffer, remap_gray_kernel writes level 0.  The buffer is the
+// pool's own, not a context scratch buffer, because a tracker uploads on its front stream while the context's stream runs a
+// local BA; e_stage, recorded behind every remap on whichever stream ran it, orders each reuse of the buffer behind the
+// last read of it.
+int upload_undistorted(ygzb_frames* f, int first, int count, const uint8_t* src, int channels, size_t frame_stride) {
+    ygzb_ctx* ctx = f->ctx;
+    const Geometry& g = ctx->geo;
+    const size_t frame = (size_t)g.lv[0].w * g.lv[0].h * channels, bytes = frame * count;
+    if (f->stage_bytes < bytes) {
+        YGZB_CUDA(ctx, cudaEventSynchronize(f->e_stage));
+        if (f->d_stage) cudaFree(f->d_stage);
+        f->d_stage = nullptr;
+        f->stage_bytes = 0;
+        YGZB_CUDA(ctx, cudaMalloc((void**)&f->d_stage, bytes));
+        f->stage_bytes = bytes;
+    }
+    YGZB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, f->e_stage, 0));
+    int rc = stage_frames(ctx, f->d_stage, src, count, frame, frame_stride);
+    if (rc == YGZB_OK) rc = launch_pyramid(f, first, count, f->d_stage, channels, true);
+    // recorded even after a failed launch: a copy into the buffer may be in flight
+    const int rc_ev = check_cuda(ctx, cudaEventRecord(f->e_stage, ctx->stream), "cudaEventRecord");
+    return rc != YGZB_OK ? rc : rc_ev;
+}
+
+}  // namespace
+
+int ygzb::frames_upload(ygzb_frames* f, int first, int count, const uint8_t* host, int channels, size_t frame_stride, bool undistort) {
     if (!f || !host || first < 0 || count < 0 || first + count > f->capacity) return YGZB_ERR_INVALID;
     ygzb_ctx* ctx = f->ctx;
     const Geometry& g = ctx->geo;
@@ -431,6 +483,7 @@ int ygzb_frames_upload(ygzb_frames* f, int first, int count, const uint8_t* host
     if (channels != 1 && channels != 3) return set_error(ctx, YGZB_ERR_INVALID, "channels must be 1 or 3");
     if (frame_stride < row * g.lv[0].h) return set_error(ctx, YGZB_ERR_INVALID, "frame_stride smaller than one image");
     if (count == 0) return YGZB_OK;
+    if (undistort && f->undistort) return upload_undistorted(f, first, count, host, channels, frame_stride);
     // cudaMemcpyDefault: `host` may also be a device pointer (frames already resident in HBM, unified addressing).
     // A strided batch copy treats one image as a "row", so its pitch is limited (cudaDeviceProp::memPitch, 2^31 - 1):
     // longer strides (a stacked [stream][frame] array of thousands of frames) fall back to one copy per image.
@@ -446,7 +499,7 @@ int ygzb_frames_upload(ygzb_frames* f, int first, int count, const uint8_t* host
                 YGZB_CUDA(ctx, cudaMemcpy2DAsync(dst + (size_t)i * ctx->slot_stride, g.lv[0].pitch, host + (size_t)i * frame_stride,
                                                  row, row, g.lv[0].h, cudaMemcpyDefault, ctx->stream));
         }
-        return launch_pyramid(f, first, count, nullptr);
+        return launch_pyramid(f, first, count, nullptr, 1, false);
     }
     uint8_t* d_bgr = (uint8_t*)dev_scratch(ctx, 0, (size_t)count * row * g.lv[0].h);
     if (!d_bgr) return YGZB_ERR_CUDA;
@@ -458,7 +511,95 @@ int ygzb_frames_upload(ygzb_frames* f, int first, int count, const uint8_t* host
             YGZB_CUDA(ctx, cudaMemcpyAsync(d_bgr + (size_t)i * row * g.lv[0].h, host + (size_t)i * frame_stride, row * g.lv[0].h,
                                            cudaMemcpyDefault, ctx->stream));
     }
-    return launch_pyramid(f, first, count, d_bgr);
+    return launch_pyramid(f, first, count, d_bgr, 3, false);
+}
+
+extern "C" {
+
+int ygzb_frames_upload(ygzb_frames* f, int first, int count, const uint8_t* host, int channels, size_t frame_stride) {
+    return frames_upload(f, first, count, host, channels, frame_stride, true);
+}
+
+int ygzb_frames_set_undistort(ygzb_frames* f, const int16_t* map_xy, const uint16_t* map_a) {
+    if (!f) return YGZB_ERR_INVALID;
+    ygzb_ctx* ctx = f->ctx;
+    if (!map_xy != !map_a) return set_error(ctx, YGZB_ERR_INVALID, "set_undistort: map_xy and map_a must both be given, or both be NULL");
+    cudaSetDevice(ctx->device);
+    if (!map_xy) {   // uploads in flight keep reading the maps, which stay allocated until the pool is destroyed
+        f->undistort = false;
+        return YGZB_OK;
+    }
+    // the maps are read into host memory and checked before anything of the pool changes
+    const size_t n = (size_t)ctx->geo.W * ctx->geo.H;
+    std::vector<int16_t> xy(2 * n);
+    std::vector<uint16_t> a(n);
+    YGZB_CUDA(ctx, cudaMemcpy(xy.data(), map_xy, 2 * n * sizeof(int16_t), cudaMemcpyDefault));
+    YGZB_CUDA(ctx, cudaMemcpy(a.data(), map_a, n * sizeof(uint16_t), cudaMemcpyDefault));
+    for (size_t i = 0; i < n; ++i)
+        if (a[i] >= 1024)
+            return set_error(ctx, YGZB_ERR_INVALID, "set_undistort: map_a[%zu] = %d is not a 5 + 5-bit fraction (< 1024)", i, (int)a[i]);
+    if (!f->e_stage) YGZB_CUDA(ctx, cudaEventCreateWithFlags(&f->e_stage, cudaEventDisableTiming));
+    if (!f->d_map_xy) YGZB_CUDA(ctx, cudaMalloc((void**)&f->d_map_xy, n * sizeof(short2)));
+    if (!f->d_map_a) YGZB_CUDA(ctx, cudaMalloc((void**)&f->d_map_a, n * sizeof(uint16_t)));
+    // behind the last remap (which may still read the old maps, on a tracker's front stream), and complete on return
+    YGZB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, f->e_stage, 0));
+    YGZB_CUDA(ctx, cudaMemcpyAsync(f->d_map_xy, xy.data(), 2 * n * sizeof(int16_t), cudaMemcpyHostToDevice, ctx->stream));
+    YGZB_CUDA(ctx, cudaMemcpyAsync(f->d_map_a, a.data(), n * sizeof(uint16_t), cudaMemcpyHostToDevice, ctx->stream));
+    YGZB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    f->undistort = true;
+    return YGZB_OK;
+}
+
+// cv::initUndistortRectifyMap(K, D, R = I, newK, size, CV_16SC2) (OpenCV modules/calib3d, undistort), restated as OpenCV's
+// x86-64 build computes it (its AVX2 + FMA code path, 8 columns per step): the inverse of newK by the cofactor formula of
+// cv::invert for 3x3; per row the ray start _y = fma(i, iR11, iR12); per column _x = start of its group of 8 (advanced by
+// 8 iR00 per group) + k iR00, the columns after the last full group advanced by iR00 one by one; then the radial-tangential
+// model with its multiply-adds fused as OpenCV's vector code fuses them, projection with K, rounding to 1/32 pixel (cvRound:
+// half to even) and the split into the integer pixel and the 5 + 5-bit fraction.  Every other step is one IEEE double
+// operation (the host build does not contract them).  The fusing matters at exact ties only: on the TUM and EuRoC cameras the
+// plain sums give the same maps.
+int ygzb_undistort_map(int width, int height, const double K[4], const double dist[5], const double newK[4], int16_t* map_xy,
+                       uint16_t* map_a) {
+    if (width < 1 || height < 1 || width > 32767 || height > 32767 || !K || !dist || !map_xy || !map_a) return YGZB_ERR_INVALID;
+    const double* A = newK ? newK : K;
+    const double afx = A[0], afy = A[1], acx = A[2], acy = A[3];
+    if (!(afx * afy != 0.0)) return YGZB_ERR_INVALID;
+    // iR = newK^-1 (cv::invert, DECOMP_LU, 3x3: d = 1 / det3, cofactors times d), the zero entries dropped
+    const double d = 1.0 / (afx * afy);
+    const double ir0 = afy * d, ir2 = -(acx * afy) * d, ir4 = afx * d, ir5 = -(afx * acy) * d, ir8 = (afx * afy) * d;
+    const double fx = K[0], fy = K[1], u0 = K[2], v0 = K[3];
+    const double k1 = dist[0], k2 = dist[1], p1 = dist[2], p2 = dist[3], k3 = dist[4];
+    const double w = 1.0 / ir8;
+    std::vector<double> xs(width);
+    {
+        double base = ir2;
+        const int full = width / 8 * 8;
+        for (int j = 0; j < full; j += 8, base += 8 * ir0)
+            for (int k = 0; k < 8; ++k) xs[j + k] = base + k * ir0;
+        for (int j = full; j < width; ++j, base += ir0) xs[j] = base;
+    }
+    for (int i = 0; i < height; ++i) {
+        const double y = std::fma((double)i, ir4, ir5) * w;
+        for (int j = 0; j < width; ++j) {
+            const double x = xs[j] * w;
+            const double x2 = x * x, y2 = y * y;
+            const double r2 = x2 + y2, _2xy = 2 * x * y;
+            const double kr = std::fma(std::fma(std::fma(k3, r2, k2), r2, k1), r2, 1.0);
+            const double xd = std::fma(p2, r2 + 2 * x2, std::fma(p1, _2xy, x * kr));
+            const double yd = std::fma(p2, _2xy, std::fma(p1, r2 + 2 * y2, y * kr));
+            const double u = std::fma(fx, xd, u0), v = std::fma(fy, yd, v0);
+            const double su = u * 32.0, sv = v * 32.0;
+            // saturate_cast<int>: round half to even, clamped to the int range (NaN: INT_MIN, as x86's cvtsd2si gives it)
+            const int iu = su >= 2147483647.0 ? INT32_MAX : (su <= -2147483648.0 || su != su) ? INT32_MIN : (int)std::nearbyint(su);
+            const int iv = sv >= 2147483647.0 ? INT32_MAX : (sv <= -2147483648.0 || sv != sv) ? INT32_MIN : (int)std::nearbyint(sv);
+            const size_t o = (size_t)i * width + j;
+            // saturate_cast<short> of the integer pixel: a ray that leaves the image far away must not wrap back into it
+            map_xy[2 * o] = (int16_t)std::min(std::max(iu >> 5, -32768), 32767);
+            map_xy[2 * o + 1] = (int16_t)std::min(std::max(iv >> 5, -32768), 32767);
+            map_a[o] = (uint16_t)((iv & 31) * 32 + (iu & 31));
+        }
+    }
+    return YGZB_OK;
 }
 
 int ygzb_frames_download_level(ygzb_frames* f, int slot, int level, uint8_t* host) {

@@ -93,6 +93,14 @@ struct ygzb_frames {
     int tma_levels;
     int32_t* d_offsets;               // [capacity+1]
     int last_n;
+    // lens undistortion (ygzb_frames_set_undistort): OpenCV fixed-point maps, [H][W] each, and the pool's own staging of the
+    // raw frames a remap reads (uploads run on the context's stream and on a tracker's front stream: no shared scratch)
+    bool undistort;                   // maps set: uploads remap level 0
+    short2* d_map_xy;
+    uint16_t* d_map_a;
+    uint8_t* d_stage;
+    size_t stage_bytes;
+    cudaEvent_t e_stage;              // recorded behind the last remap, on whichever stream ran it: reuse of d_stage waits for it
 };
 
 namespace ygzb {
@@ -144,7 +152,12 @@ struct ProfScope {
 };
 
 // ---- stage launchers (one .cu each) -----------------------------------------------------------
-int launch_pyramid(ygzb_frames* f, int first, int count, const uint8_t* d_bgr /* or null */);
+// d_src = raw frames staged on the device (`channels` 1 or 3) or null (level 0 already in the slots); remap: level 0 =
+// remap_gray_kernel of d_src through the pool's undistortion maps, otherwise d_src must be BGR (bgr2gray_kernel)
+int launch_pyramid(ygzb_frames* f, int first, int count, const uint8_t* d_src, int channels, bool remap);
+// ygzb_frames_upload; undistort = false skips the pool's undistortion maps (images that are undistorted already, e.g. the
+// key-frame and reference images of the tracker's records)
+int frames_upload(ygzb_frames* f, int first, int count, const uint8_t* host, int channels, size_t frame_stride, bool undistort);
 int launch_pyrdown_ptrs(ygzb_ctx* ctx, const uint8_t* const* d_src_ptr, uint8_t* const* d_dst_ptr, int sw, int sh, int spitch,
                         int dw, int dh, int dpitch, int count);
 int launch_detect(ygzb_frames* f, int n, bool have_occupied);

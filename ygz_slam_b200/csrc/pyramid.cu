@@ -7,6 +7,10 @@
 //     gray = (B*3735 + G*19235 + R*9798 + 16384) >> 15
 //     pyrDown: separable [1 4 6 4 1], (sum + 128) >> 8, BORDER_REFLECT_101, dst = ((w+1)/2, (h+1)/2)
 //
+// With undistortion maps on the pool (ygzb_frames_set_undistort), level 0 is instead
+//     cv::remap(gray, map_xy, map_a, INTER_LINEAR, BORDER_CONSTANT, 0)      (remap_gray_kernel, the BGR conversion per tap)
+// of the raw frames staged in the pool's own buffer; the pyramid kernels are the same.
+//
 // Layout: every frame slot holds all levels back to back, each level pitch-linear with a 16-byte
 // multiple pitch (so level rows can be moved with 16-byte vectors / TMA boxes).
 // Roofline class: HBM.  Algorithmic bytes per frame (8 levels, grey in): 307,200 read + 102,400
@@ -249,13 +253,82 @@ __global__ void __launch_bounds__(256) bgr2gray_kernel(const uint8_t* __restrict
     }
 }
 
+// one tap of the remap: the grey value of source pixel (x, y), 0 outside the image (BORDER_CONSTANT, value 0); a BGR tap is
+// converted with bgr2gray_kernel's formula, so that the result is cv::remap(cv::cvtColor(image))
+template <int C>
+__device__ __forceinline__ int remap_tap(const uint8_t* __restrict__ img, int x, int y, int w, int h) {
+    if ((unsigned)x >= (unsigned)w || (unsigned)y >= (unsigned)h) return 0;
+    const uint8_t* p = img + ((size_t)y * w + x) * C;
+    if (C == 1) return p[0];
+    return (p[0] * 3735 + p[1] * 19235 + p[2] * 9798 + (1 << 14)) >> 15;
+}
+
+// one output pixel: source pixel (sx, sy), fraction a = (fy << 5) | fx
+template <int C>
+__device__ __forceinline__ uint8_t remap_pixel(const uint8_t* __restrict__ img, int sx, int sy, int a, int w, int h) {
+    const int fx = a & 31, fy = a >> 5;
+    const int p00 = remap_tap<C>(img, sx, sy, w, h), p01 = remap_tap<C>(img, sx + 1, sy, w, h);
+    const int p10 = remap_tap<C>(img, sx, sy + 1, w, h), p11 = remap_tap<C>(img, sx + 1, sy + 1, w, h);
+    const int sum = ((32 - fx) * (32 - fy) * p00 + fx * (32 - fy) * p01 + (32 - fx) * fy * p10 + fx * fy * p11) * 32;
+    return (uint8_t)((sum + (1 << 14)) >> 15);
+}
+
+// cv::remap(src, map_xy, map_a, INTER_LINEAR, BORDER_CONSTANT, 0) with OpenCV's fixed-point maps (CV_16SC2 + CV_16UC1), of a grey
+// (C = 1) or BGR (C = 3) frame, 4 adjacent output pixels per thread.  OpenCV's weight table entry (fy, fx) is
+//   32 * {(32 - fx)(32 - fy), fx (32 - fy), (32 - fx) fy, fx fy}        (the float products (1 - x)(1 - y) .. scaled by 2^15)
+// and the result (sum w p + 2^14) >> 15.  The products are exact, so the table is this formula, except entry 0, whose 32768
+// saturates to 32767 in OpenCV's int16 table before the rounding correction moves the missing unit to another tap; with 8-bit
+// taps that cannot change a result (32768 p0 + d + 2^14 with |d| <= 255 has the same quotient), so no table is read.
+template <int C>
+__global__ void __launch_bounds__(256) remap_gray_kernel(const uint8_t* __restrict__ src, size_t src_frame_stride,
+                                                         const short2* __restrict__ map_xy, const uint16_t* __restrict__ map_a,
+                                                         uint8_t* __restrict__ pyr, size_t slot_stride, int first_slot, LevelGeom l0) {
+    const int quads_per_row = (l0.w + 3) / 4;
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= quads_per_row * l0.h) return;
+    const int y = q / quads_per_row, x = (q - y * quads_per_row) * 4;
+    const uint8_t* img = src + (size_t)blockIdx.y * src_frame_stride;
+    const size_t m = (size_t)y * l0.w + x;
+    uint8_t* out = pyr + (size_t)(first_slot + blockIdx.y) * slot_stride + l0.off + (size_t)y * l0.pitch + x;
+    if (x + 3 < l0.w && (l0.w & 3) == 0) {
+        // m % 4 == 0: the four map pairs are one 16-byte load, the four fractions one 8-byte load; x % 4 == 0 and the
+        // level pitch is a multiple of 16: the four pixels are one 32-bit store
+        const int4 xy4 = *reinterpret_cast<const int4*>(map_xy + m);
+        const uint2 a4 = *reinterpret_cast<const uint2*>(map_a + m);
+        const int xy[4] = {xy4.x, xy4.y, xy4.z, xy4.w};
+        const unsigned a[4] = {a4.x & 0xFFFFu, a4.x >> 16, a4.y & 0xFFFFu, a4.y >> 16};
+        uint32_t packed = 0;
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+            packed |= (uint32_t)remap_pixel<C>(img, (short)(xy[j] & 0xFFFF), (short)(xy[j] >> 16), (int)a[j], l0.w, l0.h) << (8 * j);
+        *reinterpret_cast<uint32_t*>(out) = packed;
+        return;
+    }
+    for (int j = 0; j < 4 && x + j < l0.w; ++j) {
+        const short2 s = map_xy[m + j];
+        out[j] = remap_pixel<C>(img, s.x, s.y, map_a[m + j], l0.w, l0.h);
+    }
+}
+
 }  // namespace
 
-int launch_pyramid(ygzb_frames* f, int first, int count, const uint8_t* d_bgr) {
+int launch_pyramid(ygzb_frames* f, int first, int count, const uint8_t* d_src, int channels, bool remap) {
     ygzb_ctx* ctx = f->ctx;
     const Geometry& g = ctx->geo;
     if (count <= 0) return YGZB_OK;
-    if (d_bgr) {
+    if (d_src && remap) {
+        // undistortion (ygzb_frames_set_undistort): level 0 = remap of the staged raw frames, in place of bgr2gray_kernel
+        const int quads = ((g.lv[0].w + 3) / 4) * g.lv[0].h;
+        const size_t frame = (size_t)g.lv[0].w * g.lv[0].h * channels;
+        dim3 grid((quads + 255) / 256, count);
+        ProfScope ps(ctx, kStageBgr2Gray);
+        if (channels == 3)
+            remap_gray_kernel<3><<<grid, 256, 0, ctx->stream>>>(d_src, frame, f->d_map_xy, f->d_map_a, f->d_pyr, ctx->slot_stride, first, g.lv[0]);
+        else
+            remap_gray_kernel<1><<<grid, 256, 0, ctx->stream>>>(d_src, frame, f->d_map_xy, f->d_map_a, f->d_pyr, ctx->slot_stride, first, g.lv[0]);
+        YGZB_LAUNCHED(ctx);
+    } else if (d_src) {
+        const uint8_t* d_bgr = d_src;
         const int quads = ((g.lv[0].w + 3) / 4) * g.lv[0].h;
         dim3 grid((quads + 255) / 256, count);
         ProfScope ps(ctx, kStageBgr2Gray);

@@ -1234,7 +1234,8 @@ int ygzb_tracker_import(ygzb_tracker* t, int stream, const int32_t* entries, con
         YGZB_LAUNCHED(ctx);
     }
     const size_t WH = (size_t)st.W * st.H;
-    for (int k = 0; k < n && rc == YGZB_OK; ++k) rc = ygzb_frames_upload(t->f, kf_slots[k], 1, in->image + k * WH, 1, WH);
+    // the record's images are level 0 of key-frames, undistorted already: the pool's undistortion maps must not warp them again
+    for (int k = 0; k < n && rc == YGZB_OK; ++k) rc = frames_upload(t->f, kf_slots[k], 1, in->image + k * WH, 1, WH, false);
     if (rc == YGZB_OK) rc = check_cuda(ctx, cudaEventRecord(t->e_fill, ctx->stream), "cudaEventRecord");
     return rc;
 }
@@ -1313,7 +1314,7 @@ int ygzb_tracker_import_reference(ygzb_tracker* t, int stream, const ygzb_refere
         YGZB_LAUNCHED(ctx);
     }
     const size_t WH = (size_t)st.W * st.H;
-    rc = ygzb_frames_upload(t->f, t->ref_slots[stream], 1, in->image, 1, WH);
+    rc = frames_upload(t->f, t->ref_slots[stream], 1, in->image, 1, WH, false);   // undistorted already, like a map record's images
     if (rc == YGZB_OK) rc = check_cuda(ctx, cudaEventRecord(t->e_fill, ctx->stream), "cudaEventRecord");
     if (rc != YGZB_OK) return rc;
     t->cur_ref[stream] = t->ref_slots[stream];

@@ -107,7 +107,15 @@ struct MapPoint {  // include/ygz/Basic/MapPoint.h:17-46 (fields used on the hot
 
 class PinholeCamera {  // include/ygz/Basic/Camera.h:10-112
   public:
-    PinholeCamera(float fx = 520.9f, float fy = 521.0f, float cx = 325.1f, float cy = 249.7f) : _fx(fx), _fy(fy), _cx(cx), _cy(cy) {}
+    PinholeCamera(float fx = 520.9f, float fy = 521.0f, float cx = 325.1f, float cy = 249.7f, float k1 = 0.f, float k2 = 0.f, float p1 = 0.f,
+                  float p2 = 0.f)
+        : _fx(fx), _fy(fy), _cx(cx), _cy(cy), _k1(k1), _k2(k2), _p1(p1), _p2(p2) {}
+    // camera.k1 k2 p1 p2 (Camera.h:19-22): the radial-tangential model of UndistortPoint (:96-104).  The reference stores
+    // them and never applies them; b200::Runtime::SetUndistortion(camera) undistorts every later InitFrame with them.
+    float k1() const { return _k1; }
+    float k2() const { return _k2; }
+    float p1() const { return _p1; }
+    float p2() const { return _p2; }
     Vector3d World2Camera(const Vector3d& p_w, const SE3& T_c_w) const { return T_c_w * p_w; }
     Vector2d Camera2Pixel(const Vector3d& p) const { return Vector2d(_fx * p[0] / p[2] + _cx, _fy * p[1] / p[2] + _cy); }
     Vector2d World2Pixel(const Vector3d& p_w, const SE3& T) const { return Camera2Pixel(World2Camera(p_w, T)); }
@@ -121,6 +129,7 @@ class PinholeCamera {  // include/ygz/Basic/Camera.h:10-112
     float cy() const { return _cy; }
   protected:
     float _fx, _fy, _cx, _cy;
+    float _k1, _k2, _p1, _p2;
 };
 
 class ORBVocabulary;
@@ -220,6 +229,24 @@ class Runtime {
         }
     }
     int FreeSlots() const { return (int)free_.size(); }
+    // undistort every later Frame::InitFrame with the camera's k1 k2 p1 p2 (k3 = 0, the model of Camera.h:96-104): the maps of
+    // cv::initUndistortRectifyMap(K, D, I, K) are built on the host (ygzb_undistort_map) and set on the pool
+    // (ygzb_frames_set_undistort).  The undistorted camera keeps K, so the same PinholeCamera projects the undistorted
+    // frames.  A camera without distortion clears the maps.
+    void SetUndistortion(const PinholeCamera& cam) {
+        Ensure();
+        if (cam.k1() == 0.f && cam.k2() == 0.f && cam.p1() == 0.f && cam.p2() == 0.f) {
+            Check(ygzb_frames_set_undistort(frames_, nullptr, nullptr), "ygzb_frames_set_undistort");
+            return;
+        }
+        const int w = params_.image_width, h = params_.image_height;
+        const double K[4] = {cam.fx(), cam.fy(), cam.cx(), cam.cy()};
+        const double D[5] = {cam.k1(), cam.k2(), cam.p1(), cam.p2(), 0.0};
+        std::vector<int16_t> xy((size_t)w * h * 2);
+        std::vector<uint16_t> a((size_t)w * h);
+        Check(ygzb_undistort_map(w, h, K, D, nullptr, xy.data(), a.data()), "ygzb_undistort_map");
+        Check(ygzb_frames_set_undistort(frames_, xy.data(), a.data()), "ygzb_frames_set_undistort");
+    }
     void Check(int rc, const char* what) {
         if (rc != YGZB_OK) throw Error(std::string(what) + ": " + (ctx_ ? ygzb_last_error(ctx_) : "?"));
     }

@@ -107,6 +107,66 @@ def render_plane(tex: np.ndarray, T_cw: np.ndarray, plane_z: float = 2.0, metres
     return gray, d  # depth along the optical axis (ray z component is 1)
 
 
+def undistort_rays(u, v, dist, fx: float = FX, fy: float = FY, cx: float = CX, cy: float = CY, iters: int = 30):
+    """Normalised rays (x, y) whose radial-tangential projection (k1, k2, p1, p2, k3) through K is the pixel (u, v):
+    fixed-point iteration x = (xd - tangential(x, y)) / radial(x, y), as cv::undistortPoints does."""
+    k1, k2, p1, p2, k3 = (tuple(dist) + (0.0,) * 5)[:5]
+    xd, yd = (u - cx) / fx, (v - cy) / fy
+    x, y = xd.copy(), yd.copy()
+    for _ in range(iters):
+        r2 = x * x + y * y
+        kr = 1 + ((k3 * r2 + k2) * r2 + k1) * r2
+        x = (xd - (2 * p1 * x * y + p2 * (r2 + 2 * x * x))) / kr
+        y = (yd - (p1 * (r2 + 2 * y * y) + 2 * p2 * x * y)) / kr
+    return x, y
+
+
+def render_plane_lens(tex: np.ndarray, T_cw: np.ndarray, dist, plane_z: float = 2.0, metres_per_texel: float = 0.0025,
+                      noise_sigma: float = 0.0, seed: int = 1):
+    """render_plane through a lens: the camera K = (FX, FY, CX, CY) with radial-tangential distortion dist = (k1, k2, p1, p2[,
+    k3]).  Every distorted pixel is undistorted iteratively to its ray, the ray is intersected with the plane z = plane_z and
+    the texture is sampled there.  Returns (raw distorted gray uint8 HxW, depth HxW of the UNDISTORTED pinhole camera with
+    the same K -- the depth map a tracker wants once its frame pool undistorts with newK = K)."""
+    R, t = T_cw[:, :3], T_cw[:, 3]
+    u, v = np.meshgrid(np.arange(W, dtype=np.float64), np.arange(H, dtype=np.float64))
+    x, y = undistort_rays(u, v, dist)
+    cw = -R.T @ t
+
+    def hit(rx, ry):
+        rw = np.stack([rx, ry, np.ones_like(rx)], -1) @ R
+        d = (plane_z - cw[2]) / rw[..., 2]
+        return cw + d[..., None] * rw, d
+
+    Xw, _ = hit(x, y)
+    size = tex.shape[0]
+    tx = np.clip(Xw[..., 0] / metres_per_texel + size / 2, 0, size - 1.001)
+    ty = np.clip(Xw[..., 1] / metres_per_texel + size / 2, 0, size - 1.001)
+    x0, y0 = tx.astype(np.int32), ty.astype(np.int32)
+    fx, fy = tx - x0, ty - y0
+    tf = tex.astype(np.float64)
+    val = ((1 - fy) * ((1 - fx) * tf[y0, x0] + fx * tf[y0, x0 + 1]) + fy * ((1 - fx) * tf[y0 + 1, x0] + fx * tf[y0 + 1, x0 + 1]))
+    if noise_sigma > 0:
+        val = val + np.random.default_rng(seed).normal(0, noise_sigma, val.shape)
+    gray = np.clip(np.rint(val), 0, 255).astype(np.uint8)
+    _, depth = hit((u - CX) / FX, (v - CY) / FY)
+    return gray, depth
+
+
+# TUM fr2's coefficients (k1, k2, p1, p2, k3): the lens of the lens-rendered streams
+LENS_TUM_FR2 = (0.2312, -0.7849, -0.0033, -0.0001, 0.9172)
+
+
+def lens_stream_frame(k: int, stream: int = 0, dist=LENS_TUM_FR2, noise_sigma: float = 2.0, tex_size: int = 2048):
+    """Frame k of synthetic stream `stream` (the trajectory of stream_frame) seen through the lens `dist`: (raw distorted
+    gray, depth of the undistorted camera, T_cw)."""
+    key = (stream, tex_size)
+    if key not in _TEX_CACHE:
+        _TEX_CACHE[key] = texture(0x59475A00 + stream, tex_size)
+    T = trajectory(k)
+    gray, depth = render_plane_lens(_TEX_CACHE[key], T, dist, noise_sigma=noise_sigma, seed=(stream << 16) + k + 1)
+    return gray, depth, T
+
+
 _TEX_CACHE: dict = {}
 
 

@@ -333,9 +333,13 @@ def _map_points(keyframes, ids):
 class GpuBackend:
     """Every call = one batched C-ABI call on the rank's context (ygz_slam_b200.capi)."""
 
-    def __init__(self, ctx, n_slots: int):
+    def __init__(self, ctx, n_slots: int, undistort=None):
+        """undistort: (map_xy, map_a) of capi.undistort_map / cv2.initUndistortRectifyMap(.., CV_16SC2), or None.  With maps
+        every frame is undistorted on the device as it is uploaded, and the loop's camera is the undistorted one."""
         self.ctx = ctx
         self.fr = ctx.frames(n_slots)
+        if undistort is not None:
+            self.fr.set_undistort(*undistort)
 
     def upload(self, slots, images):
         imgs = np.ascontiguousarray(np.stack(images))
