@@ -89,18 +89,8 @@ def _pose_err(Ta, Tb):
     return float(np.linalg.norm(se3.se3_log(se3.mul(se3.inv(Ta), Tb))))
 
 
-def _select_generation(monkeypatch, gen):
-    """ygzb_sparse_align runs the second-generation kernel (the tracker's) unless YGZB_SPARSE_GEN1 is set."""
-    if gen == 1:
-        monkeypatch.setenv("YGZB_SPARSE_GEN1", "1")
-    else:
-        monkeypatch.delenv("YGZB_SPARSE_GEN1", raising=False)
-
-
-@pytest.mark.parametrize("levels,max_level,gen", [(3, 2, 2), (8, 3, 2), (3, 2, 1), (8, 3, 1)],
-                         ids=["3-2", "8-3", "3-2-gen1", "8-3-gen1"])
-def test_sparse_align_pose_tolerance(levels, max_level, gen, ctx3, ctx8, oracle, monkeypatch):
-    _select_generation(monkeypatch, gen)
+@pytest.mark.parametrize("levels,max_level", [(3, 2), (8, 3)], ids=["3-2", "8-3"])
+def test_sparse_align_pose_tolerance(levels, max_level, ctx3, ctx8, oracle):
     ctx = ctx3 if levels == 3 else ctx8
     s = _scene(oracle, levels=levels)
     s2 = _scene(oracle, 2, 5, levels=levels)
@@ -156,16 +146,9 @@ def test_align1d_bit_exact(ctx3, oracle):
     fr.close()
 
 
-def test_alignment_and_klt_on_another_geometry(oracle, monkeypatch):
+def test_alignment_and_klt_on_another_geometry(oracle):
     """752 x 480, 4 levels (not the 640 x 480 default): FindDirectProjection bit-exact, SparseImgAlign and KLT within
     their tolerances -- the level geometry (pitches, offsets, borders) is a run-time parameter everywhere."""
-    _select_generation(monkeypatch, 2)
-    _another_geometry(oracle)
-
-
-def test_sparse_align_first_generation_on_another_geometry(oracle, monkeypatch):
-    """The same 752 x 480, 4-level checks with YGZB_SPARSE_GEN1: the first-generation sparse-alignment kernel."""
-    _select_generation(monkeypatch, 1)
     _another_geometry(oracle)
 
 
@@ -215,15 +198,13 @@ def _another_geometry(oracle):
         ctx.close()
 
 
-@pytest.mark.parametrize("gen", [2, 1])
-def test_sparse_align_global_staging_batch(ctx3, oracle, gen, monkeypatch):
+def test_sparse_align_global_staging_batch(ctx3, oracle):
     """One batch of 6,000 features, none, and 800 features (random pixels of the rendered frames with their rendered depth,
-    map-point masks with holes).  The second-generation kernel runs 4 CTAs per problem and stages a CTA's features in shared
+    map-point masks with holes).  The kernel runs 4 CTAs per problem and stages a CTA's features in shared
     memory up to (227 KB - 8 KB of static arrays) / 360 B per record = 622 features: the 6,000-feature problem (1,500 per
     CTA) stages in the global scratch, the 800-feature one (200 per CTA) in shared memory, and the empty one returns at once.
     Every pose within 1e-4 of the oracle, identical measurement counts, iterations reported per level, and two calls are
     bit-identical (each CTA sums its features in order, the cluster adds the CTA partials in rank order)."""
-    _select_generation(monkeypatch, gen)
     g1, d1, T1 = synth.stream_frame(1)
     g2, _, _ = synth.stream_frame(4)
     g3, d3, T3 = synth.stream_frame(2)

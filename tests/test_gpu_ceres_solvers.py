@@ -1,7 +1,6 @@
-"""The Ceres-flavoured solvers of ba.cu step by step against oracle/ba.cpp: local_ba_kernel<true> (ygzb_local_ba_ceres and
-ygzb_two_view_ba) truncated after k trials and on every termination path, pose_only_kernel (ygzb_pose_only, the tracking
-loop's refinement) at its frame-size, inlier-count, threshold and behind-the-camera edges, and local_ba_kernel<false>
-(the g2o kernel selected by YGZB_BA_GEN1).
+"""The Ceres-flavoured solvers of ba.cu step by step against oracle/ba.cpp: local_ba_kernel (ygzb_local_ba_ceres and
+ygzb_two_view_ba) truncated after k trials and on every termination path, and pose_only_kernel (ygzb_pose_only, the tracking
+loop's refinement) at its frame-size, inlier-count, threshold and behind-the-camera edges.
 
 The tests without the gpu mark check on the oracle alone that every constructed case reaches the branch it is built for, so
 that the GPU comparisons keep testing that branch and not merely convergence."""
@@ -29,11 +28,6 @@ def _t_aa(v):  # se3 log [upsilon; omega] -> [t; angle-axis] (the pose block of 
         T = se3.se3_exp(x)
         out.append(np.r_[T[:, 3], se3.so3_log(T[:, :3])])
     return np.array(out)
-
-
-def _g2o(v):
-    v = np.asarray(v)
-    return np.concatenate([v[..., 3:], v[..., :3]], -1)
 
 
 def _fixed(n_kf, *idx):
@@ -537,65 +531,3 @@ def _two_view_batch(ctx3, oracle, pr, names):
             assert np.abs(X[sl] - wX).max() < 1e-4, name
         assert (st[p]["iters"], st[p]["termination"]) == (wst["iters"], wst["termination"]), (name, st[p], wst)
         assert abs(st[p]["cost_final"] - wst["cost_final"]) < 1e-9 * wst["cost_final"] + 1e-15, name
-
-
-# ---- YGZB_BA_GEN1: local_ba_kernel<false> ---------------------------------------------------------------------------------
-def _pose_diff(Pa, Pb):
-    worst = 0.0
-    for a, b in zip(Pa, Pb):
-        Ta, Tb = se3.se3_exp(np.r_[a[3:], a[:3]]), se3.se3_exp(np.r_[b[3:], b[:3]])
-        worst = max(worst, float(np.linalg.norm(se3.se3_log(se3.mul(se3.inv(Ta), Tb)))))
-    return worst
-
-
-def _check_g2o(oracle, res, sc, fixed, huber=5.991, well=None):
-    P, X, out, st = res
-    wP, wX, wout, wst = oracle.local_ba(_g2o(sc["poses_noisy"]), fixed, sc["pts_noisy"], sc["kf_idx"], sc["pt_idx"], sc["px"], huber=huber)
-    well = np.arange(len(wX)) if well is None else well
-    assert _pose_diff(P, wP) < 1e-4
-    assert np.abs(X[well] - wX[well]).max() < 1e-4 and np.isfinite(X).all()
-    assert abs(st["chi2_final"] - wst["chi2_final"]) <= 1e-6 * wst["chi2_final"]
-    assert (out != wout).sum() <= 2
-
-
-@gpu
-@pytest.mark.parametrize("huber", [5.991, 0.0])
-def test_gen1_c4(ctx3, oracle, huber, monkeypatch):
-    monkeypatch.setenv("YGZB_BA_GEN1", "1")
-    sc = synth.ba_scene()
-    f = _fixed(10)
-    n_obs = len(sc["kf_idx"])
-    P, X, out, st = ctx3.local_ba([0, 10], [0, 2000], [0, n_obs], _g2o(sc["poses_noisy"]), f, sc["pts_noisy"], sc["kf_idx"], sc["pt_idx"],
-                                  sc["px"], huber=huber)
-    _check_g2o(oracle, (P, X, out, st[0]), sc, f, huber)
-    assert st[0]["iters"] >= 5
-
-
-@gpu
-def test_gen1_batched_and_edge_scene(ctx3, oracle, monkeypatch):
-    """C4 with a 6-key-frame problem that has two fixed key-frames, and the edge scene with an empty problem, through the
-    g2o kernel; a landmark observed twice by one free key-frame is rejected as by ygzb_local_ba's default kernel."""
-    from ygz_slam_b200.capi import YgzbError
-    monkeypatch.setenv("YGZB_BA_GEN1", "1")
-    a = synth.ba_scene(n_kf=10, n_pt=2000, target_obs=8000, seed=11)
-    b = synth.ba_scene(n_kf=6, n_pt=300, target_obs=1500, seed=12)
-    e = synth.ba_edge_scene()
-    empty = synth.ba_scene(n_kf=3, n_pt=20, seed=42)
-    empty.update(kf_idx=np.zeros(0, np.int32), pt_idx=np.zeros(0, np.int32), px=np.zeros((0, 2)))
-    scs, fixeds = [a, b, e, empty], [_fixed(10), _fixed(6, 0, 4), _fixed(6, 0, 1), _fixed(3)]
-    kf_off = np.cumsum([0] + [len(f) for f in fixeds])
-    pt_off = np.cumsum([0] + [len(s["pts_noisy"]) for s in scs])
-    obs_off = np.cumsum([0] + [len(s["kf_idx"]) for s in scs])
-    P, X, out, st = ctx3.local_ba(kf_off, pt_off, obs_off, np.concatenate([_g2o(s["poses_noisy"]) for s in scs]), np.concatenate(fixeds),
-                                  np.concatenate([s["pts_noisy"] for s in scs]), np.concatenate([s["kf_idx"] for s in scs]),
-                                  np.concatenate([s["pt_idx"] for s in scs]), np.concatenate([s["px"] for s in scs]))
-    res = [(P[kf_off[i]:kf_off[i + 1]], X[pt_off[i]:pt_off[i + 1]], out[obs_off[i]:obs_off[i + 1]], st[i]) for i in range(4)]
-    _check_g2o(oracle, res[0], a, fixeds[0])
-    _check_g2o(oracle, res[1], b, fixeds[1])
-    _check_g2o(oracle, res[2], e, fixeds[2], well=np.setdiff1d(np.arange(380), e["single"]))
-    assert np.array_equal(res[1][0][[0, 4]], _g2o(b["poses_noisy"])[[0, 4]])
-    assert _pose_diff(res[3][0], _g2o(empty["poses_noisy"])) < 1e-12 and np.allclose(res[3][1], empty["pts_noisy"], rtol=0, atol=1e-12)
-    q = int(np.flatnonzero((b["pt_idx"] == 0) & (b["kf_idx"] > 0) & (b["kf_idx"] != 4))[0])
-    kf_idx, pt_idx, px = np.insert(b["kf_idx"], q, b["kf_idx"][q]), np.insert(b["pt_idx"], q, 0), np.insert(b["px"], q, b["px"][q] + 0.5, 0)
-    with pytest.raises(YgzbError, match=r"rc=-1\).*observed twice"):
-        ctx3.local_ba([0, 6], [0, 300], [0, len(kf_idx)], _g2o(b["poses_noisy"]), fixeds[1], b["pts_noisy"], kf_idx, pt_idx, px)

@@ -1,14 +1,16 @@
-// ba2.cu -- ba::LocalBAG2O, second generation: a landmark-partitioned thread-block cluster per problem.
+// ba2.cu -- ba::LocalBAG2O (ygzb_local_ba and the tracking engine's local BA): a landmark-partitioned thread-block cluster
+// per problem.
 //
-// Replaces (same maths as the first-generation kernel in ba.cu, which stays in service for the Ceres twin):
+// Replaces:
 //   ba::LocalBAG2O                   reference src/Algorithm/BA.cpp:386-543
 //   VertexSE3Sophus::oplusImpl       reference include/ygz/G2oTypes.h:38-45
 //   EdgeSophusSE3ProjectXYZ          reference include/ygz/G2oTypes.h:84-132 (computeError, linearizeOplus)
 // g2o itself is outside the reference tree: the Levenberg schedule follows oracle/ba.cpp (SURVEY.md appendix A.3).
 //
-// Why a second generation: the first one strides observations over the cluster, keeps a 21-double linearisation record
-// per observation in global memory that every CTA reads through L2 (__ldcg), combines partial sums with f64 atomics and
-// crosses ~13 cluster barriers per LM trial; its issue slots sat mostly idle.
+// Why it is organised differently from the Ceres kernel in ba.cu: that layout strides observations over the cluster, keeps a
+// 21-double linearisation record per observation in global memory that every CTA reads through L2 (__ldcg) and combines
+// partial sums with f64 atomics; running this solver, it crossed ~13 cluster barriers per LM trial and its issue slots sat
+// mostly idle.
 // Here
 //   * the LANDMARKS are partitioned over the CTAs of the cluster (contiguous ranges of the landmark-major observation
 //     list), so everything a landmark needs -- its observations, Hll, bl, (Hll + lambda I)^-1, the 6-double

@@ -1,4 +1,4 @@
-// ba2.cuh -- interface of the second-generation local BA (ba2.cu), shared with the C-ABI marshalling (ba.cu) and the
+// ba2.cuh -- interface of the g2o-flavoured local BA (ba2.cu), shared with the C-ABI marshalling (ba.cu) and the
 // device-resident tracking engine (track.cu).
 #pragma once
 

@@ -182,13 +182,10 @@ int launch_project_align(ygzb_frames* f, int n, const int32_t* d_ref_slot, const
 int launch_sparse_align(ygzb_frames* f, int n_problems, const int32_t* d_ref_slot, const int32_t* d_cur_slot,
                         const int32_t* d_offsets, const double* d_px, const double* d_depth, const uint8_t* d_has_mp,
                         const double* d_T_ref, double* d_T_cur, int max_level, int min_level, int n_iter, double eps,
-                        int32_t* d_n_meas, int32_t* d_iters, float* d_ref_patch, float* d_gdx, float* d_gdy, double* d_frame_jac,
-                        uint8_t* d_visible, double* d_ws, void* d_feat_scratch, size_t feat_stride);
-// YGZB_SPARSE_GEN1 set: the first-generation kernel, which uses d_ref_patch .. d_ws (size sparse_align_ws_doubles).  Otherwise
-// the second-generation kernel on kTrackCluster CTAs per problem, which uses only d_feat_scratch: feat_stride bytes per problem,
-// at least sparse_align2_scratch_bytes(1, features of the largest problem).
-bool sparse_align_gen1();
-size_t sparse_align_ws_doubles(int n_problems);
+                        int32_t* d_n_meas, int32_t* d_iters, void* d_feat_scratch, size_t feat_stride);
+// sparse_align2_kernel on kTrackCluster CTAs per problem.  d_feat_scratch holds feat_stride bytes per problem, at least
+// sparse_align2_scratch_bytes(1, features of the largest problem): the global fall-back for CTAs whose share of the features
+// does not fit shared memory.
 size_t sparse_align2_scratch_bytes(int n_problems, int max_features);
 constexpr int kTrackCluster = 4;   // CTAs per problem of the tracker's sparse alignment and pose-only (YGZB_TRACK_CLUSTER: 1, 2, 4 or 8)
 

@@ -651,12 +651,6 @@ size_t ref_store_bytes(const TrackStore& st) {
     return (c.bytes() + 255) & ~(size_t)255;
 }
 
-void wave_scratch(Carver& c, TrackBatch& b, size_t F, int S, int ref_cap) {
-    b.ref_patch = c.take<float>(F * 16); b.gdx = c.take<float>(F * 16); b.gdy = c.take<float>(F * 16);
-    b.frame_jac = c.take<double>(F * 12); b.visible = c.take<uint8_t>(F);
-    b.sa2_scratch = c.take<double>(sparse_align2_scratch_bytes(S, ref_cap) / 8 + 1);
-}
-
 // ygzb_tracker_track in YGZB_TRACK_REF_PREVIOUS mode.  A stream's jobs are tracked in batch order, each against the one
 // before it (its first against the stream's reference).  The batch runs in waves (wave w = the w-th job of every stream),
 // each wave the whole chain -- sparse alignment, candidates, direct projection, pose-only -- followed by the kernel that
@@ -695,10 +689,8 @@ int track_previous(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, ygzb
     b.prev = 1;
     b.job_ref_slot = t->d_aux;
     b.orig = t->d_aux + t->max_jobs;
-    {   // the sparse alignment's per-feature scratch, for ref_cap features per problem (a wave has at most one job per stream)
-        Carver c(static_cast<uint8_t*>(t->d_ref) + ref_store_bytes(t->st));
-        wave_scratch(c, b, (size_t)S * t->st.ref_cap, S, t->st.ref_cap);
-    }
+    // the sparse alignment's per-feature scratch, for ref_cap features per problem (a wave has at most one job per stream)
+    b.sa2_scratch = static_cast<uint8_t*>(t->d_ref) + ref_store_bytes(t->st);
     t->last_J = n_jobs;
     const int cl = t->cluster;
     // uploads ran on the front stream; a key-frame insertion (and its BA) is on this stream already
@@ -777,7 +769,7 @@ int ygzb_tracker_create(ygzb_frames* f, int n_streams, int max_jobs, const doubl
     if (rc == YGZB_OK) rc = dalloc(ctx, &t->d_depth, S * g.W * g.H);
     st.depth_map = t->d_depth;
     if (rc == YGZB_OK) {
-        const size_t J = (size_t)max_jobs, F = J * cells, Cn = J * cap;
+        const size_t J = (size_t)max_jobs, Cn = J * cap;
         TrackBatch& b = t->b;
         b.J = 0;
         b.cap = (int)cap;
@@ -786,9 +778,6 @@ int ygzb_tracker_create(ygzb_frames* f, int n_streams, int max_jobs, const doubl
             b.ref_slot = c.take<int32_t>(J); b.cur_slot = c.take<int32_t>(J); b.offsets = c.take<int32_t>(J + 1); b.in_off = c.take<int32_t>(J);
             b.n_feat = c.take<int32_t>(J); b.n_meas = c.take<int32_t>(J);
             b.T_ref = c.take<double>(J * 12); b.T_cur = c.take<double>(J * 12); b.T_aligned = c.take<double>(J * 12);
-            b.ref_patch = c.take<float>(F * 16); b.gdx = c.take<float>(F * 16); b.gdy = c.take<float>(F * 16);
-            b.frame_jac = c.take<double>(F * 12); b.visible = c.take<uint8_t>(F);
-            b.sparse_ws = c.take<double>(sparse_align_ws_doubles((int)J));
             b.sa2_scratch = c.take<double>(sparse_align2_scratch_bytes((int)J, (int)cells) / 8 + 1);
             b.aligned = c.take<int32_t>(J); b.rel = c.take<double>(J * kTrackMaxLocal * 12);
             b.cand_ok = c.take<uint8_t>(Cn); b.cand_px = c.take<double>(Cn * 2); b.n_cand = c.take<int32_t>(J);
@@ -886,11 +875,8 @@ int ygzb_tracker_set_reference_mode(ygzb_tracker* t, int mode, const int32_t* re
     if (mode == YGZB_TRACK_REF_PREVIOUS && !t->d_ref) {
         TrackStore st = t->st;
         st.ref_cap = (kTrackMaxLocal + 1) * st.cells;
-        Carver sz(nullptr);
-        TrackBatch tmp{};
-        wave_scratch(sz, tmp, (size_t)S * st.ref_cap, S, st.ref_cap);
-        const size_t head = ref_store_bytes(st);
-        int rc = check_cuda(ctx, cudaMalloc(&t->d_ref, head + sz.bytes() + 256), "cudaMalloc(reference store)");
+        const size_t head = ref_store_bytes(st);   // (256-byte multiple) the store, then the sparse alignment's wave scratch
+        int rc = check_cuda(ctx, cudaMalloc(&t->d_ref, head + sparse_align2_scratch_bytes(S, st.ref_cap)), "cudaMalloc(reference store)");
         if (rc == YGZB_OK) rc = check_cuda(ctx, cudaMemsetAsync(t->d_ref, 0, head, ctx->stream), "memset");
         if (rc == YGZB_OK) rc = check_cuda(ctx, cudaMallocHost((void**)&t->h_aux, sizeof(int32_t) * 2 * (size_t)t->max_jobs), "cudaMallocHost");
         if (rc == YGZB_OK) rc = dalloc(ctx, &t->d_aux, 2 * (size_t)t->max_jobs);

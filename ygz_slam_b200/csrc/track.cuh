@@ -47,11 +47,7 @@ struct TrackBatch {
     int32_t *ref_slot, *cur_slot, *offsets, *in_off, *n_feat, *n_meas;
     double *T_ref, *T_cur;      // [J][12]; T_cur: reference pose in, aligned pose, then pose-only result
     double* T_aligned;          // [J][12]  the aligned pose (pose-only's start), kept for ygzb_tracker_debug_job
-    float *ref_patch, *gdx, *gdy;
-    double* frame_jac;
-    uint8_t* visible;
-    double* sparse_ws;
-    void* sa2_scratch;          // global fall-back of the second-generation kernel's per-feature staging
+    void* sa2_scratch;          // global fall-back of sparse_align2_kernel's per-feature staging
     // Matcher::SparseImageAlignment's motion check, poses relative to the local key-frames
     int32_t* aligned;           // [J]
     double* rel;                // [J][kTrackMaxLocal][12]
