@@ -880,20 +880,9 @@ int launch_sparse_align2(ygzb_ctx* ctx, const SparseArgs& a, int n_problems, int
     });
     const int max_features = (int)(a.feat_stride / sizeof(SA2Feat));
     const int feat_cap = std::min(max_dyn / (int)sizeof(SA2Feat), (max_features + cluster - 1) / cluster);
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)(n_problems * cluster));
-    cfg.blockDim = dim3(kSA2Threads);
-    cfg.dynamicSmemBytes = (size_t)feat_cap * sizeof(SA2Feat);
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = cluster;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
     ProfScope ps(ctx, kStageSparseAlign);
-    YGZB_CUDA(ctx, cudaLaunchKernelEx(&cfg, sparse_align2_kernel, a, feat_cap));
+    YGZB_CUDA(ctx, launch_cluster(sparse_align2_kernel, (unsigned)(n_problems * cluster), kSA2Threads, cluster,
+                                  (size_t)feat_cap * sizeof(SA2Feat), ctx->stream, a, feat_cap));
     YGZB_LAUNCHED(ctx);
     return YGZB_OK;
 }

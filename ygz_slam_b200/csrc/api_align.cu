@@ -9,22 +9,6 @@ using namespace ygzb;
 
 namespace {
 
-template <typename T>
-int h2d(ygzb_ctx* ctx, T* dst, const T* src, size_t count) {
-    if (!count) return YGZB_OK;
-    return check_cuda(ctx, cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyHostToDevice, ctx->stream), "H2D");
-}
-template <typename T>
-int d2h(ygzb_ctx* ctx, T* dst, const T* src, size_t count) {
-    if (!count) return YGZB_OK;
-    return check_cuda(ctx, cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyDeviceToHost, ctx->stream), "D2H");
-}
-#define TRY(x)                       \
-    do {                             \
-        int _rc = (x);               \
-        if (_rc != YGZB_OK) return _rc; \
-    } while (0)
-
 int check_slots(ygzb_frames* f, const int32_t* s, int n, const char* what) {
     for (int i = 0; i < n; ++i)
         if (s[i] < 0 || s[i] >= f->capacity) return set_error(f->ctx, YGZB_ERR_INVALID, "%s[%d] = %d out of range", what, i, s[i]);
@@ -45,17 +29,18 @@ int ygzb_align2d(ygzb_frames* f, int n, const int32_t* slot, const uint8_t* leve
     for (int i = 0; i < n; ++i)
         if (level[i] >= ctx->geo.n_levels) return set_error(ctx, YGZB_ERR_INVALID, "level[%d] out of range", i);
     const size_t N = (size_t)n;
-    Carver sz(nullptr);
-    sz.take<int32_t>(N); sz.take<uint8_t>(N); sz.take<uint8_t>(N * 100); sz.take<uint8_t>(N * 64); sz.take<double>(2 * N); sz.take<uint8_t>(N);
-    void* buf = dev_scratch(ctx, 6, sz.bytes());
+    int32_t* d_slot;
+    uint8_t *d_level, *d_rb, *d_ref, *d_ok;
+    double* d_uv;
+    void* buf = carve_scratch(ctx, 6, [&](Carver& c) {
+        d_slot = c.take<int32_t>(N);
+        d_level = c.take<uint8_t>(N);
+        d_rb = c.take<uint8_t>(N * 100);
+        d_ref = c.take<uint8_t>(N * 64);
+        d_uv = c.take<double>(2 * N);
+        d_ok = c.take<uint8_t>(N);
+    });
     if (!buf) return YGZB_ERR_CUDA;
-    Carver c(buf);
-    int32_t* d_slot = c.take<int32_t>(N);
-    uint8_t* d_level = c.take<uint8_t>(N);
-    uint8_t* d_rb = c.take<uint8_t>(N * 100);
-    uint8_t* d_ref = c.take<uint8_t>(N * 64);
-    double* d_uv = c.take<double>(2 * N);
-    uint8_t* d_ok = c.take<uint8_t>(N);
     TRY(h2d(ctx, d_slot, slot, N));
     TRY(h2d(ctx, d_level, level, N));
     TRY(h2d(ctx, d_rb, ref_border, N * 100));
@@ -78,20 +63,21 @@ int ygzb_align1d(ygzb_frames* f, int n, const int32_t* slot, const uint8_t* leve
     for (int i = 0; i < n; ++i)
         if (level[i] >= ctx->geo.n_levels) return set_error(ctx, YGZB_ERR_INVALID, "level[%d] out of range", i);
     const size_t N = (size_t)n;
-    Carver sz(nullptr);
-    sz.take<int32_t>(N); sz.take<uint8_t>(N); sz.take<float>(2 * N); sz.take<uint8_t>(N * 100); sz.take<uint8_t>(N * 64); sz.take<double>(2 * N);
-    sz.take<uint8_t>(N); sz.take<double>(N);
-    void* buf = dev_scratch(ctx, 6, sz.bytes());
+    int32_t* d_slot;
+    uint8_t *d_level, *d_rb, *d_ref, *d_ok;
+    float* d_dir;
+    double *d_uv, *d_h;
+    void* buf = carve_scratch(ctx, 6, [&](Carver& c) {
+        d_slot = c.take<int32_t>(N);
+        d_level = c.take<uint8_t>(N);
+        d_dir = c.take<float>(2 * N);
+        d_rb = c.take<uint8_t>(N * 100);
+        d_ref = c.take<uint8_t>(N * 64);
+        d_uv = c.take<double>(2 * N);
+        d_ok = c.take<uint8_t>(N);
+        d_h = c.take<double>(N);
+    });
     if (!buf) return YGZB_ERR_CUDA;
-    Carver c(buf);
-    int32_t* d_slot = c.take<int32_t>(N);
-    uint8_t* d_level = c.take<uint8_t>(N);
-    float* d_dir = c.take<float>(2 * N);
-    uint8_t* d_rb = c.take<uint8_t>(N * 100);
-    uint8_t* d_ref = c.take<uint8_t>(N * 64);
-    double* d_uv = c.take<double>(2 * N);
-    uint8_t* d_ok = c.take<uint8_t>(N);
-    double* d_h = c.take<double>(N);
     TRY(h2d(ctx, d_slot, slot, N));
     TRY(h2d(ctx, d_level, level, N));
     TRY(h2d(ctx, d_dir, dir, 2 * N));
@@ -123,37 +109,33 @@ int ygzb_project_align(ygzb_frames* f, int n, const int32_t* ref_slot, const int
         if (ref_level[i] >= ctx->geo.n_levels) return set_error(ctx, YGZB_ERR_INVALID, "ref_level[%d] out of range", i);
     }
     const size_t N = (size_t)n, P = (size_t)n_poses;
-    Carver sz(nullptr);
-    sz.take<int32_t>(4 * N); sz.take<double>(12 * P); sz.take<double>(2 * N); sz.take<double>(N); sz.take<double>(2 * N);
-    sz.take<uint8_t>(N); sz.take<uint8_t>(N); sz.take<uint8_t>(N);
-    void* buf = dev_scratch(ctx, 6, sz.bytes());
+    int32_t* d_idx;
+    double *d_poses, *d_rpx, *d_depth, *d_cpx;
+    uint8_t *d_rlevel, *d_slevel, *d_ok;
+    void* buf = carve_scratch(ctx, 6, [&](Carver& c) {
+        d_idx = c.take<int32_t>(4 * N);
+        d_poses = c.take<double>(12 * P);
+        d_rpx = c.take<double>(2 * N);
+        d_depth = c.take<double>(N);
+        d_cpx = c.take<double>(2 * N);
+        d_rlevel = c.take<uint8_t>(N);
+        d_slevel = c.take<uint8_t>(N);
+        d_ok = c.take<uint8_t>(N);
+    });
     if (!buf) return YGZB_ERR_CUDA;
-    Carver c(buf);
-    int32_t* d_idx = c.take<int32_t>(4 * N);
-    double* d_poses = c.take<double>(12 * P);
-    double* d_rpx = c.take<double>(2 * N);
-    double* d_depth = c.take<double>(N);
-    double* d_cpx = c.take<double>(2 * N);
-    uint8_t* d_rlevel = c.take<uint8_t>(N);
-    uint8_t* d_slevel = c.take<uint8_t>(N);
-    uint8_t* d_ok = c.take<uint8_t>(N);
-    // the inputs are the first six sub-buffers, contiguous on the device: assemble them in pinned memory with the same
-    // layout and move them with ONE copy (nine pageable copies cost more than the kernel itself)
-    const size_t in_bytes = (size_t)((uint8_t*)(d_rlevel + N) - (uint8_t*)buf);
-    uint8_t* stage = (uint8_t*)host_scratch(ctx, 1, in_bytes);
-    if (!stage) return YGZB_ERR_CUDA;
-    YGZB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    auto put = [&](const void* dev_ptr, const void* src, size_t bytes) { memcpy(stage + ((const uint8_t*)dev_ptr - (uint8_t*)buf), src, bytes); };
-    put(d_idx, ref_slot, N * 4);
-    put(d_idx + N, cur_slot, N * 4);
-    put(d_idx + 2 * N, ref_pose, N * 4);
-    put(d_idx + 3 * N, cur_pose, N * 4);
-    put(d_poses, poses, 12 * P * 8);
-    put(d_rpx, ref_px, 2 * N * 8);
-    put(d_depth, ref_depth, N * 8);
-    put(d_cpx, cur_px, 2 * N * 8);
-    put(d_rlevel, ref_level, N);
-    YGZB_CUDA(ctx, cudaMemcpyAsync(buf, stage, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    // the inputs are the first six sub-buffers: one staged copy (nine pageable copies cost more than the kernel itself)
+    StagedUpload up;
+    TRY(up.begin(ctx, buf, (size_t)((uint8_t*)(d_rlevel + N) - (uint8_t*)buf)));
+    up.put(d_idx, ref_slot, N * 4);
+    up.put(d_idx + N, cur_slot, N * 4);
+    up.put(d_idx + 2 * N, ref_pose, N * 4);
+    up.put(d_idx + 3 * N, cur_pose, N * 4);
+    up.put(d_poses, poses, 12 * P * 8);
+    up.put(d_rpx, ref_px, 2 * N * 8);
+    up.put(d_depth, ref_depth, N * 8);
+    up.put(d_cpx, cur_px, 2 * N * 8);
+    up.put(d_rlevel, ref_level, N);
+    TRY(up.commit());
     TRY(launch_project_align(f, n, d_idx, d_idx + N, d_poses, d_idx + 2 * N, d_idx + 3 * N, d_rpx, d_depth, d_rlevel, d_cpx, d_slevel,
                              d_ok));
     TRY(d2h(ctx, cur_px, d_cpx, 2 * N));
@@ -180,40 +162,34 @@ int ygzb_sparse_align(ygzb_frames* f, int n_problems, const int32_t* ref_slot, c
     int max_nf = 0;
     for (int p = 0; p < n_problems; ++p) max_nf = std::max(max_nf, offsets[p + 1] - offsets[p]);
     const size_t feat_stride = sparse_align2_scratch_bytes(1, max_nf);
-    Carver sz(nullptr);
-    sz.take<int32_t>(2 * P); sz.take<int32_t>(P + 1); sz.take<double>(2 * T); sz.take<double>(T); sz.take<uint8_t>(T);
-    sz.take<double>(12 * P); sz.take<double>(12 * P); sz.take<int32_t>(P); sz.take<int32_t>(P * kMaxLevels);
-    sz.take<uint8_t>(P * feat_stride);
-    void* buf = dev_scratch(ctx, 6, sz.bytes());
+    int32_t *d_slots, *d_off, *d_nmeas, *d_iters;
+    double *d_px, *d_depth, *d_Tref, *d_Tcur;
+    uint8_t *d_mp, *d_feat;
+    void* buf = carve_scratch(ctx, 6, [&](Carver& c) {
+        d_slots = c.take<int32_t>(2 * P);
+        d_off = c.take<int32_t>(P + 1);
+        d_px = c.take<double>(2 * T);
+        d_depth = c.take<double>(T);
+        d_mp = c.take<uint8_t>(T);
+        d_Tref = c.take<double>(12 * P);
+        d_Tcur = c.take<double>(12 * P);
+        d_nmeas = c.take<int32_t>(P);
+        d_iters = c.take<int32_t>(P * kMaxLevels);
+        d_feat = c.take<uint8_t>(P * feat_stride);
+    });
     if (!buf) return YGZB_ERR_CUDA;
-    Carver c(buf);
-    int32_t* d_slots = c.take<int32_t>(2 * P);
-    int32_t* d_off = c.take<int32_t>(P + 1);
-    double* d_px = c.take<double>(2 * T);
-    double* d_depth = c.take<double>(T);
-    uint8_t* d_mp = c.take<uint8_t>(T);
-    double* d_Tref = c.take<double>(12 * P);
-    double* d_Tcur = c.take<double>(12 * P);
-    int32_t* d_nmeas = c.take<int32_t>(P);
-    int32_t* d_iters = c.take<int32_t>(P * kMaxLevels);
-    uint8_t* d_feat = c.take<uint8_t>(P * feat_stride);
-    {   // the inputs are the first seven sub-buffers of `buf`: one pinned staging copy instead of eight pageable ones
-        const size_t in_bytes = (size_t)((uint8_t*)(d_Tcur + 12 * P) - (uint8_t*)buf);
-        uint8_t* stage = (uint8_t*)host_scratch(ctx, 1, in_bytes);
-        if (!stage) return YGZB_ERR_CUDA;
-        YGZB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        auto put = [&](const void* dev_ptr, const void* src, size_t bytes) {
-            if (bytes) memcpy(stage + ((const uint8_t*)dev_ptr - (uint8_t*)buf), src, bytes);
-        };
-        put(d_slots, ref_slot, P * 4);
-        put(d_slots + P, cur_slot, P * 4);
-        put(d_off, offsets, (P + 1) * 4);
-        put(d_px, px, 2 * T * 8);
-        put(d_depth, depth, T * 8);
-        put(d_mp, has_mappoint, T);
-        put(d_Tref, T_cw_ref, 12 * P * 8);
-        put(d_Tcur, T_cw_cur, 12 * P * 8);
-        YGZB_CUDA(ctx, cudaMemcpyAsync(buf, stage, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    {   // the inputs are the first seven sub-buffers of `buf`: one staged copy instead of eight pageable ones
+        StagedUpload up;
+        TRY(up.begin(ctx, buf, (size_t)((uint8_t*)(d_Tcur + 12 * P) - (uint8_t*)buf)));
+        up.put(d_slots, ref_slot, P * 4);
+        up.put(d_slots + P, cur_slot, P * 4);
+        up.put(d_off, offsets, (P + 1) * 4);
+        up.put(d_px, px, 2 * T * 8);
+        up.put(d_depth, depth, T * 8);
+        up.put(d_mp, has_mappoint, T);
+        up.put(d_Tref, T_cw_ref, 12 * P * 8);
+        up.put(d_Tcur, T_cw_cur, 12 * P * 8);
+        TRY(up.commit());
     }
     YGZB_CUDA(ctx, cudaMemsetAsync(d_iters, 0, P * kMaxLevels * sizeof(int32_t), ctx->stream));
     TRY(launch_sparse_align(f, n_problems, d_slots, d_slots + P, d_off, d_px, d_depth, d_mp, d_Tref, d_Tcur, max_level, min_level,

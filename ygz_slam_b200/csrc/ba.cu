@@ -1173,20 +1173,9 @@ int launch_pose_only_dev(ygzb_ctx* ctx, int n_problems, const int32_t* d_offsets
     a.fx = ctx->prm.fx; a.fy = ctx->prm.fy; a.cx = ctx->prm.cx; a.cy = ctx->prm.cy;
     cluster = std::max(1, std::min(cluster, kPoseCluster));
     a.stage_k = pose_only_stage_k(max_points, cluster);
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)(n_problems * cluster));
-    cfg.blockDim = dim3(kPoseThreads);
-    cfg.dynamicSmemBytes = (size_t)a.stage_k * 5 * kPoseThreads * sizeof(double);
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = cluster;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
     ProfScope ps(ctx, kStagePoseOnly);
-    YGZB_CUDA(ctx, cudaLaunchKernelEx(&cfg, pose_only_kernel, a));
+    YGZB_CUDA(ctx, launch_cluster(pose_only_kernel, (unsigned)(n_problems * cluster), kPoseThreads, cluster,
+                                  (size_t)a.stage_k * 5 * kPoseThreads * sizeof(double), ctx->stream, a));
     YGZB_LAUNCHED(ctx);
     return YGZB_OK;
 }
@@ -1195,24 +1184,6 @@ int launch_pose_only_dev(ygzb_ctx* ctx, int n_problems, const int32_t* d_offsets
 
 // ---- extern "C" entry points (marshalling + index bookkeeping only) ---------------------------------------
 using namespace ygzb;
-
-namespace {
-template <typename T>
-int h2d(ygzb_ctx* ctx, T* dst, const T* src, size_t count) {
-    if (!count) return YGZB_OK;
-    return check_cuda(ctx, cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyHostToDevice, ctx->stream), "H2D");
-}
-template <typename T>
-int d2h(ygzb_ctx* ctx, T* dst, const T* src, size_t count) {
-    if (!count) return YGZB_OK;
-    return check_cuda(ctx, cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyDeviceToHost, ctx->stream), "D2H");
-}
-#define TRY(x)                          \
-    do {                                \
-        int _rc = (x);                  \
-        if (_rc != YGZB_OK) return _rc; \
-    } while (0)
-}  // namespace
 
 extern "C" {
 
@@ -1251,36 +1222,31 @@ int run_local_ba2(ygzb_ctx* ctx, int n_problems, const int32_t* kf_off, const in
     }
     in.total_pts = NP;
     in.total_obs = NO;
-    Carver sz(nullptr);
-    sz.take<int32_t>(3 * (P + 1)); sz.take<double>(6 * NK); sz.take<uint8_t>(NK); sz.take<double>(3 * NP); sz.take<int32_t>(2 * NO);
-    sz.take<double>(2 * NO);
-    const size_t in_span = sz.bytes();
-    void* buf = dev_scratch(ctx, 7, in_span + ba2_scratch_bytes(NP, NO, P) + 256);
+    int32_t *d_off, *d_idx;
+    double *d_poses, *d_pts, *d_obs;
+    uint8_t* d_fixed;
+    size_t in_span = 0;   // the inputs; the solver's scratch follows them
+    void* buf = carve_scratch(ctx, 7, [&](Carver& c) {
+        d_off = c.take<int32_t>(3 * (P + 1));
+        d_poses = c.take<double>(6 * NK);
+        d_fixed = c.take<uint8_t>(NK);
+        d_pts = c.take<double>(3 * NP);
+        d_idx = c.take<int32_t>(2 * NO);
+        d_obs = c.take<double>(2 * NO);
+    }, ba2_scratch_bytes(NP, NO, P) + 256, &in_span);
     if (!buf) return YGZB_ERR_CUDA;
-    Carver c(buf);
-    int32_t* d_off = c.take<int32_t>(3 * (P + 1));
-    double* d_poses = c.take<double>(6 * NK);
-    uint8_t* d_fixed = c.take<uint8_t>(NK);
-    double* d_pts = c.take<double>(3 * NP);
-    int32_t* d_idx = c.take<int32_t>(2 * NO);
-    double* d_obs = c.take<double>(2 * NO);
-    const size_t in_bytes = (size_t)(reinterpret_cast<uint8_t*>(d_obs + 2 * NO) - static_cast<uint8_t*>(buf));
-    uint8_t* stage = static_cast<uint8_t*>(host_scratch(ctx, 1, in_bytes));
-    if (!stage) return YGZB_ERR_CUDA;
-    YGZB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // an earlier copy may still read the staging buffer
-    auto put = [&](const void* dev_ptr, const void* src, size_t bytes) {
-        if (bytes) memcpy(stage + (static_cast<const uint8_t*>(dev_ptr) - static_cast<uint8_t*>(buf)), src, bytes);
-    };
-    put(d_off, kf_off, (P + 1) * 4);
-    put(d_off + (P + 1), pt_off, (P + 1) * 4);
-    put(d_off + 2 * (P + 1), obs_off, (P + 1) * 4);
-    put(d_poses, poses, 6 * NK * 8);
-    put(d_fixed, fixed, NK);
-    put(d_pts, pts, 3 * NP * 8);
-    put(d_idx, kf_idx, NO * 4);
-    put(d_idx + NO, pt_idx, NO * 4);
-    put(d_obs, obs_px, 2 * NO * 8);
-    YGZB_CUDA(ctx, cudaMemcpyAsync(buf, stage, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    StagedUpload up;
+    TRY(up.begin(ctx, buf, (size_t)(reinterpret_cast<uint8_t*>(d_obs + 2 * NO) - static_cast<uint8_t*>(buf))));
+    up.put(d_off, kf_off, (P + 1) * 4);
+    up.put(d_off + (P + 1), pt_off, (P + 1) * 4);
+    up.put(d_off + 2 * (P + 1), obs_off, (P + 1) * 4);
+    up.put(d_poses, poses, 6 * NK * 8);
+    up.put(d_fixed, fixed, NK);
+    up.put(d_pts, pts, 3 * NP * 8);
+    up.put(d_idx, kf_idx, NO * 4);
+    up.put(d_idx + NO, pt_idx, NO * 4);
+    up.put(d_obs, obs_px, 2 * NO * 8);
+    TRY(up.commit());
     in.kf_off = d_off; in.pt_off = d_off + (P + 1); in.obs_off = d_off + 2 * (P + 1);
     in.poses = d_poses; in.fixed = d_fixed; in.pts = d_pts; in.kf_idx = d_idx; in.pt_idx = d_idx + NO; in.obs = d_obs;
     in.lm_start = nullptr;
@@ -1409,59 +1375,51 @@ int run_local_ba(ygzb_ctx* ctx, int n_problems, const int32_t* kf_off, const int
     }
     const size_t NPAIR = pair_o1.size(), NPS = pair_start.size();
 
-    Carver sz(nullptr);
-    sz.take<int32_t>(3 * (P + 1)); sz.take<double>(6 * NK); sz.take<uint8_t>(NK); sz.take<double>(3 * NP); sz.take<int32_t>(2 * NO);
-    sz.take<double>(2 * NO); sz.take<int32_t>(NP + 1 + NO + NK + 1 + NO); sz.take<int32_t>(P + 1 + NPS + 2 * NPAIR);
-    sz.take<double>(21 * NO); sz.take<double>(9 * NP); sz.take<double>(3 * NP); sz.take<double>(9 * NP); sz.take<double>(3 * NP);
-    sz.take<double>(3 * NP); sz.take<double>(3 * NP); sz.take<double>(8 * P);
-    void* buf = dev_scratch(ctx, 7, sz.bytes());
-    if (!buf) return YGZB_ERR_CUDA;
-    Carver c(buf);
-    int32_t* d_off = c.take<int32_t>(3 * (P + 1));
-    double* d_poses = c.take<double>(6 * NK);
-    uint8_t* d_fixed = c.take<uint8_t>(NK);
-    double* d_pts = c.take<double>(3 * NP);
-    int32_t* d_idx = c.take<int32_t>(2 * NO);
-    double* d_obs = c.take<double>(2 * NO);
-    int32_t* d_csr = c.take<int32_t>(NP + 1 + NO + NK + 1 + NO);
-    int32_t* d_pairs = c.take<int32_t>(P + 1 + NPS + 2 * NPAIR);
+    int32_t *d_off, *d_idx, *d_csr, *d_pairs;
+    double *d_poses, *d_pts, *d_obs;
+    uint8_t* d_fixed;
     BAArgs a;
-    a.lin = c.take<double>(21 * NO);
-    a.Hll = c.take<double>(9 * NP);
-    a.bl = c.take<double>(3 * NP);
-    a.Dinv = c.take<double>(9 * NP);
-    a.xl = c.take<double>(3 * NP);
-    a.pts_backup = c.take<double>(3 * NP);
-    a.scale_l = c.take<double>(3 * NP);
-    a.stats = c.take<double>(8 * P);
+    void* buf = carve_scratch(ctx, 7, [&](Carver& c) {
+        d_off = c.take<int32_t>(3 * (P + 1));
+        d_poses = c.take<double>(6 * NK);
+        d_fixed = c.take<uint8_t>(NK);
+        d_pts = c.take<double>(3 * NP);
+        d_idx = c.take<int32_t>(2 * NO);
+        d_obs = c.take<double>(2 * NO);
+        d_csr = c.take<int32_t>(NP + 1 + NO + NK + 1 + NO);
+        d_pairs = c.take<int32_t>(P + 1 + NPS + 2 * NPAIR);
+        a.lin = c.take<double>(21 * NO);
+        a.Hll = c.take<double>(9 * NP);
+        a.bl = c.take<double>(3 * NP);
+        a.Dinv = c.take<double>(9 * NP);
+        a.xl = c.take<double>(3 * NP);
+        a.pts_backup = c.take<double>(3 * NP);
+        a.scale_l = c.take<double>(3 * NP);
+        a.stats = c.take<double>(8 * P);
+    });
+    if (!buf) return YGZB_ERR_CUDA;
     // kf_idx / pt_idx stay LOCAL to the problem; lm_obs / ps_obs / pair entries are GLOBAL observation ids.
-    // All inputs sit at the front of the device buffer in one contiguous run: they are assembled in a pinned staging
-    // buffer with the same layout and travel as ONE host-to-device copy (instead of 17 pageable ones).
-    const size_t in_bytes = (size_t)(reinterpret_cast<uint8_t*>(d_pairs + P + 1 + NPS + 2 * NPAIR) - static_cast<uint8_t*>(buf));
-    uint8_t* stage = static_cast<uint8_t*>(host_scratch(ctx, 1, in_bytes));
-    if (!stage) return YGZB_ERR_CUDA;
-    YGZB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // an earlier copy may still read the staging buffer
-    auto put = [&](const void* dev_ptr, const void* src, size_t bytes) {
-        if (bytes) memcpy(stage + (static_cast<const uint8_t*>(dev_ptr) - static_cast<uint8_t*>(buf)), src, bytes);
-    };
-    put(d_off, kf_off, (P + 1) * 4);
-    put(d_off + (P + 1), pt_off, (P + 1) * 4);
-    put(d_off + 2 * (P + 1), obs_off, (P + 1) * 4);
-    put(d_poses, poses, 6 * NK * 8);
-    put(d_fixed, fixed, NK);
-    put(d_pts, pts, 3 * NP * 8);
-    put(d_idx, kf_idx, NO * 4);
-    put(d_idx + NO, pt_idx, NO * 4);
-    put(d_obs, obs_px, 2 * NO * 8);
-    put(d_csr, lm_start.data(), (NP + 1) * 4);
-    put(d_csr + NP + 1, lm_obs.data(), NO * 4);
-    put(d_csr + NP + 1 + NO, ps_start.data(), (NK + 1) * 4);
-    put(d_csr + NP + 1 + NO + NK + 1, ps_obs.data(), NO * 4);
-    put(d_pairs, pair_off.data(), (P + 1) * 4);
-    put(d_pairs + P + 1, pair_start.data(), NPS * 4);
-    put(d_pairs + P + 1 + NPS, pair_o1.data(), NPAIR * 4);
-    put(d_pairs + P + 1 + NPS + NPAIR, pair_o2.data(), NPAIR * 4);
-    YGZB_CUDA(ctx, cudaMemcpyAsync(buf, stage, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    // All inputs sit at the front of the device buffer in one contiguous run (one staged copy instead of 17 pageable ones).
+    StagedUpload up;
+    TRY(up.begin(ctx, buf, (size_t)(reinterpret_cast<uint8_t*>(d_pairs + P + 1 + NPS + 2 * NPAIR) - static_cast<uint8_t*>(buf))));
+    up.put(d_off, kf_off, (P + 1) * 4);
+    up.put(d_off + (P + 1), pt_off, (P + 1) * 4);
+    up.put(d_off + 2 * (P + 1), obs_off, (P + 1) * 4);
+    up.put(d_poses, poses, 6 * NK * 8);
+    up.put(d_fixed, fixed, NK);
+    up.put(d_pts, pts, 3 * NP * 8);
+    up.put(d_idx, kf_idx, NO * 4);
+    up.put(d_idx + NO, pt_idx, NO * 4);
+    up.put(d_obs, obs_px, 2 * NO * 8);
+    up.put(d_csr, lm_start.data(), (NP + 1) * 4);
+    up.put(d_csr + NP + 1, lm_obs.data(), NO * 4);
+    up.put(d_csr + NP + 1 + NO, ps_start.data(), (NK + 1) * 4);
+    up.put(d_csr + NP + 1 + NO + NK + 1, ps_obs.data(), NO * 4);
+    up.put(d_pairs, pair_off.data(), (P + 1) * 4);
+    up.put(d_pairs + P + 1, pair_start.data(), NPS * 4);
+    up.put(d_pairs + P + 1 + NPS, pair_o1.data(), NPAIR * 4);
+    up.put(d_pairs + P + 1 + NPS + NPAIR, pair_o2.data(), NPAIR * 4);
+    TRY(up.commit());
     a.kf_off = d_off; a.pt_off = d_off + (P + 1); a.obs_off = d_off + 2 * (P + 1);
     a.poses = d_poses; a.fixed = d_fixed; a.pts = d_pts; a.kf_idx = d_idx; a.pt_idx = d_idx + NO; a.obs = d_obs;
     a.lm_start = d_csr; a.lm_obs = d_csr + NP + 1; a.ps_start = d_csr + NP + 1 + NO; a.ps_obs = d_csr + NP + 1 + NO + NK + 1;
@@ -1491,26 +1449,10 @@ int run_local_ba(ygzb_ctx* ctx, int n_problems, const int32_t* kf_off, const int
     {
         // one cluster of CTAs (= SMs) per problem.  Every LM trial crosses ~8 cluster barriers, so small problems (a few
         // thousand observations: the local BA of the tracking loop) are faster on fewer CTAs; large ones want all eight
-        int cluster = kClusterSize;
-        if (const char* e = getenv("YGZB_BA_CLUSTER")) {   // tuning knob: 1, 2, 4 or 8
-            const int v = atoi(e);
-            if (v == 1 || v == 2 || v == 4 || v == 8 || v == 16) cluster = v;
-        }
+        const int cluster = cluster_knob("YGZB_BA_CLUSTER", kClusterSize, true);
         if (cluster > 8) YGZB_CUDA(ctx, cudaFuncSetAttribute(local_ba_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3((unsigned)(n_problems * cluster));
-        cfg.blockDim = dim3(kBAThreads);
-        cfg.dynamicSmemBytes = smem;
-        cfg.stream = ctx->stream;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = cluster;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
         ProfScope ps(ctx, kStageLocalBA);
-        YGZB_CUDA(ctx, cudaLaunchKernelEx(&cfg, local_ba_kernel, a, d_ws));
+        YGZB_CUDA(ctx, launch_cluster(local_ba_kernel, (unsigned)(n_problems * cluster), kBAThreads, cluster, smem, ctx->stream, a, d_ws));
     }
     YGZB_LAUNCHED(ctx);
     TRY(d2h(ctx, poses, d_poses, 6 * NK));
@@ -1519,6 +1461,18 @@ int run_local_ba(ygzb_ctx* ctx, int n_problems, const int32_t* kf_off, const int
     TRY(d2h(ctx, hst.data(), a.stats, 8 * P));
     YGZB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return YGZB_OK;
+}
+
+// the public statistics of local_ba_kernel's problems from their 8 raw ones (hst as run_local_ba returns it)
+void fill_ceres_stats(ygzb_ceres_stats* stats, const std::vector<double>& hst) {
+    for (size_t p = 0; p < hst.size() / 8; ++p) {
+        stats[p].iters = (int)hst[8 * p];
+        stats[p].successful_steps = (int)hst[8 * p + 1];
+        stats[p].cost_initial = hst[8 * p + 2];
+        stats[p].cost_final = hst[8 * p + 3];
+        stats[p].radius_final = hst[8 * p + 4];
+        stats[p].termination = (int)hst[8 * p + 5];
+    }
 }
 }  // namespace
 
@@ -1563,15 +1517,7 @@ int ygzb_local_ba_ceres(ygzb_ctx* ctx, int n_problems, const int32_t* kf_off, co
     } catch (const std::exception& e) {
         return set_error(ctx, YGZB_ERR_INVALID, "ygzb_local_ba_ceres: %s", e.what());
     }
-    if (stats)
-        for (size_t p = 0; p < (size_t)n_problems; ++p) {
-            stats[p].iters = (int)hst[8 * p];
-            stats[p].successful_steps = (int)hst[8 * p + 1];
-            stats[p].cost_initial = hst[8 * p + 2];
-            stats[p].cost_final = hst[8 * p + 3];
-            stats[p].radius_final = hst[8 * p + 4];
-            stats[p].termination = (int)hst[8 * p + 5];
-        }
+    if (stats) fill_ceres_stats(stats, hst);
     return YGZB_OK;
 }
 
@@ -1657,27 +1603,23 @@ int ygzb_two_view_ba(ygzb_ctx* ctx, int n_problems, const int32_t* offsets, cons
         std::vector<double> hst;
         TRY(run_local_ba(ctx, n_problems, kf_off.data(), pt_off.data(), obs_off.data(), poses.data(), fixed.data(), X.data(),
                          kf_idx.data(), pt_idx.data(), obs.data(), 50, 0.1, hst, mask.data()));
-        if (stats)
-            for (size_t p = 0; p < P; ++p) {
-                stats[p].iters = (int)hst[8 * p]; stats[p].successful_steps = (int)hst[8 * p + 1]; stats[p].cost_initial = hst[8 * p + 2];
-                stats[p].cost_final = hst[8 * p + 3]; stats[p].radius_final = hst[8 * p + 4]; stats[p].termination = (int)hst[8 * p + 5];
-            }
+        if (stats) fill_ceres_stats(stats, hst);
         std::memcpy(pts, X.data(), 3 * N * sizeof(double));
         // inlier classification + pose conversion on the device
-        Carver sz(nullptr);
-        sz.take<int32_t>(N); sz.take<double>(12 * P); sz.take<double>(12 * P); sz.take<double>(3 * N); sz.take<double>(2 * N); sz.take<double>(2 * N);
-        sz.take<uint8_t>(N); sz.take<double>(12 * P);
-        void* buf = dev_scratch(ctx, 6, sz.bytes());
+        int32_t* d_prob;
+        double *d_Tref, *d_poses, *d_pts, *d_pr, *d_pc, *d_Tcur;
+        uint8_t* d_in;
+        void* buf = carve_scratch(ctx, 6, [&](Carver& c) {
+            d_prob = c.take<int32_t>(N);
+            d_Tref = c.take<double>(12 * P);
+            d_poses = c.take<double>(12 * P);
+            d_pts = c.take<double>(3 * N);
+            d_pr = c.take<double>(2 * N);
+            d_pc = c.take<double>(2 * N);
+            d_in = c.take<uint8_t>(N);
+            d_Tcur = c.take<double>(12 * P);
+        });
         if (!buf) return YGZB_ERR_CUDA;
-        Carver c(buf);
-        int32_t* d_prob = c.take<int32_t>(N);
-        double* d_Tref = c.take<double>(12 * P);
-        double* d_poses = c.take<double>(12 * P);
-        double* d_pts = c.take<double>(3 * N);
-        double* d_pr = c.take<double>(2 * N);
-        double* d_pc = c.take<double>(2 * N);
-        uint8_t* d_in = c.take<uint8_t>(N);
-        double* d_Tcur = c.take<double>(12 * P);
         TRY(h2d(ctx, d_prob, prob_of.data(), N));
         TRY(h2d(ctx, d_Tref, T_cw_ref, 12 * P));
         TRY(h2d(ctx, d_poses, poses.data(), 12 * P));
@@ -1710,62 +1652,38 @@ int ygzb_pose_only(ygzb_ctx* ctx, int n_problems, const int32_t* offsets, const 
     }
     const size_t P = (size_t)n_problems, N = (size_t)offsets[n_problems];
     if (N && (!pt_world || !px || !inlier || !depth)) return YGZB_ERR_INVALID;
-    Carver sz(nullptr);
-    sz.take<int32_t>(P + 1); sz.take<double>(3 * N); sz.take<double>(2 * N); sz.take<double>(12 * P); sz.take<uint8_t>(N);
-    sz.take<double>(N); sz.take<int32_t>(P); sz.take<uint8_t>(N); sz.take<double>(P * 4 * kPoseCluster * kPoseRed);
-    void* buf = dev_scratch(ctx, 7, sz.bytes());
+    int32_t *d_off, *d_n_inlier;
+    double *d_pw, *d_px, *d_T_cw, *d_depth, *d_ws;
+    uint8_t *d_inlier, *d_enable;
+    void* buf = carve_scratch(ctx, 7, [&](Carver& c) {
+        d_off = c.take<int32_t>(P + 1);
+        d_pw = c.take<double>(3 * N);
+        d_px = c.take<double>(2 * N);
+        d_T_cw = c.take<double>(12 * P);
+        d_inlier = c.take<uint8_t>(N);
+        d_depth = c.take<double>(N);
+        d_n_inlier = c.take<int32_t>(P);
+        d_enable = c.take<uint8_t>(N);
+        d_ws = c.take<double>(P * 4 * kPoseCluster * kPoseRed);
+    });
     if (!buf) return YGZB_ERR_CUDA;
-    Carver c(buf);
-    PoseOnlyArgs a;
-    int32_t* d_off = c.take<int32_t>(P + 1);
-    double* d_pw = c.take<double>(3 * N);
-    double* d_px = c.take<double>(2 * N);
-    a.T_cw = c.take<double>(12 * P);
-    a.inlier = c.take<uint8_t>(N);
-    a.depth = c.take<double>(N);
-    a.n_inlier = c.take<int32_t>(P);
-    a.enable = c.take<uint8_t>(N);
-    a.ws = c.take<double>(P * 4 * kPoseCluster * kPoseRed);
-    a.offsets = d_off; a.counts = nullptr; a.pw = d_pw; a.px = d_px;
-    a.fx = ctx->prm.fx; a.fy = ctx->prm.fy; a.cx = ctx->prm.cx; a.cy = ctx->prm.cy;
-    {   // the four inputs are the first sub-buffers of `buf`: one pinned staging copy instead of four pageable ones
-        const size_t in_bytes = (size_t)(reinterpret_cast<uint8_t*>(a.T_cw + 12 * P) - static_cast<uint8_t*>(buf));
-        uint8_t* stage = static_cast<uint8_t*>(host_scratch(ctx, 1, in_bytes));
-        if (!stage) return YGZB_ERR_CUDA;
-        YGZB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        auto put = [&](const void* dev_ptr, const void* src, size_t bytes) {
-            if (bytes) memcpy(stage + (static_cast<const uint8_t*>(dev_ptr) - static_cast<uint8_t*>(buf)), src, bytes);
-        };
-        put(d_off, offsets, (P + 1) * 4);
-        put(d_pw, pt_world, 3 * N * 8);
-        put(d_px, px, 2 * N * 8);
-        put(a.T_cw, T_cw, 12 * P * 8);
-        YGZB_CUDA(ctx, cudaMemcpyAsync(buf, stage, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    {   // the four inputs are the first sub-buffers of `buf`: one staged copy instead of four pageable ones
+        StagedUpload up;
+        TRY(up.begin(ctx, buf, (size_t)(reinterpret_cast<uint8_t*>(d_T_cw + 12 * P) - static_cast<uint8_t*>(buf))));
+        up.put(d_off, offsets, (P + 1) * 4);
+        up.put(d_pw, pt_world, 3 * N * 8);
+        up.put(d_px, px, 2 * N * 8);
+        up.put(d_T_cw, T_cw, 12 * P * 8);
+        TRY(up.commit());
     }
-    {
-        int max_points = 0;
-        for (size_t q = 0; q < P; ++q) max_points = std::max(max_points, offsets[q + 1] - offsets[q]);
-        a.stage_k = pose_only_stage_k(max_points, kPoseCluster);
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3((unsigned)(n_problems * kPoseCluster));
-        cfg.blockDim = dim3(kPoseThreads);
-        cfg.dynamicSmemBytes = (size_t)a.stage_k * 5 * kPoseThreads * sizeof(double);
-        cfg.stream = ctx->stream;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = kPoseCluster;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        ProfScope ps(ctx, kStagePoseOnly);
-        YGZB_CUDA(ctx, cudaLaunchKernelEx(&cfg, pose_only_kernel, a));
-    }
-    YGZB_LAUNCHED(ctx);
-    TRY(d2h(ctx, T_cw, a.T_cw, 12 * P));
-    TRY(d2h(ctx, inlier, a.inlier, N));
-    TRY(d2h(ctx, depth, a.depth, N));
-    TRY(d2h(ctx, n_inlier, a.n_inlier, P));
+    int max_points = 0;
+    for (size_t q = 0; q < P; ++q) max_points = std::max(max_points, offsets[q + 1] - offsets[q]);
+    TRY(launch_pose_only_dev(ctx, n_problems, d_off, nullptr, d_pw, d_px, d_T_cw, d_inlier, d_depth, d_n_inlier, d_enable, d_ws, kPoseCluster,
+                             max_points));
+    TRY(d2h(ctx, T_cw, d_T_cw, 12 * P));
+    TRY(d2h(ctx, inlier, d_inlier, N));
+    TRY(d2h(ctx, depth, d_depth, N));
+    TRY(d2h(ctx, n_inlier, d_n_inlier, P));
     YGZB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return YGZB_OK;
 }

@@ -1127,13 +1127,32 @@ __global__ void __launch_bounds__(1024) csr_build_kernel(const int32_t* __restri
     }
 }
 
+// the solver's scratch behind a caller's inputs: NP points, NO observations, P problems
+struct BA2Scratch {
+    int32_t *cnt, *lm_start, *so_orig, *so_kf;
+    double *so_uv, *lin, *stats, *debug;
+    uint8_t *slot, *outlier;
+};
+
+void ba2_scratch_carve(Carver& c, BA2Scratch& s, size_t NP, size_t NO, size_t P) {
+    s.cnt = c.take<int32_t>(NP + 1);
+    s.lm_start = c.take<int32_t>(NP + 1);
+    s.so_orig = c.take<int32_t>(NO);
+    s.so_kf = c.take<int32_t>(NO);
+    s.so_uv = c.take<double>(2 * NO);
+    s.lin = c.take<double>(ba2_stage_doubles(NP + 8 * 16 * P, NO));   // global fall-back of the CTA-private staging areas (+ per-CTA rounding slack)
+    s.slot = c.take<uint8_t>(NP * kBA2MaxFree);
+    s.outlier = c.take<uint8_t>(NO);
+    s.stats = c.take<double>(8 * P);
+    s.debug = c.take<double>(8 * P);   // (YGZB_BA_DEBUG)
+}
+
 }  // namespace
 
 size_t ba2_scratch_bytes(size_t NP, size_t NO, size_t P) {
     Carver sz(nullptr);
-    sz.take<int32_t>(NP + 1); sz.take<int32_t>(NP + 1); sz.take<int32_t>(NO); sz.take<int32_t>(NO); sz.take<double>(2 * NO);
-    sz.take<double>(ba2_stage_doubles(NP + 8 * 16 * P, NO));   // global fall-back of the staging areas (+ per-CTA rounding slack)
-    sz.take<uint8_t>(NP * kBA2MaxFree); sz.take<uint8_t>(NO); sz.take<double>(8 * P); sz.take<double>(8 * P);
+    BA2Scratch s;
+    ba2_scratch_carve(sz, s, NP, NO, P);
     return sz.bytes();
 }
 
@@ -1143,17 +1162,11 @@ int launch_local_ba2(ygzb_ctx* ctx, const BA2Problem& in, void* scratch, const y
                      double** d_stats_out) {
     const size_t P = (size_t)in.n_problems, NP = in.total_pts, NO = in.total_obs;
     Carver c(scratch);
-    int32_t* d_cnt = c.take<int32_t>(NP + 1);
-    int32_t* d_lm_start = c.take<int32_t>(NP + 1);
-    int32_t* d_so_orig = c.take<int32_t>(NO);
-    int32_t* d_so_kf = c.take<int32_t>(NO);
-    double* d_so_uv = c.take<double>(2 * NO);
+    BA2Scratch s;
+    ba2_scratch_carve(c, s, NP, NO, P);
     BA2Args a;
-    a.lin = c.take<double>(ba2_stage_doubles(NP + 8 * 16 * P, NO));   // global fall-back of the CTA-private staging areas
-    a.slot = c.take<uint8_t>(NP * kBA2MaxFree);
-    a.outlier = c.take<uint8_t>(NO);
-    a.stats = c.take<double>(8 * P);
-    a.debug = getenv("YGZB_BA_DEBUG") ? c.take<double>(8 * P) : nullptr;
+    a.lin = s.lin; a.slot = s.slot; a.outlier = s.outlier; a.stats = s.stats;
+    a.debug = getenv("YGZB_BA_DEBUG") ? s.debug : nullptr;
     {
         const char* e = getenv("YGZB_BA_SOLVER");
         a.solver = e && atoi(e) == 1 ? 1 : 0;
@@ -1161,20 +1174,20 @@ int launch_local_ba2(ygzb_ctx* ctx, const BA2Problem& in, void* scratch, const y
     if (in.lm_start) {   // the caller already has landmark-major lists (the tracking engine builds them itself)
         a.lm_start = in.lm_start; a.so_kf = in.kf_idx; a.so_uv = in.obs; a.so_orig = nullptr;
     } else {
-        YGZB_CUDA(ctx, cudaMemsetAsync(d_cnt, 0, (NP + 1) * sizeof(int32_t), ctx->stream));
+        YGZB_CUDA(ctx, cudaMemsetAsync(s.cnt, 0, (NP + 1) * sizeof(int32_t), ctx->stream));
         if (NO) {
             ProfScope ps(ctx, kStageOther);
             const dim3 grid((unsigned)std::min<size_t>((in.max_obs + 255) / 256, 64), (unsigned)P);
-            csr_count_kernel<<<grid, 256, 0, ctx->stream>>>((int)P, in.obs_off, in.pt_off, in.pt_idx, d_cnt);
+            csr_count_kernel<<<grid, 256, 0, ctx->stream>>>((int)P, in.obs_off, in.pt_off, in.pt_idx, s.cnt);
             YGZB_LAUNCHED(ctx);
         }
         {
             ProfScope ps(ctx, kStageOther);
-            csr_build_kernel<<<(unsigned)P, 1024, 0, ctx->stream>>>(in.obs_off, in.pt_off, in.kf_idx, in.pt_idx, in.obs, d_cnt, d_lm_start,
-                                                                    d_so_orig, d_so_kf, d_so_uv, (int)P - 1);
+            csr_build_kernel<<<(unsigned)P, 1024, 0, ctx->stream>>>(in.obs_off, in.pt_off, in.kf_idx, in.pt_idx, in.obs, s.cnt, s.lm_start,
+                                                                    s.so_orig, s.so_kf, s.so_uv, (int)P - 1);
             YGZB_LAUNCHED(ctx);
         }
-        a.lm_start = d_lm_start; a.so_kf = d_so_kf; a.so_uv = d_so_uv; a.so_orig = d_so_orig;
+        a.lm_start = s.lm_start; a.so_kf = s.so_kf; a.so_uv = s.so_uv; a.so_orig = s.so_orig;
     }
     a.kf_off = in.kf_off; a.pt_off = in.pt_off; a.obs_off = in.obs_off;
     a.n_kf = in.n_kf; a.n_pt = in.n_pt;
@@ -1192,10 +1205,7 @@ int launch_local_ba2(ygzb_ctx* ctx, const BA2Problem& in, void* scratch, const y
         auto items_per_warp = [&](int c) { return tasks * (((in.max_pts + c - 1) / c + 31) / 32) / (kT / 32); };
         while (cluster < 16 && items_per_warp(cluster) > 24) cluster *= 2;
     }
-    if (const char* e = getenv("YGZB_BA_CLUSTER")) {   // tuning knob: 1, 2, 4 or 8
-        const int v = atoi(e);
-        if (v == 1 || v == 2 || v == 4 || v == 8 || v == 16) cluster = v;
-    }
+    cluster = cluster_knob("YGZB_BA_CLUSTER", cluster, true);
     if (cluster > 8) cudaFuncSetAttribute(local_ba2_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
     const int np = std::max(in.max_free, 0), dimp = 6 * np, n_pairs = np * (np + 1) / 2;
     const int V = kPairW * n_pairs + kPoseW * np;
@@ -1216,21 +1226,9 @@ int launch_local_ba2(ygzb_ctx* ctx, const BA2Problem& in, void* scratch, const y
     const size_t dyn = std::min(cap, sys + 2 * (size_t)V + stage);
     a.dyn_doubles = (long long)dyn;
 
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)(P * cluster));
-    cfg.blockDim = dim3(kT);
-    cfg.dynamicSmemBytes = dyn * sizeof(double);
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = cluster;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
     {
         ProfScope ps(ctx, kStageLocalBA);
-        YGZB_CUDA(ctx, cudaLaunchKernelEx(&cfg, local_ba2_kernel, a));
+        YGZB_CUDA(ctx, launch_cluster(local_ba2_kernel, (unsigned)(P * cluster), kT, cluster, dyn * sizeof(double), ctx->stream, a));
     }
     YGZB_LAUNCHED(ctx);
     if (a.debug) {   // YGZB_BA_DEBUG: phase cycles of problem 0 (blocking; diagnostics only)

@@ -392,20 +392,20 @@ int ygzb_bow_transform(ygzb_vocab* v, int n_frames, const int32_t* offsets, cons
             return YGZB_OK;
         }
         if (!desc || !word || !node || !weight || !bow_word || !bow_value) return YGZB_ERR_INVALID;
-        Carver sz(nullptr);
-        sz.take<int32_t>(F + 1); sz.take<uint8_t>(32 * N); sz.take<int32_t>(N); sz.take<int32_t>(N); sz.take<double>(N); sz.take<int32_t>(F);
-        sz.take<int32_t>(N); sz.take<double>(N);
-        void* buf = dev_scratch(ctx, 6, sz.bytes());
+        int32_t *d_off, *d_word, *d_node, *d_cnt, *d_bw;
+        uint8_t* d_desc;
+        double *d_w, *d_bv;
+        void* buf = carve_scratch(ctx, 6, [&](Carver& c) {
+            d_off = c.take<int32_t>(F + 1);
+            d_desc = c.take<uint8_t>(32 * N);
+            d_word = c.take<int32_t>(N);
+            d_node = c.take<int32_t>(N);
+            d_w = c.take<double>(N);
+            d_cnt = c.take<int32_t>(F);
+            d_bw = c.take<int32_t>(N);
+            d_bv = c.take<double>(N);
+        });
         if (!buf) return YGZB_ERR_CUDA;
-        Carver c(buf);
-        int32_t* d_off = c.take<int32_t>(F + 1);
-        uint8_t* d_desc = c.take<uint8_t>(32 * N);
-        int32_t* d_word = c.take<int32_t>(N);
-        int32_t* d_node = c.take<int32_t>(N);
-        double* d_w = c.take<double>(N);
-        int32_t* d_cnt = c.take<int32_t>(F);
-        int32_t* d_bw = c.take<int32_t>(N);
-        double* d_bv = c.take<double>(N);
         YGZB_CUDA(ctx, cudaMemcpyAsync(d_off, offsets, (F + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
         YGZB_CUDA(ctx, cudaMemcpyAsync(d_desc, desc, 32 * N, cudaMemcpyHostToDevice, ctx->stream));
         {
@@ -457,21 +457,21 @@ int ygzb_search_by_bow(ygzb_ctx* ctx, int n_pairs, const int32_t* off1, const in
         if (!desc1 || !node1 || !match12 || (N2 && (!desc2 || !node2)) || (check_orientation && (!angle1 || (N2 && !angle2)))) return YGZB_ERR_INVALID;
         int max1 = 0;
         for (size_t p = 0; p < P; ++p) max1 = std::max(max1, off1[p + 1] - off1[p]);
-        Carver sz(nullptr);
-        sz.take<int32_t>(2 * (P + 1)); sz.take<uint8_t>(32 * N1); sz.take<uint8_t>(32 * N2 + 32); sz.take<int32_t>(N1); sz.take<int32_t>(N2 + 1);
-        sz.take<float>(N1); sz.take<float>(N2 + 1); sz.take<int32_t>(N1); sz.take<int32_t>(P);
-        void* buf = dev_scratch(ctx, 6, sz.bytes());
+        int32_t *d_off, *d_n1, *d_n2, *d_m, *d_cnt;
+        uint8_t *d_d1, *d_d2;
+        float *d_a1, *d_a2;
+        void* buf = carve_scratch(ctx, 6, [&](Carver& c) {
+            d_off = c.take<int32_t>(2 * (P + 1));
+            d_d1 = c.take<uint8_t>(32 * N1);
+            d_d2 = c.take<uint8_t>(32 * N2 + 32);
+            d_n1 = c.take<int32_t>(N1);
+            d_n2 = c.take<int32_t>(N2 + 1);
+            d_a1 = c.take<float>(N1);
+            d_a2 = c.take<float>(N2 + 1);
+            d_m = c.take<int32_t>(N1);
+            d_cnt = c.take<int32_t>(P);
+        });
         if (!buf) return YGZB_ERR_CUDA;
-        Carver c(buf);
-        int32_t* d_off = c.take<int32_t>(2 * (P + 1));
-        uint8_t* d_d1 = c.take<uint8_t>(32 * N1);
-        uint8_t* d_d2 = c.take<uint8_t>(32 * N2 + 32);
-        int32_t* d_n1 = c.take<int32_t>(N1);
-        int32_t* d_n2 = c.take<int32_t>(N2 + 1);
-        float* d_a1 = c.take<float>(N1);
-        float* d_a2 = c.take<float>(N2 + 1);
-        int32_t* d_m = c.take<int32_t>(N1);
-        int32_t* d_cnt = c.take<int32_t>(P);
         auto H2D = [&](void* dst, const void* src, size_t bytes) {
             return bytes ? check_cuda(ctx, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, ctx->stream), "H2D") : YGZB_OK;
         };

@@ -4,8 +4,10 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <stdlib.h>
 #include <string.h>
 
+#include <utility>
 #include <vector>
 
 #include "../../include/ygz_b200.h"
@@ -133,6 +135,24 @@ void* host_scratch(ygzb_ctx* ctx, int which, size_t bytes);
         if (_rc != YGZB_OK) return _rc;                                    \
     } while (0)
 
+#define TRY(x)                          \
+    do {                                \
+        int _rc = (x);                  \
+        if (_rc != YGZB_OK) return _rc; \
+    } while (0)
+
+// typed copies on the context's stream (nothing is enqueued for a count of zero)
+template <typename T>
+int h2d(ygzb_ctx* ctx, T* dst, const T* src, size_t count) {
+    if (!count) return YGZB_OK;
+    return check_cuda(ctx, cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyHostToDevice, ctx->stream), "H2D");
+}
+template <typename T>
+int d2h(ygzb_ctx* ctx, T* dst, const T* src, size_t count) {
+    if (!count) return YGZB_OK;
+    return check_cuda(ctx, cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyDeviceToHost, ctx->stream), "D2H");
+}
+
 // ---- per-stage device timing -------------------------------------------------------------------
 enum Stage {
     kStageBgr2Gray = 0, kStagePyrDown, kStageFastCells, kStageMergeCells, kStageDescribe, kStageMatch,
@@ -203,6 +223,76 @@ struct Carver {
     }
     size_t bytes() const { return off + 256; }
 };
+
+// One scratch buffer, described once.  `layout(Carver&)` takes the sub-buffers in order and assigns the caller's pointers; it
+// runs on a null Carver to size the buffer and again on the buffer dev_scratch returned for that size (a slot may move when it
+// grows, so only the pointers of that second run are used).  `extra` bytes follow the layout; `sized` receives the layout's
+// Carver::bytes().  Null if the allocation fails.
+template <typename Layout>
+void* carve_scratch(ygzb_ctx* ctx, int which, Layout&& layout, size_t extra = 0, size_t* sized = nullptr) {
+    Carver sz(nullptr);
+    layout(sz);
+    if (sized) *sized = sz.bytes();
+    void* buf = dev_scratch(ctx, which, sz.bytes() + extra);
+    if (buf) {
+        Carver c(buf);
+        layout(c);
+    }
+    return buf;
+}
+
+// The inputs of an entry point are the first sub-buffers of its device buffer `buf`, contiguous up to in_bytes: they are
+// assembled in pinned memory (host slot 1) with the same layout and travel as ONE host-to-device copy instead of one pageable
+// copy each.  begin, put every input at its device address, commit.
+struct StagedUpload {
+    ygzb_ctx* ctx;
+    void* buf;
+    size_t in_bytes;
+    uint8_t* stage;
+    int begin(ygzb_ctx* ctx_, void* buf_, size_t in_bytes_) {
+        ctx = ctx_; buf = buf_; in_bytes = in_bytes_;
+        stage = static_cast<uint8_t*>(host_scratch(ctx, 1, in_bytes));
+        if (!stage) return YGZB_ERR_CUDA;
+        YGZB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // an earlier copy may still read the staging buffer
+        return YGZB_OK;
+    }
+    void put(const void* dev_ptr, const void* src, size_t bytes) const {
+        if (bytes) memcpy(stage + (static_cast<const uint8_t*>(dev_ptr) - static_cast<uint8_t*>(buf)), src, bytes);
+    }
+    int commit() const {
+        YGZB_CUDA(ctx, cudaMemcpyAsync(buf, stage, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
+        return YGZB_OK;
+    }
+};
+
+// `kernel` on n_ctas CTAs of `threads` threads, grouped into clusters of `cluster` CTAs (n_ctas is a multiple of it)
+template <typename... Params, typename... Args>
+cudaError_t launch_cluster(void (*kernel)(Params...), unsigned n_ctas, unsigned threads, int cluster, size_t smem_bytes, cudaStream_t stream,
+                           Args&&... args) {
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(n_ctas);
+    cfg.blockDim = dim3(threads);
+    cfg.dynamicSmemBytes = smem_bytes;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = cluster;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+}
+
+// cluster-size tuning knobs (YGZB_BA_CLUSTER, YGZB_TRACK_CLUSTER): the variable's value if it is 1, 2, 4 or 8 -- or 16 where
+// the kernel can run on the non-portable size --, `dflt` if it is unset or anything else
+inline int cluster_knob(const char* name, int dflt, bool allow_16) {
+    if (const char* e = getenv(name)) {
+        const int v = atoi(e);
+        if (v == 1 || v == 2 || v == 4 || v == 8 || (allow_16 && v == 16)) return v;
+    }
+    return dflt;
+}
 
 // device helpers shared by kernels ---------------------------------------------------------------
 __device__ __forceinline__ unsigned float_orderable(float f) {

@@ -739,28 +739,29 @@ int ygzb_initializer_ransac(ygzb_ctx* ctx, int n_lists, const int32_t* offsets, 
                 if (sets[p * I * 8 + k] < 0 || sets[p * I * 8 + k] >= n) return set_error(ctx, YGZB_ERR_INVALID, "initializer: set index out of range (list %zu)", p);
         }
         const size_t Hn = P * I * 2;
-        Carver sz(nullptr);
-        sz.take<int32_t>(P + 1); sz.take<double>(2 * N); sz.take<double>(2 * N); sz.take<double>(2 * N); sz.take<double>(2 * N);
-        sz.take<int32_t>(P * I * 8); sz.take<Norm>(P); sz.take<double>(9 * Hn); sz.take<double>(9 * Hn); sz.take<float>(Hn);
-        sz.take<double>(18 * P); sz.take<float>(2 * P); sz.take<int32_t>(2 * P); sz.take<uint8_t>(N); sz.take<uint8_t>(N);
-        void* buf = dev_scratch(ctx, 6, sz.bytes());
+        int32_t *d_off, *d_sets, *d_obest;
+        double *d_px1, *d_px2, *d_pn1, *d_pn2, *d_models, *d_aux, *d_out;
+        Norm* d_norm;
+        float *d_scores, *d_oscore;
+        uint8_t *d_inlH, *d_inlF;
+        void* buf = carve_scratch(ctx, 6, [&](Carver& c) {
+            d_off = c.take<int32_t>(P + 1);
+            d_px1 = c.take<double>(2 * N);
+            d_px2 = c.take<double>(2 * N);
+            d_pn1 = c.take<double>(2 * N);
+            d_pn2 = c.take<double>(2 * N);
+            d_sets = c.take<int32_t>(P * I * 8);
+            d_norm = c.take<Norm>(P);
+            d_models = c.take<double>(9 * Hn);
+            d_aux = c.take<double>(9 * Hn);
+            d_scores = c.take<float>(Hn);
+            d_out = c.take<double>(18 * P);
+            d_oscore = c.take<float>(2 * P);
+            d_obest = c.take<int32_t>(2 * P);
+            d_inlH = c.take<uint8_t>(N);
+            d_inlF = c.take<uint8_t>(N);
+        });
         if (!buf) return YGZB_ERR_CUDA;
-        Carver c(buf);
-        int32_t* d_off = c.take<int32_t>(P + 1);
-        double* d_px1 = c.take<double>(2 * N);
-        double* d_px2 = c.take<double>(2 * N);
-        double* d_pn1 = c.take<double>(2 * N);
-        double* d_pn2 = c.take<double>(2 * N);
-        int32_t* d_sets = c.take<int32_t>(P * I * 8);
-        Norm* d_norm = c.take<Norm>(P);
-        double* d_models = c.take<double>(9 * Hn);
-        double* d_aux = c.take<double>(9 * Hn);
-        float* d_scores = c.take<float>(Hn);
-        double* d_out = c.take<double>(18 * P);
-        float* d_oscore = c.take<float>(2 * P);
-        int32_t* d_obest = c.take<int32_t>(2 * P);
-        uint8_t* d_inlH = c.take<uint8_t>(N);
-        uint8_t* d_inlF = c.take<uint8_t>(N);
         YGZB_CUDA(ctx, cudaMemcpyAsync(d_off, offsets, (P + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
         YGZB_CUDA(ctx, cudaMemcpyAsync(d_px1, px1, 16 * N, cudaMemcpyHostToDevice, ctx->stream));
         YGZB_CUDA(ctx, cudaMemcpyAsync(d_px2, px2, 16 * N, cudaMemcpyHostToDevice, ctx->stream));
@@ -820,31 +821,31 @@ int ygzb_initializer_reconstruct(ygzb_ctx* ctx, int n_lists, const int32_t* offs
         if (rc != YGZB_OK) return rc;
         const size_t P = (size_t)n_lists, N = (size_t)offsets[n_lists];
         if (N == 0) return set_error(ctx, YGZB_ERR_INVALID, "initializer_reconstruct: no point pairs");
-        Carver sz(nullptr);
-        sz.take<int32_t>(P + 1); sz.take<double>(2 * N); sz.take<double>(2 * N); sz.take<int32_t>(P); sz.take<double>(9 * P); sz.take<uint8_t>(N);
-        sz.take<double>(8 * 3 * N); sz.take<uint8_t>(8 * N); sz.take<float>(8 * N); sz.take<int32_t>(P); sz.take<double>(9 * P);
-        sz.take<double>(3 * P); sz.take<double>(3 * N); sz.take<uint8_t>(N); sz.take<int32_t>(8 * P); sz.take<double>(P); sz.take<double>(96 * P);
-        void* buf = dev_scratch(ctx, 6, sz.bytes());
-        if (!buf) return YGZB_ERR_CUDA;
-        Carver c(buf);
         ReconArgs a;
-        int32_t* d_off = c.take<int32_t>(P + 1);
-        double* d_px1 = c.take<double>(2 * N);
-        double* d_px2 = c.take<double>(2 * N);
-        int32_t* d_use = c.take<int32_t>(P);
-        double* d_model = c.take<double>(9 * P);
-        uint8_t* d_inl = c.take<uint8_t>(N);
-        a.p3d_all = c.take<double>(8 * 3 * N);
-        a.good_all = c.take<uint8_t>(8 * N);
-        a.cos_all = c.take<float>(8 * N);
-        a.ok = c.take<int32_t>(P);
-        a.R21 = c.take<double>(9 * P);
-        a.t21 = c.take<double>(3 * P);
-        a.p3d = c.take<double>(3 * N);
-        a.triangulated = c.take<uint8_t>(N);
-        a.n_good = c.take<int32_t>(8 * P);
-        a.parallax = c.take<double>(P);
-        a.candidates = candidates ? c.take<double>(96 * P) : nullptr;
+        int32_t *d_off, *d_use;
+        double *d_px1, *d_px2, *d_model;
+        uint8_t* d_inl;
+        void* buf = carve_scratch(ctx, 6, [&](Carver& c) {
+            d_off = c.take<int32_t>(P + 1);
+            d_px1 = c.take<double>(2 * N);
+            d_px2 = c.take<double>(2 * N);
+            d_use = c.take<int32_t>(P);
+            d_model = c.take<double>(9 * P);
+            d_inl = c.take<uint8_t>(N);
+            a.p3d_all = c.take<double>(8 * 3 * N);
+            a.good_all = c.take<uint8_t>(8 * N);
+            a.cos_all = c.take<float>(8 * N);
+            a.ok = c.take<int32_t>(P);
+            a.R21 = c.take<double>(9 * P);
+            a.t21 = c.take<double>(3 * P);
+            a.p3d = c.take<double>(3 * N);
+            a.triangulated = c.take<uint8_t>(N);
+            a.n_good = c.take<int32_t>(8 * P);
+            a.parallax = c.take<double>(P);
+            a.candidates = c.take<double>(96 * P);   // (laid out whether or not the caller asks for them)
+        });
+        if (!buf) return YGZB_ERR_CUDA;
+        if (!candidates) a.candidates = nullptr;
         a.off = d_off; a.px1 = d_px1; a.px2 = d_px2; a.use_h = d_use; a.model = d_model; a.inliers = d_inl;
         a.K[0] = ctx->prm.fx; a.K[1] = ctx->prm.fy; a.K[2] = ctx->prm.cx; a.K[3] = ctx->prm.cy;
         a.sigma2 = sigma2; a.min_parallax = min_parallax; a.min_triangulated = min_triangulated; a.ratio_h = good_point_ratio_h;

@@ -310,22 +310,23 @@ static int klt_impl(ygzb_frames* f, int n_pairs, const int32_t* ref_slot, const 
         extra_bytes += ((size_t)a.lv[L].pitch * a.lv[L].h + 255) & ~(size_t)255;
     }
     const size_t T = (size_t)total;
-    Carver sz(nullptr);
-    sz.take<uint8_t>(extra_bytes * n_img); sz.take<const uint8_t*>((size_t)n_img * kMaxKltLevels); sz.take<int32_t>(2 * T);
-    sz.take<float>(2 * T); sz.take<float>(2 * T); sz.take<uint8_t>(T); sz.take<float>(T);
-    sz.take<const uint8_t*>((size_t)n_img); sz.take<uint8_t*>((size_t)n_img);
-    void* buf = dev_scratch(ctx, 6, sz.bytes());
+    uint8_t *d_extra, *d_status;
+    const uint8_t **d_ptrs, **d_src;
+    uint8_t** d_dst;
+    int32_t* d_img;
+    float *d_ref, *d_cur, *d_err;
+    void* buf = carve_scratch(ctx, 6, [&](Carver& c) {
+        d_extra = c.take<uint8_t>(extra_bytes * n_img);
+        d_ptrs = c.take<const uint8_t*>((size_t)n_img * kMaxKltLevels);
+        d_img = c.take<int32_t>(2 * T);
+        d_ref = c.take<float>(2 * T);
+        d_cur = c.take<float>(2 * T);
+        d_status = c.take<uint8_t>(T);
+        d_err = c.take<float>(T);
+        d_src = c.take<const uint8_t*>((size_t)n_img);
+        d_dst = c.take<uint8_t*>((size_t)n_img);
+    });
     if (!buf) return YGZB_ERR_CUDA;
-    Carver c(buf);
-    uint8_t* d_extra = c.take<uint8_t>(extra_bytes * n_img);
-    const uint8_t** d_ptrs = c.take<const uint8_t*>((size_t)n_img * kMaxKltLevels);
-    int32_t* d_img = c.take<int32_t>(2 * T);
-    float* d_ref = c.take<float>(2 * T);
-    float* d_cur = c.take<float>(2 * T);
-    uint8_t* d_status = c.take<uint8_t>(T);
-    float* d_err = c.take<float>(T);
-    const uint8_t** d_src = c.take<const uint8_t*>((size_t)n_img);
-    uint8_t** d_dst = c.take<uint8_t*>((size_t)n_img);
     std::vector<const uint8_t*> ptrs((size_t)n_img * kMaxKltLevels, nullptr);
     for (int im = 0; im < n_img; ++im) {
         const int slot = (im & 1) ? cur_slot[im / 2] : ref_slot[im / 2];

@@ -644,10 +644,16 @@ int check_reference_call(ygzb_tracker* t, int stream, const ygzb_reference_recor
 
 }  // namespace
 
-size_t ref_store_bytes(const TrackStore& st) {
+// the previous-frame reference store of st.S streams (two records each, st.ref_cap features per record)
+void ref_store_carve(Carver& c, TrackStore& st) {
     const size_t R2 = 2 * (size_t)st.S, cap = st.ref_cap;
+    st.ref_px = c.take<double>(R2 * cap * 2); st.ref_depth = c.take<double>(R2 * cap); st.ref_n = c.take<int32_t>(R2);
+    st.ref_T = c.take<double>(R2 * 12); st.ref_cur = c.take<int32_t>(st.S);
+}
+
+size_t ref_store_bytes(TrackStore st) {
     Carver c(nullptr);
-    c.take<double>(R2 * cap * 2); c.take<double>(R2 * cap); c.take<int32_t>(R2); c.take<double>(R2 * 12); c.take<int32_t>(st.S);
+    ref_store_carve(c, st);
     return (c.bytes() + 255) & ~(size_t)255;
 }
 
@@ -740,11 +746,7 @@ int ygzb_tracker_create(ygzb_frames* f, int n_streams, int max_jobs, const doubl
     t->f = f;
     t->ctx = ctx;
     t->max_jobs = max_jobs;
-    t->cluster = kTrackCluster;
-    if (const char* e = getenv("YGZB_TRACK_CLUSTER")) {   // tuning knob: 1, 2, 4 or 8
-        const int v = atoi(e);
-        if (v == 1 || v == 2 || v == 4 || v == 8) t->cluster = v;
-    }
+    t->cluster = cluster_knob("YGZB_TRACK_CLUSTER", kTrackCluster, false);
     const Geometry& g = ctx->geo;
     const size_t S = (size_t)n_streams, R = YGZB_TRACK_RING, cells = (size_t)g.n_cells, E = S * R, cap = kTrackMaxLocal * cells;
     TrackStore& st = t->st;
@@ -752,18 +754,19 @@ int ygzb_tracker_create(ygzb_frames* f, int n_streams, int max_jobs, const doubl
     st.fx = K[0]; st.fy = K[1]; st.cx = K[2]; st.cy = K[3];
     int rc = YGZB_OK;
     {
-        Carver sz(nullptr);
-        sz.take<double>(E * 12); sz.take<int32_t>(E); sz.take<int32_t>(E); sz.take<long long>(E); sz.take<double>(E * cells * 2);
-        sz.take<uint8_t>(E * cells); sz.take<double>(E * cells); sz.take<double>(E * cells * 3); sz.take<int32_t>(E);
-        sz.take<long long>(E * cap); sz.take<double>(E * cap * 2);
-        rc = check_cuda(ctx, cudaMalloc(&t->d_store, sz.bytes()), "cudaMalloc(tracker store)");
-        if (rc == YGZB_OK) rc = check_cuda(ctx, cudaMemsetAsync(t->d_store, 0, sz.bytes(), ctx->stream), "memset");
-        if (rc == YGZB_OK) {
-            Carver c(t->d_store);
+        auto carve = [&](Carver& c) {
             st.kf_T = c.take<double>(E * 12); st.kf_n = c.take<int32_t>(E); st.kf_slot = c.take<int32_t>(E); st.kf_mp0 = c.take<long long>(E);
             st.kf_px = c.take<double>(E * cells * 2); st.kf_level = c.take<uint8_t>(E * cells); st.kf_depth = c.take<double>(E * cells);
             st.kf_pw = c.take<double>(E * cells * 3); st.kf_nobs = c.take<int32_t>(E); st.kf_obs_id = c.take<long long>(E * cap);
             st.kf_obs_px = c.take<double>(E * cap * 2);
+        };
+        Carver sz(nullptr);
+        carve(sz);
+        rc = check_cuda(ctx, cudaMalloc(&t->d_store, sz.bytes()), "cudaMalloc(tracker store)");
+        if (rc == YGZB_OK) rc = check_cuda(ctx, cudaMemsetAsync(t->d_store, 0, sz.bytes(), ctx->stream), "memset");
+        if (rc == YGZB_OK) {
+            Carver c(t->d_store);
+            carve(c);
         }
     }
     if (rc == YGZB_OK) rc = dalloc(ctx, &t->d_depth, S * g.W * g.H);
@@ -888,9 +891,7 @@ int ygzb_tracker_set_reference_mode(ygzb_tracker* t, int mode, const int32_t* re
             return rc;
         }
         Carver c(t->d_ref);
-        const size_t R2 = 2 * (size_t)S, cap = st.ref_cap;
-        st.ref_px = c.take<double>(R2 * cap * 2); st.ref_depth = c.take<double>(R2 * cap); st.ref_n = c.take<int32_t>(R2);
-        st.ref_T = c.take<double>(R2 * 12); st.ref_cur = c.take<int32_t>(S);
+        ref_store_carve(c, st);
         t->st = st;
     }
     t->ref_mode = mode;

@@ -142,21 +142,21 @@ int ygzb_search_for_triangulation(ygzb_ctx* ctx, int n_pairs, const int32_t* off
     if (!desc1 || !px1 || !node1 || !match12 || (N2 && (!desc2 || !px2 || !node2))) return YGZB_ERR_INVALID;
     int max1 = 0;
     for (size_t p = 0; p < P; ++p) max1 = std::max(max1, off1[p + 1] - off1[p]);
-    Carver sz(nullptr);
-    sz.take<int32_t>(2 * (P + 1)); sz.take<double>(9 * P); sz.take<uint8_t>(32 * N1); sz.take<uint8_t>(32 * N2 + 32); sz.take<double>(2 * N1);
-    sz.take<double>(2 * N2 + 2); sz.take<int32_t>(N1); sz.take<int32_t>(N2 + 1); sz.take<int32_t>(N1);
-    void* buf = dev_scratch(ctx, 6, sz.bytes());
+    int32_t *d_off, *d_n1, *d_n2, *d_m;
+    double *d_E, *d_p1, *d_p2;
+    uint8_t *d_d1, *d_d2;
+    void* buf = carve_scratch(ctx, 6, [&](Carver& c) {
+        d_off = c.take<int32_t>(2 * (P + 1));
+        d_E = c.take<double>(9 * P);
+        d_d1 = c.take<uint8_t>(32 * N1);
+        d_d2 = c.take<uint8_t>(32 * N2 + 32);
+        d_p1 = c.take<double>(2 * N1);
+        d_p2 = c.take<double>(2 * N2 + 2);
+        d_n1 = c.take<int32_t>(N1);
+        d_n2 = c.take<int32_t>(N2 + 1);
+        d_m = c.take<int32_t>(N1);
+    });
     if (!buf) return YGZB_ERR_CUDA;
-    Carver c(buf);
-    int32_t* d_off = c.take<int32_t>(2 * (P + 1));
-    double* d_E = c.take<double>(9 * P);
-    uint8_t* d_d1 = c.take<uint8_t>(32 * N1);
-    uint8_t* d_d2 = c.take<uint8_t>(32 * N2 + 32);
-    double* d_p1 = c.take<double>(2 * N1);
-    double* d_p2 = c.take<double>(2 * N2 + 2);
-    int32_t* d_n1 = c.take<int32_t>(N1);
-    int32_t* d_n2 = c.take<int32_t>(N2 + 1);
-    int32_t* d_m = c.take<int32_t>(N1);
     auto H2D = [&](void* dst, const void* src, size_t bytes) {
         return bytes ? check_cuda(ctx, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, ctx->stream), "H2D") : YGZB_OK;
     };
@@ -186,18 +186,19 @@ int ygzb_depth_from_triangulation(ygzb_ctx* ctx, int n, int n_poses, const doubl
         for (int i = 0; i < n; ++i)
             if (pose_of[i] < 0 || pose_of[i] >= n_poses) return set_error(ctx, YGZB_ERR_INVALID, "pose_of[%d] out of range", i);
     const size_t N = (size_t)n, P = (size_t)n_poses;
-    Carver sz(nullptr);
-    sz.take<double>(12 * P); sz.take<int32_t>(N); sz.take<double>(3 * N); sz.take<double>(3 * N); sz.take<double>(N); sz.take<double>(N); sz.take<uint8_t>(N);
-    void* buf = dev_scratch(ctx, 6, sz.bytes());
+    double *d_T, *d_fr, *d_fc, *d_d1, *d_d2;
+    int32_t* d_po;
+    uint8_t* d_ok;
+    void* buf = carve_scratch(ctx, 6, [&](Carver& c) {
+        d_T = c.take<double>(12 * P);
+        d_po = c.take<int32_t>(N);
+        d_fr = c.take<double>(3 * N);
+        d_fc = c.take<double>(3 * N);
+        d_d1 = c.take<double>(N);
+        d_d2 = c.take<double>(N);
+        d_ok = c.take<uint8_t>(N);
+    });
     if (!buf) return YGZB_ERR_CUDA;
-    Carver c(buf);
-    double* d_T = c.take<double>(12 * P);
-    int32_t* d_po = c.take<int32_t>(N);
-    double* d_fr = c.take<double>(3 * N);
-    double* d_fc = c.take<double>(3 * N);
-    double* d_d1 = c.take<double>(N);
-    double* d_d2 = c.take<double>(N);
-    uint8_t* d_ok = c.take<uint8_t>(N);
     YGZB_CUDA(ctx, cudaMemcpyAsync(d_T, T_search_ref, 12 * P * 8, cudaMemcpyHostToDevice, ctx->stream));
     if (pose_of) YGZB_CUDA(ctx, cudaMemcpyAsync(d_po, pose_of, 4 * N, cudaMemcpyHostToDevice, ctx->stream));
     YGZB_CUDA(ctx, cudaMemcpyAsync(d_fr, f_ref, 24 * N, cudaMemcpyHostToDevice, ctx->stream));
