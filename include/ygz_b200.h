@@ -52,6 +52,8 @@ typedef struct {
 
 void ygzb_default_params(ygzb_params* p);
 int ygzb_create(int device, const ygzb_params* p, ygzb_ctx** out);
+/* the parameters the context was created with (image size and camera for callers that size their buffers from it) */
+int ygzb_get_params(const ygzb_ctx* ctx, ygzb_params* out);
 void ygzb_destroy(ygzb_ctx* ctx);
 const char* ygzb_last_error(const ygzb_ctx* ctx);
 int ygzb_synchronize(ygzb_ctx* ctx);

@@ -1,0 +1,87 @@
+/*
+ * ygz_vo.h -- streaming C API of libygz_vo.so: the device-resident tracking engine (host/vo_driver.cpp) fed frame by
+ * frame.  The reference's VisualOdometry::AddFrame (src/Module/VisualOdometry.cpp:38-107) takes one frame at a time; this
+ * API takes frames as they arrive, per stream, and runs them in the engine's rounds: per stream a window of queued frames
+ * up to the first one that may become a key-frame is tracked as one chain on the device, key-frames are inserted (Detect,
+ * depth-initialised map points, local BA) behind it, and the BA overlaps the next round's alignment.  The results are
+ * those of the batch entry points (ygz_vo_run_ex) on the same frames, whatever the pacing of push and step.
+ *
+ * Conventions are those of ygz_b200.h: YGZB_OK or a negative YGZB_ERR_* code, no exceptions, poses T_cw 3x4 row-major.
+ *
+ * Buffer lifetime: ygz_vo_push keeps the caller's pointers; no host copy is made.  An image and a depth map must stay
+ * valid and unchanged until ygz_vo_poll has returned the result of that frame (the reference's Frame owns its _color and
+ * _depth the same way).  Page-locked buffers (ygzb_host_alloc) make the uploads asynchronous.
+ *
+ * Depth: a frame's depth map (image_width * image_height doubles, metres, host or device memory) initialises the map
+ * points of the key-frame the frame becomes; it is uploaded (ygzb_tracker_set_depth) only then, right before the
+ * key-frame insertion.  NULL means the stream's current depth map stays valid: that of the last key-frame that had one.
+ * A stream's first frame always becomes a key-frame, so it must have a depth map.
+ *
+ * Results: come out in frame order within each stream, each frame exactly once, and only when final.  A key-frame's pose
+ * is its pose after its local BA, the value ygz_vo_run writes to its trajectory.  Once a stream is lost (its alignment
+ * moved too far, or pose-only kept fewer than min_inliers inliers), that frame and every later one report
+ * YGZ_VO_LOST with the last pose.  `frame` counts the stream's pushes from 0.
+ *
+ * Threading: one ygz_vo per context and host thread; the context's stream carries all of its work.
+ */
+#ifndef YGZ_VO_H_
+#define YGZ_VO_H_
+
+#include <stdint.h>
+
+#include "ygz_b200.h"
+
+#ifdef __cplusplus
+extern "C" {
+#endif
+
+typedef struct ygz_vo ygz_vo;
+
+typedef struct {
+    int n_streams;          /* independent sequences, >= 1                                                          */
+    int window;             /* frames of one stream tracked per round at most, >= 1 (a result never depends on it)   */
+    int ref_mode;           /* YGZB_TRACK_REF_KEYFRAME or YGZB_TRACK_REF_PREVIOUS (ygzb_tracker_set_reference_mode)  */
+    int kf_min_frames;      /* NeedNewKeyFrame (VisualOdometry.cpp:304-321): frames since the last key-frame ...       */
+    double kf_min_rot, kf_min_trans;   /* ... and the rotation (rad) or translation (m) from it that make a key-frame */
+    int min_inliers;        /* pose-only inliers below which a stream is lost (vo.keyframe.min_features, 30)         */
+    double K[4];            /* fx, fy, cx, cy in double; must round to the context's float fx..cy                   */
+} ygz_vo_config;
+
+#define YGZ_VO_TRACKED 0
+#define YGZ_VO_KEYFRAME 1
+#define YGZ_VO_LOST 2
+typedef struct {
+    int32_t stream, frame;
+    int64_t tag;            /* the caller's tag of the frame (ygz_vo_push)                                          */
+    int32_t status;         /* YGZ_VO_TRACKED, YGZ_VO_KEYFRAME or YGZ_VO_LOST                                       */
+    int32_t n_inliers;      /* pose-only inliers (0 for a stream's first frame)                                     */
+    double T_cw[12];
+} ygz_vo_result;
+
+/* A tracker on `ctx` for cfg->n_streams streams; the image size is the context's (ygzb_params image_width/height).
+ * YGZB_ERR_INVALID for a NULL argument or a config that does not match the context.                                 */
+int ygz_vo_create(ygzb_ctx* ctx, const ygz_vo_config* cfg, ygz_vo** out);
+/* queues a grey image (image_width * image_height bytes, host or device memory) of `stream`.  Nothing runs until
+ * ygz_vo_step or ygz_vo_flush.  YGZB_ERR_INVALID, with nothing queued, for a stream out of range, a NULL image, or a NULL
+ * depth on a stream that has no depth map yet.                                                                      */
+int ygz_vo_push(ygz_vo* vo, int stream, const uint8_t* image, const double* depth, int64_t tag);
+/* one round over what is queued, with one host synchronisation: the results of the windows it tracks are final on
+ * return, except a frame that triggers a key-frame, whose insertion is enqueued by the next round.                 */
+int ygz_vo_step(ygz_vo* vo);
+/* rounds until nothing is queued or in flight: every pushed frame has its result                                    */
+int ygz_vo_flush(ygz_vo* vo);
+/* moves up to `capacity` final results, oldest first, into `out`; *n = how many                                     */
+int ygz_vo_poll(ygz_vo* vo, ygz_vo_result* out, int capacity, int* n);
+/* the 16 counters ygz_vo_run reports per stream: lost, key-frames, local BAs, candidates, projected, inliers, BA
+ * observations, BA points, BA key-frames, BA LM trials, BA iterations, BA model FLOP, 0, 0, 0, 0                  */
+int ygz_vo_stream_stats(ygz_vo* vo, int stream, int64_t stats[16]);
+/* the local map of `stream` (every key-frame still in its ring, oldest first) into `out`, sized for YGZB_TRACK_RING
+ * key-frames (ygzb_tracker_export): asynchronous, valid after ygzb_synchronize(ctx); call after ygz_vo_flush         */
+int ygz_vo_export_map(ygz_vo* vo, int stream, ygzb_map_record* out);
+void ygz_vo_destroy(ygz_vo* vo);
+
+#ifdef __cplusplus
+}
+#endif
+
+#endif /* YGZ_VO_H_ */

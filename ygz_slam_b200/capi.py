@@ -33,7 +33,7 @@ class Keypoints(C.Structure):
 
 # every symbol include/ygz_b200.h declares (tests check that the library exports all of them)
 EXPORTS = [
-    "ygzb_default_params", "ygzb_create", "ygzb_destroy", "ygzb_last_error", "ygzb_synchronize", "ygzb_stream",
+    "ygzb_default_params", "ygzb_create", "ygzb_get_params", "ygzb_destroy", "ygzb_last_error", "ygzb_synchronize", "ygzb_stream",
     "ygzb_launch_count", "ygzb_timer_start", "ygzb_timer_stop", "ygzb_profile_enable", "ygzb_profile_read", "ygzb_profile_stage_count",
     "ygzb_profile_stage_name", "ygzb_host_alloc", "ygzb_host_free", "ygzb_frames_create", "ygzb_frames_destroy",
     "ygzb_frames_upload", "ygzb_frames_copy", "ygzb_frames_build_pyramid", "ygzb_frames_layout", "ygzb_frames_device_ptr",

@@ -333,6 +333,12 @@ int ygzb_host_alloc(void** ptr, size_t bytes) {
 }
 int ygzb_host_free(void* ptr) { return cudaFreeHost(ptr) == cudaSuccess ? YGZB_OK : YGZB_ERR_CUDA; }
 
+int ygzb_get_params(const ygzb_ctx* ctx, ygzb_params* out) {
+    if (!ctx || !out) return YGZB_ERR_INVALID;
+    *out = ctx->prm;
+    return YGZB_OK;
+}
+
 int ygzb_grid_dims(const ygzb_ctx* ctx, int* rows, int* cols) {
     if (!ctx) return YGZB_ERR_INVALID;
     if (rows) *rows = ctx->geo.grid_rows;

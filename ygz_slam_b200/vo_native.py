@@ -34,6 +34,15 @@ def _lib():
         _LIB.ygz_vo_run_stages.restype = C.c_int
         _LIB.ygz_vo_run_stages.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                            C.c_double, C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        _LIB.ygz_vo_create.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        _LIB.ygz_vo_push.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int64]
+        _LIB.ygz_vo_step.argtypes = [C.c_void_p]
+        _LIB.ygz_vo_flush.argtypes = [C.c_void_p]
+        _LIB.ygz_vo_poll.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+        _LIB.ygz_vo_stream_stats.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        _LIB.ygz_vo_export_map.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        _LIB.ygz_vo_destroy.argtypes = [C.c_void_p]
+        _LIB.ygz_vo_destroy.restype = None
     return _LIB
 
 
@@ -120,3 +129,101 @@ def _result(traj, stats, totals, sec, dev_ms, S, n, details, return_device_ms):
         return out + (dict(device_ms=dev_ms.value, gpu_launches=int(totals[0]), h2d_image_bytes=int(totals[1]),
                            h2d_other_bytes=int(totals[2]), d2h_bytes=int(totals[3])),)
     return out + (dev_ms.value,) if return_device_ms else out
+
+
+class VoConfig(C.Structure):
+    _fields_ = [("n_streams", C.c_int), ("window", C.c_int), ("ref_mode", C.c_int), ("kf_min_frames", C.c_int), ("kf_min_rot", C.c_double),
+                ("kf_min_trans", C.c_double), ("min_inliers", C.c_int), ("K", C.c_double * 4)]
+
+
+STATUS = ("tracked", "keyframe", "lost")   # YGZ_VO_TRACKED / _KEYFRAME / _LOST
+RESULT_DTYPE = np.dtype([("stream", np.int32), ("frame", np.int32), ("tag", np.int64), ("status", np.int32), ("n_inliers", np.int32),
+                         ("T_cw", np.float64, (12,))])   # ygz_vo_result
+_STAT_KEYS = ("lost", "keyframes", "ba", "candidates", "projected", "inliers", "ba_obs", "ba_pts", "ba_kfs", "ba_trials", "ba_iters", "ba_flops")
+
+
+class Engine:
+    """The device-resident engine fed frame by frame (include/ygz_vo.h): push frames per stream as they arrive, step or
+    flush, poll the final results.  The image size is the context's; K (fx, fy, cx, cy in double) defaults to the
+    context's camera at the shortest decimal that rounds to it (520.9 for the float 520.9f), which is the TUM camera the
+    batch functions (run) use.  The pushed arrays are kept alive here until their results have been polled."""
+
+    def __init__(self, ctx, n_streams, window=8, ref_mode="keyframe", kf_min_frames=10, kf_min_rot=0.1, kf_min_trans=0.1,
+                 min_inliers=30, K=None):
+        if ref_mode not in _REF_MODES:
+            raise ValueError(f"ref_mode must be 'keyframe' or 'previous', not {ref_mode!r}")
+        p = ctx.params
+        if K is None:
+            K = [float(str(np.float32(v))) for v in (p.fx, p.fy, p.cx, p.cy)]
+        self.ctx, self.n_streams, self.shape = ctx, int(n_streams), (p.image_height, p.image_width)
+        self.cfg = VoConfig(int(n_streams), int(window), _REF_MODES[ref_mode], int(kf_min_frames), float(kf_min_rot), float(kf_min_trans),
+                            int(min_inliers), (C.c_double * 4)(*map(float, K)))
+        self.lib = _lib()
+        self.h = C.c_void_p()
+        ctx.check(self.lib.ygz_vo_create(ctx.h, C.byref(self.cfg), C.byref(self.h)), "ygz_vo_create")
+        self._pushed = [0] * self.n_streams
+        self._alive = {}   # (stream, frame) -> the arrays its result still needs
+
+    def push(self, stream, image, depth=None, tag=None):
+        """Queue grey `image` (H, W) uint8 of `stream` with its depth map (H, W) float64, or None to keep the stream's current
+        map.  Returns the frame's index in its stream; tag (default: that index) comes back with its result."""
+        if not 0 <= stream < self.n_streams:
+            raise ValueError(f"stream {stream} out of range [0, {self.n_streams})")
+        img = np.ascontiguousarray(image, np.uint8)
+        dep = None if depth is None else np.ascontiguousarray(depth, np.float64)
+        if img.shape != self.shape or (dep is not None and dep.shape != self.shape):
+            raise ValueError(f"image and depth must be {self.shape}")
+        frame = self._pushed[stream]
+        tag = frame if tag is None else int(tag)
+        self.ctx.check(self.lib.ygz_vo_push(self.h, int(stream), img.ctypes.data, None if dep is None else dep.ctypes.data, tag),
+                       "ygz_vo_push")
+        self._alive[(stream, frame)] = (img, dep)
+        self._pushed[stream] += 1
+        return frame
+
+    def step(self):
+        self.ctx.check(self.lib.ygz_vo_step(self.h), "ygz_vo_step")
+
+    def flush(self):
+        self.ctx.check(self.lib.ygz_vo_flush(self.h), "ygz_vo_flush")
+
+    def poll(self, capacity=4096):
+        """Final results since the last poll, oldest first: a RESULT_DTYPE array (status indexes STATUS)."""
+        out = []
+        while True:
+            buf = np.zeros(capacity, RESULT_DTYPE)
+            n = C.c_int(0)
+            self.ctx.check(self.lib.ygz_vo_poll(self.h, buf.ctypes.data, capacity, C.byref(n)), "ygz_vo_poll")
+            out.append(buf[:n.value])
+            if n.value < capacity:
+                break
+        res = np.concatenate(out)
+        for s_, f in zip(res["stream"].tolist(), res["frame"].tolist()):
+            self._alive.pop((s_, f), None)
+        return res
+
+    def stats(self, stream):
+        """The counters of ygz_vo_run for one stream, as run's dicts."""
+        row = np.zeros(16, np.int64)
+        self.ctx.check(self.lib.ygz_vo_stream_stats(self.h, int(stream), row.ctypes.data), "ygz_vo_stream_stats")
+        return dict(zip(_STAT_KEYS, map(int, row[:12])))
+
+    def export_map(self, stream):
+        """The stream's local map (every key-frame still in its ring, oldest first) as a capi.MapBuffers; call after flush."""
+        from .capi import TRACK_RING, MapBuffers
+        m = MapBuffers(TRACK_RING, self.shape[1], self.shape[0], self.ctx.n_cells)
+        self.ctx.check(self.lib.ygz_vo_export_map(self.h, int(stream), C.byref(m.rec)), "ygz_vo_export_map")
+        self.ctx.synchronize()
+        return m
+
+    def close(self):
+        if self.h:
+            self.lib.ygz_vo_destroy(self.h)
+            self.h = C.c_void_p()
+        self._alive.clear()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
