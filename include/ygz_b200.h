@@ -418,7 +418,8 @@ typedef struct {
     int32_t kf_slot;       /* slot that keeps its pyramid from now on (copied device-to-device)             */
     int32_t entry;         /* ring entry to (over)write                                                     */
     int32_t track_job;     /* job index in the LAST ygzb_tracker_track batch whose pose and inlier observations
-                              the key-frame takes over, or -1: first key-frame (identity pose, nothing tracked) */
+                              the key-frame takes over, or -1: first key-frame (at the stream's start pose,
+                              ygzb_tracker_set_start_pose; nothing tracked)                                  */
     int32_t n_local;       /* local key-frames AFTER the insertion, oldest first (the last one is `entry`)  */
     int32_t local_entry[YGZB_TRACK_RING];
     int32_t run_ba;        /* non-zero: LocalBAG2O over the local key-frames                                */
@@ -439,6 +440,14 @@ void ygzb_tracker_destroy(ygzb_tracker* t);
 /* depth image (image_width * image_height doubles, host or device) that initialises the map points of the next key-frame
  * of `stream` (the reference's drivers read it from the TUM depth frame, test/test_feature_alignment.cpp:72-85)   */
 int ygzb_tracker_set_depth(ygzb_tracker* t, int stream, const double* depth);
+/* T_cw (3x4 row-major) that the next first key-frame of `stream` (a key-frame job with track_job = -1) takes: it places a
+ * sequence in the caller's world frame, as the reference's drivers do for their first frame
+ * (test/test_feature_alignment.cpp:63); the key-frame's map points go to that world frame.  Identity from
+ * ygzb_tracker_create.  Like ygzb_tracker_set_depth it applies to the insertions enqueued after it: the pose is read
+ * before the call returns and travels with the key-frame jobs, so a later call never changes an insertion already
+ * enqueued.  YGZB_ERR_INVALID, with the tracker untouched, for a NULL tracker or pose, a stream out of range, an entry
+ * that is not finite, or a rotation that is not orthonormal with determinant +1 (within 1e-6 per entry).           */
+int ygzb_tracker_set_start_pose(ygzb_tracker* t, int stream, const double T_cw[12]);
 /* host -> device copy of `count` grey frames into slots [first, first+count) and their pyramids, like ygzb_frames_upload,
  * but on the tracker's second CUDA stream: behind the last key-frame insertion and tracking chain (which still read the
  * slots), concurrent with a local BA in flight.  ygzb_tracker_track orders itself behind these uploads.              */

@@ -20,7 +20,12 @@
  * Results: come out in frame order within each stream, each frame exactly once, and only when final.  A key-frame's pose
  * is its pose after its local BA, the value ygz_vo_run writes to its trajectory.  Once a stream is lost (its alignment
  * moved too far, or pose-only kept fewer than min_inliers inliers), that frame and every later one report
- * YGZ_VO_LOST with the last pose.  `frame` counts the stream's pushes from 0.
+ * YGZ_VO_LOST with the last pose, until ygz_vo_restart starts a new sequence.  `frame` counts the stream's pushes from
+ * 0, across restarts.
+ *
+ * Sequences: a stream's first frame becomes its first key-frame at the identity pose, or at the pose ygz_vo_restart set
+ * before that push.  ygz_vo_restart on a stream that has frames starts a new sequence at the next push: nothing is
+ * matched against the old one and none of its map is reused; the stream is bootstrapped exactly as a fresh one.
  *
  * Threading: one ygz_vo per context and host thread; the context's stream carries all of its work.
  */
@@ -63,8 +68,24 @@ typedef struct {
 int ygz_vo_create(ygzb_ctx* ctx, const ygz_vo_config* cfg, ygz_vo** out);
 /* queues a grey image (image_width * image_height bytes, host or device memory) of `stream`.  Nothing runs until
  * ygz_vo_step or ygz_vo_flush.  YGZB_ERR_INVALID, with nothing queued, for a stream out of range, a NULL image, or a NULL
- * depth on a stream that has no depth map yet.                                                                      */
+ * depth on a stream that has no depth map yet or whose next frame starts a new sequence (ygz_vo_restart).          */
 int ygz_vo_push(ygz_vo* vo, int stream, const uint8_t* image, const double* depth, int64_t tag);
+/* starts a new sequence of `stream` whose first key-frame takes pose T_cw (3x4 row-major; NULL: identity), to place a
+ * sequence in the caller's world frame or to resume a lost stream, e.g. at the pose of its last YGZ_VO_LOST result.
+ *  - Barrier: the frames pushed before the call belong to the old sequence and get exactly the results they would get
+ *    without it -- tracked, key-frames (a pending key-frame insertion completes and its result comes first) or
+ *    YGZ_VO_LOST.  No round tracks frames of both sequences together.
+ *  - The first frame pushed after the call becomes the stream's first key-frame at T_cw; that push must bring a depth
+ *    map.  From then on the stream is a fresh one: empty local map, key-frame ring and slots reused from the start, map
+ *    point ids from 0, frames since the last key-frame, the lost flag and the previous-frame reference reset.  Its
+ *    results are those of a fresh engine fed the same frames; ygz_vo_export_map holds only the new key-frames.
+ *  - Before the stream's first push the call only sets the pose its first key-frame takes.  Of two calls with no push
+ *    in between, the last one counts.
+ *  - ygz_vo_stream_stats: counter 0 (lost) describes the current sequence, counter 12 counts the restarts that have
+ *    started a sequence, the other counters keep accumulating.
+ * The engine never restarts a stream by itself.  YGZB_ERR_INVALID, changing nothing, for a NULL vo, a stream out of
+ * range, a non-finite entry, or a rotation that is not orthonormal with determinant +1 (within 1e-6 per entry).      */
+int ygz_vo_restart(ygz_vo* vo, int stream, const double T_cw[12]);
 /* one round over what is queued, with one host synchronisation: the results of the windows it tracks are final on
  * return, except a frame that triggers a key-frame, whose insertion is enqueued by the next round.                 */
 int ygz_vo_step(ygz_vo* vo);
@@ -73,7 +94,8 @@ int ygz_vo_flush(ygz_vo* vo);
 /* moves up to `capacity` final results, oldest first, into `out`; *n = how many                                     */
 int ygz_vo_poll(ygz_vo* vo, ygz_vo_result* out, int capacity, int* n);
 /* the 16 counters ygz_vo_run reports per stream: lost, key-frames, local BAs, candidates, projected, inliers, BA
- * observations, BA points, BA key-frames, BA LM trials, BA iterations, BA model FLOP, 0, 0, 0, 0                  */
+ * observations, BA points, BA key-frames, BA LM trials, BA iterations, BA model FLOP, restarts (ygz_vo_restart),
+ * 0, 0, 0                                                                                                         */
 int ygz_vo_stream_stats(ygz_vo* vo, int stream, int64_t stats[16]);
 /* the local map of `stream` (every key-frame still in its ring, oldest first) into `out`, sized for YGZB_TRACK_RING
  * key-frames (ygzb_tracker_export): asynchronous, valid after ygzb_synchronize(ctx); call after ygz_vo_flush         */

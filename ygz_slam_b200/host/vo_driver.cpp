@@ -540,16 +540,20 @@ struct QFrame {
     const double* depth;   // NULL: the stream's current depth map stays valid
     int64_t tag;
     bool stacked;          // image lies in the caller's stacked sequence of the stream (one allocation, batch entry points)
+    bool restart = false;  // first frame of a new sequence (ygz_vo_restart): it becomes a first key-frame
 };
 struct EStream {
     std::deque<KfInfo> kfs;   // at most YGZB_TRACK_RING, the newest is the reference key-frame; the last kLocalKeyframes are local
     std::deque<QFrame> queue; // frames without a final result, oldest first; the first one is frame next_frame
     Mat34 T = identity();
+    Mat34 start = identity(); // pose of the next sequence's first key-frame (ygz_vo_restart)
+    std::deque<Mat34> starts; // poses of the queued frames that start a sequence (the stream's first, restarts), in order
     bool has_pose = false, lost = false, has_depth = false;
+    bool restart_pending = false;   // the next push starts a new sequence at `start`
     int frames_since_kf = 0, next_frame = 0;
     long next_mp = 0;
     long n_keyframes = 0, n_ba = 0, n_candidates = 0, n_projected = 0, n_inliers = 0;
-    long ba_obs = 0, ba_pts = 0, ba_kfs = 0, ba_trials = 0, ba_iters = 0;
+    long ba_obs = 0, ba_pts = 0, ba_kfs = 0, ba_trials = 0, ba_iters = 0, n_restarts = 0;
     double ba_flops = 0;
 };
 
@@ -606,10 +610,31 @@ class Engine {
     int height() const { return H_; }
     long long h2d_image_bytes = 0, h2d_other_bytes = 0, d2h_bytes = 0;
 
-    // queues frame (image, depth, tag) of tracker stream i; the caller has checked the arguments
+    // queues frame (image, depth, tag) of tracker stream i; the caller has checked the arguments.  The stream's first frame
+    // and the first one after a restart queue the pose their key-frame starts at
     void push(int i, const uint8_t* image, const double* depth, int64_t tag, bool stacked = false) {
-        st_[i].queue.push_back({image, depth, tag, stacked});
-        st_[i].has_depth |= depth != nullptr;
+        EStream& s = st_[i];
+        QFrame f{image, depth, tag, stacked};
+        if (pushed(i) == 0 || s.restart_pending) {
+            f.restart = s.restart_pending;
+            s.starts.push_back(s.start);
+            s.restart_pending = false;
+        }
+        s.queue.push_back(f);
+        s.has_depth |= depth != nullptr;
+    }
+    // frames pushed to stream i so far (those with a final result or a pending key-frame insertion, then the queued ones)
+    long pushed(int i) const { return st_[i].next_frame + (long)st_[i].queue.size(); }
+    // the next frame pushed to stream i starts a new sequence at T (before the stream's first push: its first sequence
+    // starts at T); the frames pushed before keep the results they would have had without the call.  The tracker checks
+    // T (finite, a rotation) and keeps it; that does not reach an insertion of the old sequence, because step 1 of a round
+    // sets every first key-frame's own pose right before its insertion
+    int restart(int i, const Mat34& T) {
+        CHK(ygzb_tracker_set_start_pose(tr_, i, T.m));
+        EStream& s = st_[i];
+        s.start = T;
+        s.restart_pending = pushed(i) > 0;
+        return YGZB_OK;
     }
     // final results go to `traj` (this group's [S][n_frames][12], rows in the caller's stream order; NULL: none) and, with
     // collect, to the result queue that pop_results drains
@@ -672,31 +697,36 @@ class Engine {
                     CHK(ygzb_tracker_set_depth(tr_, kjobs_[q].stream, kframes_[q].depth));
                     h2d_other_bytes += (long long)W_ * H_ * (long long)sizeof(double);
                 }
+                // a sequence's first key-frame starts at the pose its frame was pushed with
+                if (kjobs_[q].track_job < 0) CHK(ygzb_tracker_set_start_pose(tr_, kjobs_[q].stream, s.T.m));
             }
             CHK(ygzb_tracker_make_keyframes(tr_, (int)kjobs_.size(), kjobs_.data(), &ba_, h_kres_));
-            h2d_other_bytes += (long long)(kjobs_.size() * (sizeof(ygzb_keyframe_job) + 4));
+            // per job: the job, its start pose (staged behind the jobs in the same copy) and its problem index
+            h2d_other_bytes += (long long)(kjobs_.size() * (sizeof(ygzb_keyframe_job) + 12 * sizeof(double) + 4));
             d2h_bytes += (long long)(kjobs_.size() * sizeof(ygzb_keyframe_result));
         }
         // ---- 2. next window of every stream: uploads + tracking chain (asynchronous, right behind the key-frames)
         std::vector<ygzb_track_job> jobs;
         for (int i = 0; i < S_; ++i) {
             EStream& s = st_[i];
-            if (s.lost) {   // the reference keeps the last pose and reports VO_LOST
-                while (!s.queue.empty()) emit_front(i, YGZ_VO_LOST, 0);
-                continue;
-            }
+            if (s.lost)   // the reference keeps the last pose and reports VO_LOST, up to a restart
+                while (!s.queue.empty() && !s.queue.front().restart) emit_front(i, YGZ_VO_LOST, 0);
             if (s.queue.empty()) continue;
             // window: up to and including the first frame that may become a key-frame; past that point every frame may, and a
             // few frames are tracked speculatively -- the ones behind a key-frame trigger are dropped and tracked again against
-            // the new key-frame next round (results stay those of frame-by-frame processing); never more than is queued
+            // the new key-frame next round (results stay those of frame-by-frame processing); never more than is queued, and
+            // never past a restart.  A sequence's first frame is a window of its own
+            const bool first = s.kfs.empty() || s.queue.front().restart;
             int w = 1;
-            if (!s.kfs.empty()) {
+            if (!first) {
                 const int sure = prm_.kf_min_frames - s.frames_since_kf;
                 w = sure >= 1 ? std::min(F_, sure) : std::min(F_, kSpeculativeFrames);
+                for (int t = 1; t < w && t < (int)s.queue.size(); ++t)
+                    if (s.queue[t].restart) w = t;
             }
             w = std::min(w, (int)s.queue.size());
             CHK(upload(i, w));
-            if (s.kfs.empty()) {
+            if (first) {
                 wins_.push_back({i, s.next_frame, 1, -1});
                 continue;
             }
@@ -747,8 +777,17 @@ class Engine {
         // ---- 4. results of the tracking batch
         for (const Win& b : wins_) {
             EStream& s = st_[b.stream];
-            if (b.job0 < 0) {   // first frame of the stream: becomes the first key-frame (depth-initialised map)
-                s.T = identity();
+            if (b.job0 < 0) {   // first frame of a sequence: becomes its first key-frame (depth-initialised map)
+                const QFrame& f = s.queue.front();
+                if (f.restart) {   // the old sequence is final (its last insertion applied in step 3): start as a fresh stream
+                    s.kfs.clear();
+                    s.lost = false;
+                    s.frames_since_kf = 0;
+                    s.next_mp = 0;
+                    s.n_restarts += 1;
+                }
+                s.T = s.starts.front();
+                s.starts.pop_front();
                 s.has_pose = true;
                 pend_keyframe(b.stream, b.stream * F_, -1, 0);
                 continue;
@@ -792,6 +831,7 @@ class Engine {
         for (int c = 0; c < 16; ++c) o[c] = 0;
         o[0] = st.lost; o[1] = st.n_keyframes; o[2] = st.n_ba; o[3] = st.n_candidates; o[4] = st.n_projected; o[5] = st.n_inliers;
         o[6] = st.ba_obs; o[7] = st.ba_pts; o[8] = st.ba_kfs; o[9] = st.ba_trials; o[10] = st.ba_iters; o[11] = (int64_t)st.ba_flops;
+        o[12] = st.n_restarts;
     }
 
     // local map of stream i (every key-frame still in its ring, oldest first) into `rec`: asynchronous, valid after
@@ -1272,9 +1312,17 @@ int ygz_vo_create(ygzb_ctx* ctx, const ygz_vo_config* cfg, ygz_vo** out) {
 
 int ygz_vo_push(ygz_vo* vo, int stream, const uint8_t* image, const double* depth, int64_t tag) {
     if (!vo || stream < 0 || stream >= vo->n_streams || !image) return YGZB_ERR_INVALID;
-    if (!depth && !vo->eng->streams()[stream].has_depth) return YGZB_ERR_INVALID;
+    const EStream& s = vo->eng->streams()[stream];
+    if (!depth && (!s.has_depth || s.restart_pending)) return YGZB_ERR_INVALID;
     vo->eng->push(stream, image, depth, tag);
     return YGZB_OK;
+}
+
+int ygz_vo_restart(ygz_vo* vo, int stream, const double T_cw[12]) {
+    if (!vo || stream < 0 || stream >= vo->n_streams) return YGZB_ERR_INVALID;
+    Mat34 T = identity();
+    if (T_cw) std::memcpy(T.m, T_cw, sizeof(T.m));
+    return vo->eng->restart(stream, T);
 }
 
 int ygz_vo_step(ygz_vo* vo) {

@@ -62,6 +62,7 @@ class Stream:
     trajectory: list = field(default_factory=list)
     next_mp: int = 0
     last_obs: tuple = None      # (ids, px) of the inlier observations of the most recent tracked frame
+    start: np.ndarray = field(default_factory=lambda: np.eye(4)[:3].copy())   # T_cw of the first keyframe
     stats: dict = field(default_factory=lambda: dict(frames=0, keyframes=0, candidates=0, projected=0, inliers=0, ba=0))
 
 
@@ -101,6 +102,18 @@ class VisualOdometry:
             self.KF_MIN_TRANS = kf_min_trans
         self._slot_use = [0] * n_streams
 
+    def set_start_pose(self, i: int, T_cw):
+        """T_cw (3, 4) of stream i's first keyframe (identity by default), to place the sequence in the caller's world frame
+        as the reference's drivers do (test/test_feature_alignment.cpp:63); set it before the stream's first frame.  The
+        rules of ygzb_tracker_set_start_pose: finite, and a rotation (orthonormal, det +1) within 1e-6."""
+        T = np.array(T_cw, np.float64).reshape(3, 4)
+        R = T[:, :3]
+        if not np.all(np.isfinite(T)) or np.abs(R @ R.T - np.eye(3)).max() > 1e-6 or abs(np.linalg.det(R) - 1) > 1e-6:
+            raise ValueError("start pose must be finite with an orthonormal rotation of determinant +1")
+        if self.streams[i].keyframes:
+            raise RuntimeError(f"stream {i} has started already")
+        self.streams[i].start = T
+
     # ---- slot ring: current frame always goes to the next free slot of the stream -------------------------
     def _next_slot(self, si: int) -> int:
         st = self.streams[si]
@@ -123,7 +136,7 @@ class VisualOdometry:
         boot = [i for i in live if self.streams[i].ref is None]
         if boot:
             for i in boot:
-                self.streams[i].T_cw = np.eye(4)[:3].copy()
+                self.streams[i].T_cw = self.streams[i].start.copy()
             self._make_keyframes(boot, cur_slots, depths, frame_id, fresh=True)
         track = [i for i in live if i not in boot]
         if track:

@@ -36,6 +36,7 @@ def _lib():
                                            C.c_double, C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         _LIB.ygz_vo_create.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         _LIB.ygz_vo_push.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int64]
+        _LIB.ygz_vo_restart.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         _LIB.ygz_vo_step.argtypes = [C.c_void_p]
         _LIB.ygz_vo_flush.argtypes = [C.c_void_p]
         _LIB.ygz_vo_poll.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
@@ -181,6 +182,15 @@ class Engine:
         self._pushed[stream] += 1
         return frame
 
+    def restart(self, stream, T_cw=None):
+        """Start a new sequence of `stream` with the next push, whose frame becomes the first key-frame at T_cw (3, 4)
+        (None: identity) and must bring a depth map; frames pushed before keep their results (ygz_vo_restart).  Before
+        the stream's first push it only sets the pose of its first key-frame."""
+        if not 0 <= stream < self.n_streams:
+            raise ValueError(f"stream {stream} out of range [0, {self.n_streams})")
+        T = None if T_cw is None else np.ascontiguousarray(T_cw, np.float64).reshape(12)
+        self.ctx.check(self.lib.ygz_vo_restart(self.h, int(stream), None if T is None else T.ctypes.data), "ygz_vo_restart")
+
     def step(self):
         self.ctx.check(self.lib.ygz_vo_step(self.h), "ygz_vo_step")
 
@@ -207,6 +217,12 @@ class Engine:
         row = np.zeros(16, np.int64)
         self.ctx.check(self.lib.ygz_vo_stream_stats(self.h, int(stream), row.ctypes.data), "ygz_vo_stream_stats")
         return dict(zip(_STAT_KEYS, map(int, row[:12])))
+
+    def restarts(self, stream):
+        """How many restarts (ygz_vo_restart) have started a new sequence of `stream`: counter 12 of ygz_vo_stream_stats."""
+        row = np.zeros(16, np.int64)
+        self.ctx.check(self.lib.ygz_vo_stream_stats(self.h, int(stream), row.ctypes.data), "ygz_vo_stream_stats")
+        return int(row[12])
 
     def export_map(self, stream):
         """The stream's local map (every key-frame still in its ring, oldest first) as a capi.MapBuffers; call after flush."""
