@@ -48,7 +48,8 @@ def needs_build() -> bool:
 
 def build(force: bool = False, verbose: bool = False) -> Path:
     if not force and not needs_build():
-        vo_deps = [HERE / "host" / "vo_driver.cpp", HERE / "host" / "e2e_driver.cpp", HERE.parent / "include" / "ygz_vo.h"]
+        vo_deps = [HERE / "host" / "vo_driver.cpp", HERE / "host" / "e2e_driver.cpp", HERE / "host" / "timed_threads.h",
+                   HERE.parent / "include" / "ygz_vo.h"]
         if not VO_LIB.exists() or VO_LIB.stat().st_mtime < max(d.stat().st_mtime for d in vo_deps):
             build_vo_driver()
         return LIB

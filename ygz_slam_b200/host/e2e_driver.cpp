@@ -7,13 +7,11 @@
 // Per step and thread:  ygzb_frames_upload (pinned host -> device, pyramid)  ->  ygzb_detect (results to host)
 //                   ->  ygzb_match_frames (frame i against frame i+1 of the slice, cross-checked, results to host)
 // Build: host C++ only, part of libygz_vo.so (ygz_slam_b200/build.py).
-#include <barrier>
-#include <chrono>
 #include <cstdint>
-#include <thread>
 #include <vector>
 
 #include "../../include/ygz_b200.h"
+#include "timed_threads.h"
 
 namespace {
 
@@ -38,11 +36,8 @@ extern "C" {
 int ygz_e2e_run(int device, const ygzb_params* prm, int n_threads, int frames_per_thread, const uint8_t* frames, size_t frame_stride,
                 int warm_steps, int steps, double* seconds, int64_t* totals) {
     if (!prm || n_threads < 1 || frames_per_thread < 1 || !frames || steps < 1 || !seconds || !totals) return YGZB_ERR_INVALID;
-    std::vector<int> rcs(n_threads, YGZB_OK);
-    std::vector<int64_t> feat(n_threads, 0), bytes(n_threads, 0), launches(n_threads, 0), matched(n_threads, 0);
-    std::barrier sync_point(n_threads);
-    std::chrono::steady_clock::time_point t_begin, t_end;
-    auto worker = [&](int t) {
+    TimedThreads threads(n_threads);
+    return threads.run([&](int t) {
         const int B = frames_per_thread;
         ygzb_ctx* ctx = nullptr;
         ygzb_frames* fr = nullptr;
@@ -64,9 +59,7 @@ int ygz_e2e_run(int device, const ygzb_params* prm, int n_threads, int frames_pe
         long long l0 = 0;
         for (int s = 0; s < warm_steps + steps; ++s) {
             if (s == warm_steps) {
-                if (rc == YGZB_OK) ygzb_synchronize(ctx);
-                sync_point.arrive_and_wait();
-                if (t == 0) t_begin = std::chrono::steady_clock::now();
+                threads.begin(t, rc, ctx);
                 if (rc == YGZB_OK) l0 = ygzb_launch_count(ctx);
             }
             if (rc != YGZB_OK) continue;
@@ -74,37 +67,18 @@ int ygz_e2e_run(int device, const ygzb_params* prm, int n_threads, int frames_pe
             if (rc == YGZB_OK) rc = ygzb_detect(fr, slots.data(), B, nullptr, &kp);
             if (rc == YGZB_OK) rc = ygzb_match_frames(fr, slots.data(), nxt.data(), B, 1, qoff.as<int32_t>(), idx.as<int32_t>(), dist.as<int32_t>(), (int)cap);
         }
-        if (rc == YGZB_OK) ygzb_synchronize(ctx);
-        sync_point.arrive_and_wait();
-        if (t == 0) t_end = std::chrono::steady_clock::now();
-        if (rc == YGZB_OK) {
+        threads.end(t, rc, ctx);
+        if (rc == YGZB_OK) {   // features, device->host bytes, launches, matched queries
             const int64_t nf = off.as<int32_t>()[B], nq = qoff.as<int32_t>()[B];
-            feat[t] = nf;
-            bytes[t] = nf * (4 + 4 + 1 + 4 + 4 + 32 + 4) + (int64_t)(B + 1) * 4 + nq * 8 + (int64_t)(B + 1) * 4;
-            launches[t] = ygzb_launch_count(ctx) - l0;
             int64_t m = 0;
             for (int64_t q = 0; q < nq; ++q) m += idx.as<int32_t>()[q] >= 0;
-            matched[t] = m;
+            threads.tot[t] = {nf, nf * (4 + 4 + 1 + 4 + 4 + 32 + 4) + (int64_t)(B + 1) * 4 + nq * 8 + (int64_t)(B + 1) * 4,
+                              ygzb_launch_count(ctx) - l0, m};
         }
         if (fr) ygzb_frames_destroy(fr);
         if (ctx) ygzb_destroy(ctx);
-        rcs[t] = rc;
-    };
-    std::vector<std::thread> pool;
-    for (int t = 1; t < n_threads; ++t) pool.emplace_back(worker, t);
-    worker(0);
-    for (auto& th : pool) th.join();
-    *seconds = std::chrono::duration<double>(t_end - t_begin).count();
-    totals[0] = totals[1] = totals[2] = totals[3] = 0;
-    for (int t = 0; t < n_threads; ++t) {
-        totals[0] += feat[t];
-        totals[1] += bytes[t];
-        totals[2] += launches[t];
-        totals[3] += matched[t];
-    }
-    for (int rc : rcs)
-        if (rc != YGZB_OK) return rc;
-    return YGZB_OK;
+        return rc;
+    }, seconds, totals, 4);
 }
 
 }  // extern "C"

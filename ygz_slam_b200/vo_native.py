@@ -59,6 +59,8 @@ def stack_pinned(frames):
 
 
 _REF_MODES = {"keyframe": 0, "previous": 1}   # YGZB_TRACK_REF_KEYFRAME / _PREVIOUS
+# names of the first 12 of a stream's 16 counters (ygz_vo_run's stats, ygz_vo_stream_stats); counter 12 counts restarts
+_STAT_KEYS = ("lost", "keyframes", "ba", "candidates", "projected", "inliers", "ba_obs", "ba_pts", "ba_kfs", "ba_trials", "ba_iters", "ba_flops")
 
 
 def run(ctx, frames, depths, kf_min_frames=10, kf_min_rot=0.1, kf_min_trans=0.1, warm=0, threads=1, device_frames=None,
@@ -124,8 +126,7 @@ def run(ctx, frames, depths, kf_min_frames=10, kf_min_rot=0.1, kf_min_trans=0.1,
 
 
 def _result(traj, stats, totals, sec, dev_ms, S, n, details, return_device_ms):
-    keys = ("lost", "keyframes", "ba", "candidates", "projected", "inliers", "ba_obs", "ba_pts", "ba_kfs", "ba_trials", "ba_iters", "ba_flops")
-    out = (traj.reshape(S, n, 3, 4), [dict(zip(keys, map(int, row[:12]))) for row in stats], sec.value)
+    out = (traj.reshape(S, n, 3, 4), [dict(zip(_STAT_KEYS, map(int, row[:12]))) for row in stats], sec.value)
     if details:   # timed region only: device ms (CUDA events), kernel launches, bytes through the C ABI
         return out + (dict(device_ms=dev_ms.value, gpu_launches=int(totals[0]), h2d_image_bytes=int(totals[1]),
                            h2d_other_bytes=int(totals[2]), d2h_bytes=int(totals[3])),)
@@ -140,7 +141,6 @@ class VoConfig(C.Structure):
 STATUS = ("tracked", "keyframe", "lost")   # YGZ_VO_TRACKED / _KEYFRAME / _LOST
 RESULT_DTYPE = np.dtype([("stream", np.int32), ("frame", np.int32), ("tag", np.int64), ("status", np.int32), ("n_inliers", np.int32),
                          ("T_cw", np.float64, (12,))])   # ygz_vo_result
-_STAT_KEYS = ("lost", "keyframes", "ba", "candidates", "projected", "inliers", "ba_obs", "ba_pts", "ba_kfs", "ba_trials", "ba_iters", "ba_flops")
 
 
 class Engine:
@@ -212,17 +212,18 @@ class Engine:
             self._alive.pop((s_, f), None)
         return res
 
-    def stats(self, stream):
-        """The counters of ygz_vo_run for one stream, as run's dicts."""
+    def _stat_row(self, stream):
         row = np.zeros(16, np.int64)
         self.ctx.check(self.lib.ygz_vo_stream_stats(self.h, int(stream), row.ctypes.data), "ygz_vo_stream_stats")
-        return dict(zip(_STAT_KEYS, map(int, row[:12])))
+        return row
+
+    def stats(self, stream):
+        """The counters of ygz_vo_run for one stream, as run's dicts."""
+        return dict(zip(_STAT_KEYS, map(int, self._stat_row(stream)[:12])))
 
     def restarts(self, stream):
         """How many restarts (ygz_vo_restart) have started a new sequence of `stream`: counter 12 of ygz_vo_stream_stats."""
-        row = np.zeros(16, np.int64)
-        self.ctx.check(self.lib.ygz_vo_stream_stats(self.h, int(stream), row.ctypes.data), "ygz_vo_stream_stats")
-        return int(row[12])
+        return int(self._stat_row(stream)[12])
 
     def export_map(self, stream):
         """The stream's local map (every key-frame still in its ring, oldest first) as a capi.MapBuffers; call after flush."""
