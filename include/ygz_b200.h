@@ -296,7 +296,18 @@ int ygzb_sparse_align(ygzb_frames* f, int n_problems, const int32_t* ref_slot, c
  * [kf_off[p], kf_off[p+1]), points [pt_off[p], ..), observations [obs_off[p], ..); kf_idx / pt_idx are
  * indices LOCAL to the problem.  poses = 6 doubles per keyframe in the vertex' order [omega; upsilon]
  * (in/out), fixed[k] != 0 = setFixed(true) (keyframe id 0 and non-local observers, BA.cpp:404-405,458-492),
- * pts in/out, outlier[o] = 1 iff chi2 > chi2_outlier after the optimisation (Feature::_bad, :505-515).  */
+ * pts in/out, outlier[o] = 1 iff chi2 > chi2_outlier after the optimisation (Feature::_bad, :505-515).
+ * The system is linearised once before the first iteration: chi2_initial is the robust cost of the input
+ * and lambda starts at tau * max |diag H| (free poses and landmarks), so max_iters = 0 evaluates once and
+ * reports chi2_initial = chi2_final = that cost and lambda_final = that lambda.  A pose keeps its input
+ * bits unless an LM step was accepted.  When the dense factorisation of the reduced system fails (a
+ * non-positive pivot), the trial's pose step is zero, the landmarks are back-substituted from it, its
+ * cost counts as DBL_MAX and the trial is rejected or accepted by the usual gain ratio.  With the landmark
+ * blocks (Hll + lambda I) positive definite the gain ratio's denominator is then bl^T (Hll + lambda I)^-1 bl +
+ * lambda |x_l|^2 + 1e-3 > 0, so the trial is always rejected; any pose step of that kind -- the unsolved
+ * right-hand side b_s included, which gives |b_s|^2 + the same terms -- decides alike, so which one is taken
+ * changes no result and no test can tell them apart.  A point observed
+ * twice by one key-frame makes the call fail with YGZB_ERR_INVALID.                                     */
 typedef struct {
     int max_iters;        /* optimizer.optimize(20)        */
     double huber_delta;   /* 5.991 (<= 0: no robust kernel) */

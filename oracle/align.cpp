@@ -323,6 +323,7 @@ struct SparseAlign {
     double H[6][6], Jres[6], x[6];
     size_t n_meas = 0;
     double chi2_ = 1e10;
+    bool exact_chi2 = false;   // sum the squared residuals in double and round to float once (the kernel's order-free sum)
 
     // SparseImgAlign::precomputeReferencePatches (:59-122)
     void precompute() {
@@ -370,6 +371,7 @@ struct SparseAlign {
         const int stride = im.w, border = 3;
         const float scale = 1.0f / (1 << level_);
         float chi2 = 0.0f;
+        double chi2_d = 0.0;
         for (int i = 0; i < n; ++i) {
             if (!visible[i]) continue;
             const V3 xyz_ref = cam.pixel2camera(px[2 * i], px[2 * i + 1], depth[i]);
@@ -391,6 +393,7 @@ struct SparseAlign {
                     const float res = inten - cache[pc];
                     const float weight = 1.0;
                     chi2 += res * res * weight;
+                    chi2_d += (double)(res * res * weight);
                     n_meas++;
                     if (linearize) {
                         const double* J = &jac[6 * (16 * (size_t)i + pc)];
@@ -402,6 +405,7 @@ struct SparseAlign {
                 }
             }
         }
+        if (exact_chi2) return (float)chi2_d / (float)n_meas;
         return chi2 / n_meas;
     }
 };
@@ -411,9 +415,10 @@ struct SparseAlign {
 extern "C" size_t ora_sparse_align(const uint8_t* ref_pyr, const uint8_t* cur_pyr, int w, int h, int n_levels,
                                    const ora_camera* camp, int n, const double* px, const double* depth,
                                    const uint8_t* has_mappoint, const double* T_cw_ref, double* T_cw_cur, int max_level,
-                                   int min_level, int n_iter, double eps, int32_t* iters_per_level) {
+                                   int min_level, int n_iter, double eps, int32_t* iters_per_level, int exact_chi2) {
     if (n == 0) return 0;  // run(): ref_frame->_features.empty()
     SparseAlign s;
+    s.exact_chi2 = exact_chi2 != 0;
     s.ref_pyr = ref_pyr; s.cur_pyr = cur_pyr; s.w = w; s.h = h; s.n_levels = n_levels;
     s.cam = Cam{camp->fx, camp->fy, camp->cx, camp->cy};
     s.n = n; s.px = px; s.depth = depth; s.has_mp = has_mappoint;
@@ -462,7 +467,7 @@ extern "C" int ora_matcher_sparse_alignment(const uint8_t* ref_pyr, const uint8_
     // current->_TCW = ref->_TCW; _align->run(ref, current) with SparseImgAlign(2, 0, 30, GaussNewton) (Matcher.cpp:18)
     double T[12];
     std::memcpy(T, T_cw_ref, sizeof(T));
-    ora_sparse_align(ref_pyr, cur_pyr, w, h, n_levels, cam, n, px, depth, has_mappoint, T_cw_ref, T, 2, 0, 30, 0.000001, nullptr);
+    ora_sparse_align(ref_pyr, cur_pyr, w, h, n_levels, cam, n, px, depth, has_mappoint, T_cw_ref, T, 2, 0, 30, 0.000001, nullptr, 0);
     const SE3 TCR = SE3::from_mat(T) * SE3::from_mat(T_cw_ref).inverse();
     double lg[6];
     TCR.log(lg);

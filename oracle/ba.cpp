@@ -138,10 +138,9 @@ extern "C" int ora_local_ba_g2o(const ora_camera* camp, int n_kf, double* poses,
     int iters = 0, trials_total = 0;
     double chi_first = 0, chi_last = 0;
 
-    for (int iteration = 0; iteration < prm->max_iters; ++iteration) {
-        // computeActiveErrors + buildSystem
-        double currentChi = pb.robust_chi2(pb.poses, pb.pts);
-        if (iteration == 0) chi_first = currentChi;
+    // computeActiveErrors + buildSystem at the current estimate; returns its robust chi2
+    auto build_system = [&]() {
+        const double chi = pb.robust_chi2(pb.poses, pb.pts);
         std::fill(Hpp.begin(), Hpp.end(), 0.0); std::fill(bp.begin(), bp.end(), 0.0);
         std::fill(Hll.begin(), Hll.end(), 0.0); std::fill(bl.begin(), bl.end(), 0.0);
         std::fill(Hpl.begin(), Hpl.end(), 0.0);
@@ -185,15 +184,21 @@ extern "C" int ora_local_ba_g2o(const ora_camera* camp, int n_kf, double* poses,
                 }
             }
         }
-        if (iteration == 0) {  // computeLambdaInit: tau * max |diag H| over all free vertices
-            double mx = 0;
-            for (int i = 0; i < np; ++i)
-                for (int a = 0; a < 6; ++a) mx = std::max(mx, std::fabs(Hpp[36 * (size_t)i + 7 * a]));
-            for (int j = 0; j < n_pt; ++j)
-                for (int a = 0; a < 3; ++a) mx = std::max(mx, std::fabs(Hll[9 * (size_t)j + 4 * a]));
-            lambda = prm->tau * mx;
-            ni = 2;
-        }
+        return chi;
+    };
+    // g2o linearises before the first iteration: chi2_initial and computeLambdaInit (tau * max |diag H| over all free
+    // vertices) exist even when max_iters = 0, which then reports them and returns the input
+    chi_first = chi_last = build_system();
+    {
+        double mx = 0;
+        for (int i = 0; i < np; ++i)
+            for (int a = 0; a < 6; ++a) mx = std::max(mx, std::fabs(Hpp[36 * (size_t)i + 7 * a]));
+        for (int j = 0; j < n_pt; ++j)
+            for (int a = 0; a < 3; ++a) mx = std::max(mx, std::fabs(Hll[9 * (size_t)j + 4 * a]));
+        lambda = prm->tau * mx;
+    }
+    for (int iteration = 0; iteration < prm->max_iters; ++iteration) {
+        double currentChi = iteration == 0 ? chi_first : build_system();
         double rho = 0;
         int qmax = 0;
         do {
@@ -233,7 +238,9 @@ extern "C" int ora_local_ba_g2o(const ora_camera* camp, int n_kf, double* poses,
             }
             std::vector<double> sol(bs);
             bool ok2 = dimp == 0 || cholesky_solve(S, sol, dimp);
-            xp = sol;
+            // a failed factorisation leaves sol unsolved: the trial's pose step is zero (the landmarks follow from it)
+            if (ok2) xp = sol;
+            else std::fill(xp.begin(), xp.end(), 0.0);
             for (int j = 0; j < n_pt; ++j) {
                 double r[3] = {bl[3 * (size_t)j], bl[3 * (size_t)j + 1], bl[3 * (size_t)j + 2]};
                 for (int o1 : obs_of_pt[j]) {

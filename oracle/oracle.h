@@ -143,11 +143,13 @@ void ora_find_direct_projection(const uint8_t* ref_pyr, const uint8_t* cur_pyr, 
                                 double* cur_px_inout /*2n*/, int32_t* search_level, uint8_t* ok);
 
 /* ---- sparse image alignment (src/Algorithm/SparseImageAlign.cpp; NLSSolver_impl.hpp) ---- */
-/* returns n_meas/16 (SparseImgAlign::run); T_cw_cur updated in place */
+/* returns n_meas/16 (SparseImgAlign::run); T_cw_cur updated in place.  exact_chi2 = 0: the reference's float running
+ * sum of the squared residuals; 1: their sum in double, rounded to float once, so that the rollback test chi2_new > chi2
+ * decides as in the CUDA kernel, whose sum has no fixed order */
 size_t ora_sparse_align(const uint8_t* ref_pyr, const uint8_t* cur_pyr, int w, int h, int n_levels,
                         const ora_camera* cam, int n, const double* px /*2n*/, const double* depth,
                         const uint8_t* has_mappoint, const double* T_cw_ref, double* T_cw_cur, int max_level,
-                        int min_level, int n_iter, double eps, int32_t* iters_per_level /*may be NULL*/);
+                        int min_level, int n_iter, double eps, int32_t* iters_per_level /*may be NULL*/, int exact_chi2);
 /* Matcher::SparseImageAlignment (Matcher.cpp:468-492): returns 1/0, T_cw_cur in/out */
 int ora_matcher_sparse_alignment(const uint8_t* ref_pyr, const uint8_t* cur_pyr, int w, int h, int n_levels,
                                  const ora_camera* cam, int n, const double* px, const double* depth,

@@ -234,7 +234,9 @@ class Oracle:
         return cur, lvl, ok.astype(bool)
 
     def sparse_align(self, ref_pyr, cur_pyr, w, h, n_levels, px, depth, has_mp, T_ref, T_cur, max_level=2,
-                     min_level=0, n_iter=30, eps=1e-6, cam=None):
+                     min_level=0, n_iter=30, eps=1e-6, cam=None, exact=False):
+        """SparseImgAlign::run.  exact=True sums chi2 in double and rounds it to float once, as the CUDA kernel does, so the
+        rollback decisions (and the per-level iteration counts) can be compared exactly."""
         cam = cam or default_camera()
         n = len(depth)
         T = np.ascontiguousarray(T_cur, np.float64).copy()
@@ -244,7 +246,7 @@ class Oracle:
                                        _p(np.ascontiguousarray(depth, np.float64)),
                                        _p(np.ascontiguousarray(has_mp, np.uint8)),
                                        _p(np.ascontiguousarray(T_ref, np.float64)), _p(T), max_level, min_level,
-                                       n_iter, C.c_double(eps), _p(iters))
+                                       n_iter, C.c_double(eps), _p(iters), int(exact))
         return T, int(nm), iters
 
     def matcher_sparse_alignment(self, ref_pyr, cur_pyr, w, h, n_levels, px, depth, has_mp, T_ref, T_cur, cam=None):
@@ -269,11 +271,12 @@ class Oracle:
         return v
 
     # ---- BA --------------------------------------------------------------------------------
-    def local_ba(self, poses, fixed, pts, kf_idx, pt_idx, px, max_iters=20, huber=5.991, cam=None):
+    def local_ba(self, poses, fixed, pts, kf_idx, pt_idx, px, max_iters=20, huber=5.991, cam=None, tau=1e-5, max_trials=10,
+                 chi2_outlier=5.991):
         cam = cam or default_camera()
         poses = np.ascontiguousarray(poses, np.float64).copy()
         pts = np.ascontiguousarray(pts, np.float64).copy()
-        prm = BAParams(max_iters, huber, 5.991, 1e-5, 10)
+        prm = BAParams(max_iters, huber, chi2_outlier, tau, max_trials)
         st = BAStats()
         outl = np.zeros(len(kf_idx), np.uint8)
         self.lib.ora_local_ba_g2o(C.byref(cam), len(poses), _p(poses), _p(np.ascontiguousarray(fixed, np.uint8)),

@@ -486,7 +486,8 @@ class BAStats(C.Structure):
                 ("lambda_final", C.c_double), ("n_outliers", C.c_int)]
 
 
-def _local_ba(self, kf_off, pt_off, obs_off, poses, fixed, pts, kf_idx, pt_idx, px, max_iters=20, huber=5.991):
+def _local_ba(self, kf_off, pt_off, obs_off, poses, fixed, pts, kf_idx, pt_idx, px, max_iters=20, huber=5.991, tau=1e-5,
+              max_trials=10, chi2_outlier=5.991):
     """Batched ba::LocalBAG2O.  poses: (n_kf, 6) in g2o order [omega; upsilon]."""
     kf_off = np.ascontiguousarray(kf_off, np.int32)
     P = len(kf_off) - 1
@@ -496,6 +497,9 @@ def _local_ba(self, kf_off, pt_off, obs_off, poses, fixed, pts, kf_idx, pt_idx, 
     self.lib.ygzb_default_ba_params(C.byref(prm))
     prm.max_iters = max_iters
     prm.huber_delta = huber
+    prm.tau = tau
+    prm.max_trials = max_trials
+    prm.chi2_outlier = chi2_outlier
     outl = np.zeros(len(kf_idx), np.uint8)
     st = (BAStats * P)()
     self.check(self.lib.ygzb_local_ba(self.h, P, _p(kf_off), _p(np.ascontiguousarray(pt_off, np.int32)),

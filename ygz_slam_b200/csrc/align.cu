@@ -918,7 +918,7 @@ int launch_sparse_align(ygzb_frames* f, int n_problems, const int32_t* d_ref_slo
     a.iters_out = d_iters;
     a.feat_scratch = d_feat_scratch;
     a.feat_stride = feat_stride;
-    return launch_sparse_align2(ctx, a, n_problems, kTrackCluster);
+    return launch_sparse_align2(ctx, a, n_problems, cluster_knob("YGZB_TRACK_CLUSTER", kTrackCluster, false));
 }
 
 // Tracking chain of a batch, part 1 (on whatever stream ctx->stream currently is: the tracker points it at its second

@@ -850,6 +850,7 @@ __global__ void __launch_bounds__(kT) local_ba2_kernel(const BA2Args a) {
         }
     };
     bool fresh = false;   // Hpp / bp of the accepted state are in s_x (the prologue computed them for iteration 0)
+    bool moved = false;   // a step was accepted: the poses are written back as the logarithm of s_T, else as their input bits
     for (int iteration = 0; iteration < a.max_iters && !dup; ++iteration) {
         int qmax = 0;
         do {
@@ -1007,6 +1008,7 @@ __global__ void __launch_bounds__(kT) local_ba2_kernel(const BA2Args a) {
                 // the trial becomes the accepted state: swap the double buffers, take over the poses
                 cur ^= 1;
                 fresh = true;
+                moved = true;
                 if (tid < n_kf) {
                     s_T[tid] = s_Ttry[tid];
                     for (int c = 0; c < 12; ++c) s_Rlin[tid][c] = s_Rtry[tid][c];
@@ -1043,7 +1045,7 @@ __global__ void __launch_bounds__(kT) local_ba2_kernel(const BA2Args a) {
     }
     exchange_small();
     if (rank == 0) {
-        if (tid < n_kf && s_free[tid] >= 0) {   // fixed vertices keep their input bits
+        if (moved && tid < n_kf && s_free[tid] >= 0) {   // fixed vertices, and all of them without an accepted step, keep their input bits
             double lg[6];
             se3_log(s_T[tid], lg);
             double* o = a.poses + 6 * (size_t)(k0 + tid);

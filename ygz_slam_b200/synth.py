@@ -243,6 +243,22 @@ def ba_scene(n_kf: int = 10, n_pt: int = 2000, target_obs: int = 8000, seed: int
                 px=np.array(px, np.float64))
 
 
+def ba_axis_scene(depths, errors):
+    """Local-BA problem whose reprojection errors are exact: two key-frames at the identity pose (0 fixed, 1 free) and one
+    landmark per depth on the optical axis, seen by both.  A point on the axis projects to (cx, cy) exactly in any
+    arithmetic, so observation o, at (cx + errors[o, 0], cy + errors[o, 1]), has exactly that error when the errors lie on
+    a 2^-30 grid.  Observations alternate key-frames 0 and 1 per landmark.  Returns ba_scene's keys."""
+    depths = np.asarray(depths, np.float64)
+    errors = np.asarray(errors, np.float64).reshape(2 * len(depths), 2)
+    assert np.array_equal(errors, np.round(errors * 2.0 ** 30) / 2.0 ** 30)
+    cx, cy = float(np.float32(CX)), float(np.float32(CY))   # the intrinsics as the solvers see them: float, widened
+    pts = np.stack([np.zeros_like(depths), np.zeros_like(depths), depths], 1)
+    poses = np.zeros((2, 6))
+    return dict(poses_true=poses, poses_noisy=poses.copy(), pts_true=pts, pts_noisy=pts.copy(),
+                kf_idx=np.tile(np.array([0, 1], np.int32), len(depths)), pt_idx=np.repeat(np.arange(len(depths), dtype=np.int32), 2),
+                px=errors + np.array([cx, cy]))
+
+
 def two_view_scene(seed=21, n=120, n_bad=12):
     """Two views of points in front of both cameras (the situation after Initializer::TryInitialize): true relative pose,
     noisy triangulated points, pixel noise, and a few points flagged as non-inliers (they restart from (0,0,1))."""
