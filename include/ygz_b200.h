@@ -451,6 +451,11 @@ void ygzb_tracker_destroy(ygzb_tracker* t);
 /* depth image (image_width * image_height doubles, host or device) that initialises the map points of the next key-frame
  * of `stream` (the reference's drivers read it from the TUM depth frame, test/test_feature_alignment.cpp:72-85)   */
 int ygzb_tracker_set_depth(ygzb_tracker* t, int stream, const double* depth);
+/* the read-back counterpart of ygzb_tracker_set_depth: copies the depth image `stream`'s next key-frame would use
+ * (image_width * image_height doubles) to `out` (host or device memory).  Asynchronous on the context's stream, behind
+ * every insertion already enqueued; valid after ygzb_synchronize(ctx).  YGZB_ERR_INVALID for a NULL tracker or output,
+ * or a stream out of range.                                                                                          */
+int ygzb_tracker_get_depth(ygzb_tracker* t, int stream, double* out);
 /* T_cw (3x4 row-major) that the next first key-frame of `stream` (a key-frame job with track_job = -1) takes: it places a
  * sequence in the caller's world frame, as the reference's drivers do for their first frame
  * (test/test_feature_alignment.cpp:63); the key-frame's map points go to that world frame.  Identity from

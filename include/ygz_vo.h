@@ -32,6 +32,7 @@
 #ifndef YGZ_VO_H_
 #define YGZ_VO_H_
 
+#include <stddef.h>
 #include <stdint.h>
 
 #include "ygz_b200.h"
@@ -100,6 +101,56 @@ int ygz_vo_stream_stats(ygz_vo* vo, int stream, int64_t stats[16]);
 /* the local map of `stream` (every key-frame still in its ring, oldest first) into `out`, sized for YGZB_TRACK_RING
  * key-frames (ygzb_tracker_export): asynchronous, valid after ygzb_synchronize(ctx); call after ygz_vo_flush         */
 int ygz_vo_export_map(ygz_vo* vo, int stream, ygzb_map_record* out);
+
+/* ---- stream records: a live stream as plain bytes, to move it to another engine, context, device or process ----------
+ * A stream record is the whole state of one stream: its host bookkeeping, its local map (ygzb_tracker_export), in
+ * previous-frame mode its reference (ygzb_tracker_export_reference) and the depth map its next key-frame pushed with
+ * depth = NULL would use (ygzb_tracker_get_depth).  A stream loaded from it continues exactly as the saved one would have.
+ *
+ * Layout: little-endian, packed (no padding; fields are not aligned), every count before the rows it describes.
+ *   1. header      u8 magic[4] = "YGZS", u32 version = 1, u64 size (of the whole record),
+ *                  i32 width, height, cells, n_levels, f64 K[4], i32 ref_mode                                 (68 bytes)
+ *   2. host state  i32 n_kf, then per key-frame of the stream's ring, oldest first:
+ *                      i32 entry, i32 n, i32 frame_id, i64 mp0, f64 T_cw[12]                               (116 bytes)
+ *                  f64 T_cw[12] (current pose), f64 start[12] (pose of the next sequence's first key-frame),
+ *                  u8 restart_pending, has_pose, lost, has_depth (0 or 1),
+ *                  i32 frames_since_kf, i32 next_frame (the frame index of the stream's next push), i64 next_mp,
+ *                  i64 counters[11] (stats 1-10 and 12 of ygz_vo_stream_stats), f64 ba_flops
+ *   3. map         i32 n_keyframes (= n_kf), then per key-frame:
+ *                      i32 entry, i32 n_features, i32 n_obs, i64 mp0, f64 T_cw[12], u8 image[height][width]
+ *                  then the live rows of all key-frames, key-frame after key-frame (F = sum n_features, O = sum n_obs):
+ *                      f64 px[F][2], u8 level[F], f64 depth[F], f64 pw[F][3], i64 obs_id[O], f64 obs_px[O][2]
+ *   4. reference   (ref_mode YGZB_TRACK_REF_PREVIOUS and n_kf > 0 only)
+ *                  i32 n, f64 T_cw[12], f64 px[n][2], f64 depth[n], u8 image[height][width]
+ *   5. depth       (has_depth only) f64 depth[height][width]
+ * The fields are those of ygzb_map_record and ygzb_reference_record; a stream never pushed is a record of sections 1-2
+ * and an empty map.                                                                                                 */
+#define YGZ_VO_STREAM_RECORD_VERSION 1
+/* *bytes = an upper bound of the size of any stream record of `vo`: a full ring, a full reference, a depth map.       */
+int ygz_vo_stream_record_bound(const ygz_vo* vo, size_t* bytes);
+/* the whole state of `stream` as a record in buf[0 .. *size).  Synchronous: it synchronises the context.
+ *  - The stream must have no queued frame and no pending key-frame insertion (ygz_vo_flush first), so that every frame
+ *    pushed to it has its final result; other streams of `vo` may have queued frames, which stay queued.
+ *  - It does not change the stream: the saved stream may go on tracking, and the record then forks it.
+ * YGZB_ERR_INVALID, changing nothing, for a NULL vo or size, a NULL buf with capacity > 0, a stream out of range, or a
+ * stream with queued frames or a pending insertion; YGZB_ERR_CAPACITY if the record does not fit in `capacity` bytes
+ * (*size = its size; buf = NULL, capacity = 0 asks for the size).                                                   */
+int ygz_vo_save_stream(ygz_vo* vo, int stream, void* buf, size_t capacity, size_t* size);
+/* `stream` of vo continues the saved stream: its whole state, counters included, is replaced by the record's, and its
+ * next push is the saved stream's next frame (frame index and results as the saved stream would have given them).
+ *  - The destination stream must have no queued frame and no pending key-frame insertion; results already waiting in
+ *    the result queue stay there for ygz_vo_poll.
+ *  - The engine may differ from the saved one in n_streams, window, key-frame policy and min_inliers (the destination's
+ *    apply from here on), in the stream index and in its context and device.  It must match it in image size, grid
+ *    cells, pyramid levels, K (bit for bit) and ref_mode.
+ *  - The record is checked whole on the host before anything is enqueued.
+ * Asynchronous like ygzb_tracker_import; `buf` may be released when the call returns.  YGZB_ERR_INVALID, with the
+ * stream exactly as before, for a NULL vo or buf, a stream out of range or with queued frames or a pending insertion,
+ * a wrong magic or version, a size that is not the record's, a different geometry, K or ref_mode, a count, entry,
+ * level or pose out of range, or a host state no saved stream can have (e.g. frames pushed but no key-frame, key-frames
+ * but no frame pushed, map sections that disagree with the host state).                                            */
+int ygz_vo_load_stream(ygz_vo* vo, int stream, const void* buf, size_t size);
+
 void ygz_vo_destroy(ygz_vo* vo);
 
 #ifdef __cplusplus

@@ -45,7 +45,7 @@ EXPORTS = [
     "ygzb_tracker_create", "ygzb_tracker_destroy", "ygzb_tracker_set_depth", "ygzb_tracker_upload", "ygzb_tracker_track", "ygzb_tracker_make_keyframes",
     "ygzb_tracker_export", "ygzb_tracker_import", "ygzb_tracker_debug_job", "ygzb_tracker_set_reference_mode", "ygzb_tracker_debug_reference",
     "ygzb_tracker_export_reference", "ygzb_tracker_import_reference", "ygzb_undistort_map", "ygzb_frames_set_undistort",
-    "ygzb_tracker_set_start_pose",
+    "ygzb_tracker_set_start_pose", "ygzb_tracker_get_depth",
 ]
 
 
@@ -863,6 +863,7 @@ class Tracker:
         self.lib.ygzb_tracker_export.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
         self.lib.ygzb_tracker_import.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         self.lib.ygzb_tracker_set_depth.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        self.lib.ygzb_tracker_get_depth.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         self.lib.ygzb_tracker_set_start_pose.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         self.lib.ygzb_tracker_upload.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
         self.lib.ygzb_tracker_track.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
@@ -924,6 +925,14 @@ class Tracker:
         depth = np.ascontiguousarray(depth, np.float64)
         self.ctx.check(self.lib.ygzb_tracker_set_depth(self.h, int(stream), _p(depth)), "ygzb_tracker_set_depth")
         self.ctx.synchronize()
+
+    def get_depth(self, stream: int):
+        """The depth image (H, W) `stream`'s next key-frame would use (the call synchronises the context)."""
+        f = self.frames
+        out = np.zeros((f.lh[0], f.lw[0]), np.float64)
+        self.ctx.check(self.lib.ygzb_tracker_get_depth(self.h, int(stream), _p(out)), "ygzb_tracker_get_depth")
+        self.ctx.synchronize()
+        return out
 
     def set_start_pose(self, stream: int, T_cw):
         """T_cw (3, 4) that `stream`'s next first key-frame (a key-frame job with track_job = -1) takes; identity by default."""

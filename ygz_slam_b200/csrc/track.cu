@@ -941,6 +941,16 @@ int ygzb_tracker_set_depth(ygzb_tracker* t, int stream, const double* depth) {
     return YGZB_OK;
 }
 
+int ygzb_tracker_get_depth(ygzb_tracker* t, int stream, double* out) {
+    if (!t || !out) return YGZB_ERR_INVALID;
+    ygzb_ctx* ctx = t->ctx;
+    if (stream < 0 || stream >= t->st.S) return set_error(ctx, YGZB_ERR_INVALID, "get_depth: stream %d out of range", stream);
+    cudaSetDevice(ctx->device);
+    const size_t n = (size_t)t->st.W * t->st.H;
+    YGZB_CUDA(ctx, cudaMemcpyAsync(out, t->d_depth + (size_t)stream * n, n * sizeof(double), cudaMemcpyDefault, ctx->stream));
+    return YGZB_OK;
+}
+
 int ygzb_tracker_set_start_pose(ygzb_tracker* t, int stream, const double T_cw[12]) {
     if (!t || !T_cw) return YGZB_ERR_INVALID;
     ygzb_ctx* ctx = t->ctx;

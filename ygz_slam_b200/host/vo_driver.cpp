@@ -15,6 +15,7 @@
 // Build: host C++ only (g++), links libygz_b200.so; see ygz_slam_b200/build.py (libygz_vo.so).
 #include <algorithm>
 #include <atomic>
+#include <bit>
 #include <chrono>
 #include <cmath>
 #include <cstdint>
@@ -24,6 +25,7 @@
 #include <deque>
 #include <memory>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/ygz_b200.h"
@@ -860,6 +862,19 @@ class Engine {
         st_[i] = s;
         return YGZB_OK;
     }
+    // stream i has no queued frame and no key-frame insertion pending: every frame pushed to it has its final result
+    bool settled(int i) const {
+        if (!st_[i].queue.empty()) return false;
+        for (const ygzb_keyframe_job& kj : kjobs_)
+            if (kj.stream == i) return false;
+        return true;
+    }
+    // the depth map stream i's next key-frame takes when its frame brings none (asynchronous, like export_map), and back
+    int get_depth(int i, double* out) const { return ygzb_tracker_get_depth(tr_, i, out); }
+    int set_depth(int i, const double* depth) { return ygzb_tracker_set_depth(tr_, i, depth); }
+    // the tracker's check of a start pose (finite, a rotation), which keeps it as restart() does; a round sets every first
+    // key-frame's own pose before its insertion, so the kept pose reaches nothing else
+    int check_start_pose(int i, const Mat34& T) { return ygzb_tracker_set_start_pose(tr_, i, T.m); }
 
   private:
     // the first w queued frames of stream i into its frame slots: one strided copy when they are equally spaced in one
@@ -982,6 +997,263 @@ struct RefBuf {
         px.resize(2 * cap); depth.resize(cap); image.resize((size_t)w * h);
         rec.capacity = (int32_t)cap;
         rec.px = px.data(); rec.depth = depth.data(); rec.image = image.data();
+    }
+};
+
+// ---- stream records (ygz_vo_save_stream / ygz_vo_load_stream; the layout is documented in include/ygz_vo.h) ------------
+static_assert(std::endian::native == std::endian::little, "stream records are little-endian and copied field by field");
+constexpr uint8_t kRecordMagic[4] = {'Y', 'G', 'Z', 'S'};
+
+// what a record is made under and must be loaded under: the engine's image size, grid, pyramid, camera and reference mode
+struct RecordGeom {
+    int32_t width, height, cells, n_levels;
+    double K[4];
+    int32_t ref_mode;
+    size_t wh() const { return (size_t)width * height; }
+};
+
+// the largest record of an engine: a full ring at capacity, a full reference, a depth map (the sections of write_record)
+size_t record_bound(const RecordGeom& g) {
+    const size_t R = YGZB_TRACK_RING, F = R * g.cells, O = R * YGZB_MAP_OBS_PER_CELL * g.cells;
+    const size_t C = (size_t)YGZB_TRACK_REF_FEATURES_PER_CELL * g.cells, WH = g.wh();
+    return 68 + (4 + R * 116 + 2 * 96 + 4 + 16 + 12 * 8)        // header, host state
+           + (4 + R * (116 + WH) + F * 49 + O * 24)             // map
+           + (4 + 96 + C * 24 + WH)                             // reference
+           + WH * sizeof(double);                               // depth map
+}
+
+// appends fields to `out`; out == nullptr only counts the bytes
+struct RecordWriter {
+    uint8_t* out;
+    size_t n = 0;
+    void bytes(const void* src, size_t k) {
+        if (out && k) std::memcpy(out + n, src, k);
+        n += k;
+    }
+    template <typename T> void put(T v) { bytes(&v, sizeof v); }
+};
+
+// reads fields from in[0, size); a read past the end clears ok and reads nothing from then on
+struct RecordReader {
+    const uint8_t* in;
+    size_t size, n = 0;
+    bool ok = true;
+    void bytes(void* dst, size_t k) {
+        if (!ok || k > size - n) {
+            ok = false;
+            return;
+        }
+        if (k) std::memcpy(dst, in + n, k);
+        n += k;
+    }
+    template <typename T> T get() {
+        T v{};
+        bytes(&v, sizeof v);
+        return v;
+    }
+};
+
+// the record of stream `s` with its map `m` (exported from the ring entries of s.kfs), its reference `r` (previous-frame
+// mode once it has a key-frame, else NULL) and its depth map (NULL unless s.has_depth)
+void write_record(RecordWriter& w, const RecordGeom& g, const EStream& s, const ygzb_map_record& m, const ygzb_reference_record* r,
+                  const double* depth) {
+    const size_t WH = g.wh();
+    // 1. header (the size is written last)
+    w.bytes(kRecordMagic, 4);
+    w.put<uint32_t>(YGZ_VO_STREAM_RECORD_VERSION);
+    const size_t size_at = w.n;
+    w.put<uint64_t>(0);
+    w.put<int32_t>(g.width); w.put<int32_t>(g.height); w.put<int32_t>(g.cells); w.put<int32_t>(g.n_levels);
+    w.bytes(g.K, sizeof g.K);
+    w.put<int32_t>(g.ref_mode);
+    // 2. host state
+    w.put<int32_t>((int32_t)s.kfs.size());
+    for (const KfInfo& kf : s.kfs) {
+        w.put<int32_t>(kf.entry); w.put<int32_t>(kf.n); w.put<int32_t>(kf.frame_id); w.put<int64_t>(kf.mp0);
+        w.bytes(kf.T.m, sizeof kf.T.m);
+    }
+    w.bytes(s.T.m, sizeof s.T.m);
+    w.bytes(s.start.m, sizeof s.start.m);
+    w.put<uint8_t>(s.restart_pending); w.put<uint8_t>(s.has_pose); w.put<uint8_t>(s.lost); w.put<uint8_t>(s.has_depth);
+    w.put<int32_t>(s.frames_since_kf); w.put<int32_t>(s.next_frame); w.put<int64_t>(s.next_mp);
+    for (long c : {s.n_keyframes, s.n_ba, s.n_candidates, s.n_projected, s.n_inliers, s.ba_obs, s.ba_pts, s.ba_kfs, s.ba_trials, s.ba_iters,
+                   s.n_restarts})
+        w.put<int64_t>(c);
+    w.put<double>(s.ba_flops);
+    // 3. map: per key-frame, then the live rows
+    w.put<int32_t>(m.n_keyframes);
+    size_t F = 0, O = 0;
+    for (int k = 0; k < m.n_keyframes; ++k) {
+        w.put<int32_t>(m.entry[k]); w.put<int32_t>(m.n_features[k]); w.put<int32_t>(m.n_obs[k]); w.put<int64_t>(m.mp0[k]);
+        w.bytes(m.T_cw + 12 * (size_t)k, 12 * sizeof(double));
+        w.bytes(m.image + k * WH, WH);
+        F += (size_t)m.n_features[k];
+        O += (size_t)m.n_obs[k];
+    }
+    w.bytes(m.px, F * 2 * sizeof(double)); w.bytes(m.level, F); w.bytes(m.depth, F * sizeof(double)); w.bytes(m.pw, F * 3 * sizeof(double));
+    w.bytes(m.obs_id, O * sizeof(int64_t)); w.bytes(m.obs_px, O * 2 * sizeof(double));
+    // 4. reference
+    if (r) {
+        w.put<int32_t>(r->n);
+        w.bytes(r->T_cw, sizeof r->T_cw);
+        w.bytes(r->px, (size_t)r->n * 2 * sizeof(double)); w.bytes(r->depth, (size_t)r->n * sizeof(double)); w.bytes(r->image, WH);
+    }
+    // 5. depth map
+    if (depth) w.bytes(depth, WH * sizeof(double));
+    if (w.out) {
+        const uint64_t size = w.n;
+        std::memcpy(w.out + size_at, &size, sizeof size);
+    }
+}
+
+// a record unpacked into what Engine::adopt takes: the stream's bookkeeping, its map and reference records, its depth map
+struct StreamRecord {
+    EStream s;
+    MapBuf map;
+    RefBuf ref;
+    bool has_ref = false;
+    std::vector<double> depth;
+    explicit StreamRecord(const RecordGeom& g) : map(g.cells, g.width, g.height), ref(g.cells, g.width, g.height) {}
+};
+
+// unpacks and checks the whole record in[0, size) against the engine's geometry `g`: YGZB_ERR_INVALID for anything but
+// a well-formed record of that geometry whose counts, entries and levels are in range
+int read_record(const uint8_t* in, size_t size, const RecordGeom& g, StreamRecord& out) {
+    RecordReader r{in, size};
+    const size_t WH = g.wh();
+    // 1. header
+    uint8_t magic[4];
+    r.bytes(magic, 4);
+    const uint32_t version = r.get<uint32_t>();
+    const uint64_t total = r.get<uint64_t>();
+    RecordGeom rg{};
+    rg.width = r.get<int32_t>(); rg.height = r.get<int32_t>(); rg.cells = r.get<int32_t>(); rg.n_levels = r.get<int32_t>();
+    r.bytes(rg.K, sizeof rg.K);
+    rg.ref_mode = r.get<int32_t>();
+    if (!r.ok || std::memcmp(magic, kRecordMagic, 4) != 0 || version != YGZ_VO_STREAM_RECORD_VERSION || total != size) return YGZB_ERR_INVALID;
+    if (rg.width != g.width || rg.height != g.height || rg.cells != g.cells || rg.n_levels != g.n_levels || rg.ref_mode != g.ref_mode ||
+        std::memcmp(rg.K, g.K, sizeof g.K) != 0)   // K bit for bit
+        return YGZB_ERR_INVALID;
+    // 2. host state
+    EStream& s = out.s;
+    const int32_t n_kf = r.get<int32_t>();
+    if (!r.ok || n_kf < 0 || n_kf > YGZB_TRACK_RING) return YGZB_ERR_INVALID;
+    for (int k = 0; k < n_kf; ++k) {
+        KfInfo kf;
+        kf.entry = r.get<int32_t>(); kf.n = r.get<int32_t>(); kf.frame_id = r.get<int32_t>(); kf.mp0 = (long)r.get<int64_t>();
+        r.bytes(kf.T.m, sizeof kf.T.m);
+        if (kf.entry < 0 || kf.entry >= YGZB_TRACK_RING || kf.n < 0 || kf.n > g.cells || kf.frame_id < 0 || kf.mp0 < 0) return YGZB_ERR_INVALID;
+        for (const KfInfo& o : s.kfs)
+            if (o.entry == kf.entry) return YGZB_ERR_INVALID;
+        if (!s.kfs.empty() && kf.frame_id <= s.kfs.back().frame_id) return YGZB_ERR_INVALID;   // oldest first
+        s.kfs.push_back(kf);
+    }
+    r.bytes(s.T.m, sizeof s.T.m);
+    r.bytes(s.start.m, sizeof s.start.m);
+    uint8_t flags[4];
+    r.bytes(flags, 4);
+    for (uint8_t f : flags)
+        if (f > 1) return YGZB_ERR_INVALID;
+    s.restart_pending = flags[0]; s.has_pose = flags[1]; s.lost = flags[2]; s.has_depth = flags[3];
+    s.frames_since_kf = r.get<int32_t>(); s.next_frame = r.get<int32_t>(); s.next_mp = (long)r.get<int64_t>();
+    if (s.frames_since_kf < 0 || s.next_frame < 0 || s.next_mp < 0) return YGZB_ERR_INVALID;
+    // a state a settled stream can have (the round and push rely on it: a stream's first push queues its start pose, and
+    // a stream with key-frames tracks against them):
+    //  - no key-frame: never pushed -- no frame, flag, depth map or map point yet (a restart before the first push only
+    //    sets `start`);
+    //  - key-frames: their frames lie before the next one, a pose and a depth map (the first frame brought one), frames
+    //    tracked since the newest key-frame at most the frames after it, and the next map point id right behind its points
+    if (s.kfs.empty()) {
+        if (s.next_frame != 0 || s.frames_since_kf != 0 || s.next_mp != 0 || s.restart_pending || s.has_pose || s.lost || s.has_depth)
+            return YGZB_ERR_INVALID;
+    } else {
+        const KfInfo& kf = s.kfs.back();
+        if (s.next_frame <= kf.frame_id || !s.has_pose || !s.has_depth || s.frames_since_kf > s.next_frame - 1 - kf.frame_id ||
+            s.next_mp != kf.mp0 + kf.n)
+            return YGZB_ERR_INVALID;
+    }
+    for (long* c : {&s.n_keyframes, &s.n_ba, &s.n_candidates, &s.n_projected, &s.n_inliers, &s.ba_obs, &s.ba_pts, &s.ba_kfs, &s.ba_trials,
+                    &s.ba_iters, &s.n_restarts})
+        *c = (long)r.get<int64_t>();
+    s.ba_flops = r.get<double>();
+    // 3. map: the key-frames of the host state, in the same order
+    ygzb_map_record& m = out.map.rec;
+    m.width = g.width; m.height = g.height; m.cells = g.cells; m.n_levels = g.n_levels;
+    std::memcpy(m.K, g.K, sizeof m.K);
+    m.n_keyframes = r.get<int32_t>();
+    if (!r.ok || m.n_keyframes != n_kf) return YGZB_ERR_INVALID;
+    size_t F = 0, O = 0;
+    for (int k = 0; k < n_kf; ++k) {
+        m.entry[k] = r.get<int32_t>(); m.n_features[k] = r.get<int32_t>(); m.n_obs[k] = r.get<int32_t>(); m.mp0[k] = r.get<int64_t>();
+        r.bytes(m.T_cw + 12 * (size_t)k, 12 * sizeof(double));
+        r.bytes(m.image + k * WH, WH);
+        if (m.entry[k] != s.kfs[k].entry || m.n_features[k] != s.kfs[k].n || m.mp0[k] != s.kfs[k].mp0 || m.n_obs[k] < 0 ||
+            m.n_obs[k] > YGZB_MAP_OBS_PER_CELL * g.cells)
+            return YGZB_ERR_INVALID;
+        F += (size_t)m.n_features[k];
+        O += (size_t)m.n_obs[k];
+    }
+    r.bytes(m.px, F * 2 * sizeof(double)); r.bytes(m.level, F); r.bytes(m.depth, F * sizeof(double)); r.bytes(m.pw, F * 3 * sizeof(double));
+    r.bytes(m.obs_id, O * sizeof(int64_t)); r.bytes(m.obs_px, O * 2 * sizeof(double));
+    if (!r.ok) return YGZB_ERR_INVALID;
+    for (size_t q = 0; q < F; ++q)
+        if (m.level[q] >= g.n_levels) return YGZB_ERR_INVALID;
+    // 4. reference: what a stream tracked against the previous frame aligns its next frame against, once it has one
+    out.has_ref = g.ref_mode == YGZB_TRACK_REF_PREVIOUS && n_kf > 0;
+    if (out.has_ref) {
+        ygzb_reference_record& q = out.ref.rec;
+        q.width = g.width; q.height = g.height; q.cells = g.cells; q.n_levels = g.n_levels;
+        std::memcpy(q.K, g.K, sizeof q.K);
+        q.n = r.get<int32_t>();
+        if (!r.ok || q.n < 0 || q.n > q.capacity) return YGZB_ERR_INVALID;
+        r.bytes(q.T_cw, sizeof q.T_cw);
+        r.bytes(q.px, (size_t)q.n * 2 * sizeof(double)); r.bytes(q.depth, (size_t)q.n * sizeof(double)); r.bytes(q.image, WH);
+    }
+    // 5. depth map
+    if (s.has_depth) {
+        out.depth.resize(WH);
+        r.bytes(out.depth.data(), WH * sizeof(double));
+    }
+    return r.ok && r.n == size ? YGZB_OK : YGZB_ERR_INVALID;
+}
+
+// page-locked staging of ygz_vo_save_stream, allocated on its first call: a map record at full capacity, a reference
+// record and a depth map in one ygzb_host_alloc, so that the exports copy straight into host memory
+struct SaveStage {
+    void* mem = nullptr;
+    ygzb_map_record map{};
+    ygzb_reference_record ref{};
+    double* depth = nullptr;
+    SaveStage() = default;
+    SaveStage(const SaveStage&) = delete;
+    SaveStage& operator=(const SaveStage&) = delete;
+    ~SaveStage() {
+        if (mem) ygzb_host_free(mem);
+    }
+    int init(const RecordGeom& g) {
+        size_t bytes = carve(g, nullptr);
+        CHK(ygzb_host_alloc(&mem, bytes));
+        carve(g, static_cast<uint8_t*>(mem));
+        return YGZB_OK;
+    }
+
+  private:
+    // lays the arrays out from base (nullptr: only sizes them), 8-byte aligned; returns the bytes
+    size_t carve(const RecordGeom& g, uint8_t* base) {
+        const size_t R = YGZB_TRACK_RING, F = R * g.cells, O = R * YGZB_MAP_OBS_PER_CELL * g.cells;
+        const size_t C = (size_t)YGZB_TRACK_REF_FEATURES_PER_CELL * g.cells, WH = g.wh();
+        size_t off = 0;
+        auto take = [&](auto*& p, size_t count) {
+            off = (off + 7) & ~(size_t)7;
+            p = base ? reinterpret_cast<std::remove_reference_t<decltype(p)>>(base + off) : nullptr;
+            off += count * sizeof(*p);
+        };
+        take(map.T_cw, 12 * R); take(map.mp0, R); take(map.px, 2 * F); take(map.depth, F); take(map.pw, 3 * F); take(map.obs_id, O);
+        take(map.obs_px, 2 * O); take(map.entry, R); take(map.n_features, R); take(map.n_obs, R); take(map.level, F); take(map.image, R * WH);
+        take(ref.px, 2 * C); take(ref.depth, C); take(ref.image, WH);
+        take(depth, WH);
+        ref.capacity = (int32_t)C;
+        return off;
     }
 };
 
@@ -1126,6 +1398,8 @@ struct ygz_vo {
     ygzb_ctx* ctx;
     int n_streams, width, height;
     std::unique_ptr<Engine> eng;
+    RecordGeom geom{};   // what this engine's stream records are made under
+    SaveStage stage;     // staging of ygz_vo_save_stream (allocated on its first call)
 };
 
 extern "C" {
@@ -1267,6 +1541,9 @@ int ygz_vo_create(ygzb_ctx* ctx, const ygz_vo_config* cfg, ygz_vo** out) {
     Params prm{cfg->kf_min_frames, cfg->kf_min_rot, cfg->kf_min_trans, cfg->ref_mode, cfg->min_inliers, {cfg->K[0], cfg->K[1], cfg->K[2], cfg->K[3]}};
     std::unique_ptr<ygz_vo> vo(new (std::nothrow) ygz_vo{ctx, cfg->n_streams, cp.image_width, cp.image_height, nullptr});
     if (!vo) return YGZB_ERR_INVALID;
+    int rows = 0, cols = 0;
+    CHK(ygzb_grid_dims(ctx, &rows, &cols));
+    vo->geom = RecordGeom{cp.image_width, cp.image_height, rows * cols, cp.n_levels, {cfg->K[0], cfg->K[1], cfg->K[2], cfg->K[3]}, cfg->ref_mode};
     vo->eng = std::make_unique<Engine>(ctx, cfg->n_streams, cfg->window, prm);
     vo->eng->set_outputs(nullptr, 0, true);
     CHK(vo->eng->init(nullptr));
@@ -1315,6 +1592,49 @@ int ygz_vo_stream_stats(ygz_vo* vo, int stream, int64_t stats[16]) {
 int ygz_vo_export_map(ygz_vo* vo, int stream, ygzb_map_record* out) {
     if (!vo || !out || stream < 0 || stream >= vo->n_streams) return YGZB_ERR_INVALID;
     return vo->eng->export_map(stream, out);
+}
+
+int ygz_vo_stream_record_bound(const ygz_vo* vo, size_t* bytes) {
+    if (!vo || !bytes) return YGZB_ERR_INVALID;
+    *bytes = record_bound(vo->geom);
+    return YGZB_OK;
+}
+
+// the stream's map, reference and depth map into the page-locked staging, one synchronisation, then the live rows into
+// the caller's buffer
+int ygz_vo_save_stream(ygz_vo* vo, int stream, void* buf, size_t capacity, size_t* size) {
+    if (!vo || !size || (!buf && capacity) || stream < 0 || stream >= vo->n_streams) return YGZB_ERR_INVALID;
+    Engine& e = *vo->eng;
+    if (!e.settled(stream)) return YGZB_ERR_INVALID;
+    if (!vo->stage.mem) CHK(vo->stage.init(vo->geom));
+    const EStream& s = e.streams()[stream];
+    SaveStage& st = vo->stage;
+    CHK(e.export_map(stream, &st.map));
+    const bool ref = e.has_reference(stream);
+    if (ref) CHK(e.export_reference(stream, &st.ref));
+    if (s.has_depth) CHK(e.get_depth(stream, st.depth));
+    CHK(ygzb_synchronize(vo->ctx));
+    RecordWriter count{nullptr};
+    write_record(count, vo->geom, s, st.map, ref ? &st.ref : nullptr, s.has_depth ? st.depth : nullptr);
+    *size = count.n;
+    if (count.n > capacity) return YGZB_ERR_CAPACITY;
+    RecordWriter w{static_cast<uint8_t*>(buf)};
+    write_record(w, vo->geom, s, st.map, ref ? &st.ref : nullptr, s.has_depth ? st.depth : nullptr);
+    return YGZB_OK;
+}
+
+// the whole record is unpacked and checked first (read_record, then the start pose), so a record that fails leaves the
+// stream as it was; then Engine::adopt installs it as it installs a stream handed over by the batch entry points
+int ygz_vo_load_stream(ygz_vo* vo, int stream, const void* buf, size_t size) {
+    if (!vo || !buf || stream < 0 || stream >= vo->n_streams) return YGZB_ERR_INVALID;
+    Engine& e = *vo->eng;
+    if (!e.settled(stream)) return YGZB_ERR_INVALID;
+    StreamRecord rec(vo->geom);
+    CHK(read_record(static_cast<const uint8_t*>(buf), size, vo->geom, rec));
+    CHK(e.check_start_pose(stream, rec.s.start));
+    CHK(e.adopt(stream, rec.s, &rec.map.rec, rec.has_ref ? &rec.ref.rec : nullptr));
+    if (rec.s.has_depth) CHK(e.set_depth(stream, rec.depth.data()));
+    return YGZB_OK;
 }
 
 void ygz_vo_destroy(ygz_vo* vo) { delete vo; }

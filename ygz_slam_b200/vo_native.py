@@ -42,6 +42,9 @@ def _lib():
         _LIB.ygz_vo_poll.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         _LIB.ygz_vo_stream_stats.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         _LIB.ygz_vo_export_map.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        _LIB.ygz_vo_stream_record_bound.argtypes = [C.c_void_p, C.c_void_p]
+        _LIB.ygz_vo_save_stream.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]
+        _LIB.ygz_vo_load_stream.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]
         _LIB.ygz_vo_destroy.argtypes = [C.c_void_p]
         _LIB.ygz_vo_destroy.restype = None
     return _LIB
@@ -143,6 +146,71 @@ RESULT_DTYPE = np.dtype([("stream", np.int32), ("frame", np.int32), ("tag", np.i
                          ("T_cw", np.float64, (12,))])   # ygz_vo_result
 
 
+# the int64 counters of a stream record's host state, in order (include/ygz_vo.h)
+_COUNTERS = ("n_keyframes", "n_ba", "n_candidates", "n_projected", "n_inliers", "ba_obs", "ba_pts", "ba_kfs", "ba_trials", "ba_iters",
+             "n_restarts")
+
+
+def stream_record_next_frame(rec):
+    """next_frame of a stream record (uint8 array) from its fixed offset: the 68-byte header, n_kf, n_kf key-frames of 116
+    bytes, the two poses, the four flags and frames_since_kf come before it."""
+    n_kf = int(rec[68:72].view("<i4")[0])
+    off = 72 + 116 * n_kf + 2 * 96 + 4 + 4
+    return int(rec[off:off + 4].view("<i4")[0])
+
+
+def parse_stream_record(data):
+    """The fields of a stream record (ygz_vo_save_stream, layout in include/ygz_vo.h) by name: (byte offset, value), with
+    per-key-frame fields named like "kf[1].entry" (host state) and "map[1].n_features" (map).  Values are numpy scalars
+    and arrays read from `data`; raises ValueError if the record is shorter than its counts say."""
+    buf = memoryview(bytes(data))
+    out, pos = {}, 0
+
+    def take(name, dtype, count=1):
+        nonlocal pos
+        dt = np.dtype(dtype).newbyteorder("<")
+        size = dt.itemsize * int(count)
+        if count < 0 or pos + size > len(buf):
+            raise ValueError(f"stream record ends inside {name}")
+        v = np.frombuffer(buf, dt, int(count), pos)
+        out[name] = (pos, v[0] if count == 1 else v)
+        pos += size
+        return out[name][1]
+
+    take("magic", "u1", 4)
+    take("version", "u4"); take("size", "u8")
+    W, H = take("width", "i4"), take("height", "i4")
+    take("cells", "i4"); take("n_levels", "i4"); take("K", "f8", 4)
+    mode = take("ref_mode", "i4")
+    n_kf = take("n_kf", "i4")
+    for k in range(n_kf):
+        take(f"kf[{k}].entry", "i4"); take(f"kf[{k}].n", "i4"); take(f"kf[{k}].frame_id", "i4"); take(f"kf[{k}].mp0", "i8")
+        take(f"kf[{k}].T_cw", "f8", 12)
+    take("T_cw", "f8", 12); take("start", "f8", 12)
+    take("restart_pending", "u1"); take("has_pose", "u1"); take("lost", "u1")
+    has_depth = take("has_depth", "u1")
+    take("frames_since_kf", "i4"); take("next_frame", "i4"); take("next_mp", "i8")
+    for c in _COUNTERS:
+        take(c, "i8")
+    take("ba_flops", "f8")
+    nk = take("n_keyframes", "i4")
+    F = O = 0
+    for k in range(nk):
+        take(f"map[{k}].entry", "i4")
+        F += int(take(f"map[{k}].n_features", "i4"))
+        O += int(take(f"map[{k}].n_obs", "i4"))
+        take(f"map[{k}].mp0", "i8"); take(f"map[{k}].T_cw", "f8", 12); take(f"map[{k}].image", "u1", W * H)
+    take("px", "f8", 2 * F); take("level", "u1", F); take("depth", "f8", F); take("pw", "f8", 3 * F)
+    take("obs_id", "i8", O); take("obs_px", "f8", 2 * O)
+    if mode == _REF_MODES["previous"] and n_kf > 0:
+        n = take("ref.n", "i4")
+        take("ref.T_cw", "f8", 12); take("ref.px", "f8", 2 * n); take("ref.depth", "f8", n); take("ref.image", "u1", W * H)
+    if has_depth:
+        take("depth_map", "f8", W * H)
+    out["end"] = (pos, None)
+    return out
+
+
 class Engine:
     """The device-resident engine fed frame by frame (include/ygz_vo.h): push frames per stream as they arrive, step or
     flush, poll the final results.  The image size is the context's; K (fx, fy, cx, cy in double) defaults to the
@@ -232,6 +300,28 @@ class Engine:
         self.ctx.check(self.lib.ygz_vo_export_map(self.h, int(stream), C.byref(m.rec)), "ygz_vo_export_map")
         self.ctx.synchronize()
         return m
+
+    def stream_record_bound(self):
+        """The most bytes a stream record of this engine can take (ygz_vo_stream_record_bound)."""
+        n = C.c_size_t(0)
+        self.ctx.check(self.lib.ygz_vo_stream_record_bound(self.h, C.byref(n)), "ygz_vo_stream_record_bound")
+        return n.value
+
+    def save_stream(self, stream):
+        """The whole state of `stream` as a stream record (bytes, the layout of include/ygz_vo.h); flush first.  The stream
+        is unchanged and may go on tracking."""
+        if not hasattr(self, "_record_buf"):
+            self._record_buf = np.empty(self.stream_record_bound(), np.uint8)
+        buf, n = self._record_buf, C.c_size_t(0)
+        self.ctx.check(self.lib.ygz_vo_save_stream(self.h, int(stream), buf.ctypes.data, buf.size, C.byref(n)), "ygz_vo_save_stream")
+        return buf[:n.value].tobytes()
+
+    def load_stream(self, stream, data):
+        """`stream` continues the stream saved in `data` (save_stream of any engine with the same geometry, camera and
+        reference mode): its next push gets the saved stream's next frame index."""
+        rec = np.frombuffer(data, np.uint8)
+        self.ctx.check(self.lib.ygz_vo_load_stream(self.h, int(stream), rec.ctypes.data, rec.size), "ygz_vo_load_stream")
+        self._pushed[stream] = stream_record_next_frame(rec)
 
     def close(self):
         if self.h:
