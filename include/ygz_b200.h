@@ -475,6 +475,26 @@ int ygzb_tracker_track(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, 
 int ygzb_tracker_make_keyframes(ygzb_tracker* t, int n, const ygzb_keyframe_job* jobs, const ygzb_ba_params* ba,
                                 ygzb_keyframe_result* results);
 
+/* ---- observations: the map points a tracked frame's pose rests on ----------------------------------------------------
+ * The reference keeps them in Frame::_features after LocalMapping::TrackLocalMap (LocalMapping.cpp:24-45, 82-146): one
+ * Feature per projected map point with its measured _pixel, its _mappoint and the _bad flag OptimizeCurrentPoseOnly sets.
+ * An observation row is one pose-only inlier of a tracking job: the map point's id, the pixel FindDirectProjection
+ * measured and the world position the frame was tracked against (the point may leave the ring, and with it every map
+ * record, two key-frames later).  A job's rows are its inliers in candidate order (local key-frame, then feature): the
+ * rows a key-frame made from that job takes over as its observations (obs_id / obs_px of a map record).              */
+typedef struct {
+    int64_t id;            /* map point id: mp0 of its key-frame + feature index                                      */
+    double px[2];          /* full-resolution pixel measured in the tracked frame (Feature::_pixel)                    */
+    double pw[3];          /* MapPoint::_pos_world as the frame was tracked against it                                */
+} ygzb_observation;        /* 48 bytes */
+/* From the next ygzb_tracker_track on, every batch writes job j's rows into host[j * YGZB_TRACK_RING * C ...] (C = grid
+ * cells), exactly results[j].n_inliers of them (0 for a job that did not align); they are valid after
+ * ygzb_synchronize(ctx).  A kernel behind pose-only writes them straight into `host`, which must be page-locked
+ * (ygzb_host_alloc): no further copy and no further synchronisation.  capacity (rows) >= max_jobs * YGZB_TRACK_RING * C.
+ * NULL switches the writes off (the next batch launches nothing for them).  YGZB_ERR_INVALID, with the tracker
+ * unchanged, for pageable memory or a capacity below that.                                                           */
+int ygzb_tracker_set_observations(ygzb_tracker* t, ygzb_observation* host, size_t capacity);
+
 /* ---- map record: the local map of one stream, out of a tracker and back into one ----------------------------------
  * The reference keeps its map in Memory / MapPoint objects any caller can read, and its System declares SaveMap /
  * LoadMap (include/ygz/system.h:63-67, never defined).  A map record is the tracker's side of that: `n_keyframes` ring

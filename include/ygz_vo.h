@@ -92,8 +92,26 @@ int ygz_vo_restart(ygz_vo* vo, int stream, const double T_cw[12]);
 int ygz_vo_step(ygz_vo* vo);
 /* rounds until nothing is queued or in flight: every pushed frame has its result                                    */
 int ygz_vo_flush(ygz_vo* vo);
-/* moves up to `capacity` final results, oldest first, into `out`; *n = how many                                     */
+/* moves up to `capacity` final results, oldest first, into `out`; *n = how many.  With observations on, the rows of
+ * the results it returns are discarded.                                                                            */
 int ygz_vo_poll(ygz_vo* vo, ygz_vo_result* out, int capacity, int* n);
+
+/* ---- observations: the map points each result's pose rests on (ygzb_observation, ygz_b200.h) --------------------------
+ * on != 0: every result final from here on carries its frame's pose-only inliers as observation rows (map point id,
+ * measured pixel, world point), in candidate order.  A result brings exactly n_inliers rows: a tracked frame's, a
+ * key-frame's (the rows its map record's obs_id / obs_px hold), a YGZ_VO_LOST frame whose pose-only kept too few
+ * inliers (its pose is the last good one); a sequence's first key-frame and a LOST frame after that bring none.  The
+ * tracker writes them into a page-locked buffer of n_streams * window * YGZB_TRACK_RING * cells rows (48 bytes each:
+ * 37.7 MB at 8 streams, window 8 and 3,072 cells), allocated when switched on and freed when switched off.  Stream
+ * records do not carry observations.  YGZB_ERR_INVALID, changing nothing, unless the engine is idle: nothing queued,
+ * no key-frame insertion pending, no result waiting to be polled.                                                  */
+int ygz_vo_set_observations(ygz_vo* vo, int on);
+/* ygz_vo_poll with the rows: moves whole results, oldest first, while they fit in `capacity` results and
+ * `obs_capacity` rows; result k's out[k].n_inliers rows follow those of result k - 1 in `obs`; *n results, *n_obs rows.
+ * YGZB_ERR_CAPACITY, moving nothing (*n = 0), when the rows of the first waiting result do not fit: *n_obs = its row
+ * count.  YGZB_ERR_INVALID for a NULL vo, n or n_obs, a NULL out or obs with a capacity, or observations off.       */
+int ygz_vo_poll_observations(ygz_vo* vo, ygz_vo_result* out, int capacity, int* n, ygzb_observation* obs, size_t obs_capacity,
+                             size_t* n_obs);
 /* the 16 counters ygz_vo_run reports per stream: lost, key-frames, local BAs, candidates, projected, inliers, BA
  * observations, BA points, BA key-frames, BA LM trials, BA iterations, BA model FLOP, restarts (ygz_vo_restart),
  * 0, 0, 0                                                                                                         */

@@ -45,7 +45,7 @@ EXPORTS = [
     "ygzb_tracker_create", "ygzb_tracker_destroy", "ygzb_tracker_set_depth", "ygzb_tracker_upload", "ygzb_tracker_track", "ygzb_tracker_make_keyframes",
     "ygzb_tracker_export", "ygzb_tracker_import", "ygzb_tracker_debug_job", "ygzb_tracker_set_reference_mode", "ygzb_tracker_debug_reference",
     "ygzb_tracker_export_reference", "ygzb_tracker_import_reference", "ygzb_undistort_map", "ygzb_frames_set_undistort",
-    "ygzb_tracker_set_start_pose", "ygzb_tracker_get_depth",
+    "ygzb_tracker_set_start_pose", "ygzb_tracker_get_depth", "ygzb_tracker_set_observations",
 ]
 
 

@@ -64,10 +64,12 @@ struct ygzb_tracker {
     void* d_ref;                   // reference store + the wave scratch of the sparse alignment (ref_cap features per problem)
     int32_t* h_aux;                // pinned [2][max_jobs]: job_ref_slot, orig
     int32_t* d_aux;
+    ygzb_observation* d_obs;       // device view of the caller's page-locked observation rows (ygzb_tracker_set_observations), or NULL
 };
 
 namespace {
 
+static_assert(sizeof(ygzb_observation) == 48, "an observation row is 48 bytes");
 constexpr size_t kf_stage_bytes = sizeof(ygzb_keyframe_job) + 12 * sizeof(double);   // a key-frame job and its start pose
 static_assert(sizeof(ygzb_keyframe_job) % sizeof(double) == 0, "the start poses behind the key-frame jobs are 8-byte aligned");
 
@@ -125,6 +127,32 @@ __device__ __forceinline__ int block_scan_1024(int v, int* s_w, int* total) {
     return out;
 }
 
+// the pose-only inliers of tracking job tj (batch position) in candidate order -- none when it did not align -- as rows
+// 0, 1, ...: emit(row, r, at, id) with the row's index r within its chunk of 1024 candidates, the candidate's index `at`
+// in the batch arrays and its map point's id; then, in every thread, chunk(first row of the chunk, rows of the chunk).
+// Called by a whole 1024-thread CTA (s_w as in block_scan_1024); returns the row count.  Both the key-frame observations
+// (kf_fill_kernel) and the frame observations (track_obs_kernel) are made here, so they follow one rule.
+template <typename Emit, typename Chunk>
+__device__ __forceinline__ int for_each_inlier(const TrackStore& st, const TrackBatch& b, int tj, int* s_w, Emit emit, Chunk chunk) {
+    const ygzb_track_job* job = b.jobs + tj;   // (read in place: a local copy would be indexed by k in local memory)
+    const int cnt = b.aligned[tj] ? b.c_cnt[tj] : 0;
+    int carry = 0;
+    for (int base = 0; base < cnt; base += 1024) {
+        const int q = base + (int)threadIdx.x;
+        const size_t at = (size_t)tj * b.cap + q;
+        const int flag = (q < cnt && b.inlier[at]) ? 1 : 0;
+        int chunk_total;
+        const int incl = block_scan_1024(flag, s_w, &chunk_total);
+        if (flag) {
+            const int c = b.c_src[at], k = c / st.cells, f = c - k * st.cells;
+            emit(carry + incl - 1, incl - 1, at, st.kf_mp0[job->stream * st.R + job->entry[k]] + f);
+        }
+        chunk(carry, chunk_total);
+        carry += chunk_total;   // (the same total in every thread; block_scan_1024 ends on a barrier)
+    }
+    return carry;
+}
+
 // SetKeyframe for job blockIdx.x: the features Detect left in the frame slot's store become the key-frame's features and
 // map points (depth image -> camera point -> world, VisualOdometry.cpp:182-218 with the depth initialisation of
 // test/test_feature_alignment.cpp:72-85), the inlier observations of its tracking job become its observations of older points.
@@ -133,14 +161,12 @@ __global__ void __launch_bounds__(1024) kf_fill_kernel(TrackStore st, TrackBatch
                                                       const double* __restrict__ start_T, const int32_t* __restrict__ f_count,
                                                       const int16_t* __restrict__ f_x, const int16_t* __restrict__ f_y,
                                                       const uint8_t* __restrict__ f_level, int n_cells, ygzb_keyframe_result* __restrict__ res) {
-    __shared__ int s_scan[1024];
-    __shared__ int s_carry;
+    __shared__ int s_scan[33];
     __shared__ double s_T[12], s_Tin[12];
     const ygzb_keyframe_job kj = jobs[blockIdx.x];
     const int tid = threadIdx.x, e = kj.stream * st.R + kj.entry;
     const int n = min(f_count[kj.frame_slot], st.cells);
     if (tid < 12) s_T[tid] = kj.track_job >= 0 ? b.T_cur[12 * (size_t)kj.track_job + tid] : start_T[12 * (size_t)blockIdx.x + tid];
-    if (tid == 0) s_carry = 0;
     __syncthreads();
     if (tid == 0) mat34_inv(s_T, s_Tin);
     __syncthreads();
@@ -168,29 +194,47 @@ __global__ void __launch_bounds__(1024) kf_fill_kernel(TrackStore st, TrackBatch
     // observations of older map points: the inliers of the tracking job, in candidate order
     int total = 0;
     if (kj.track_job >= 0) {
-        const int tj = kj.track_job;
-        const ygzb_track_job job = b.jobs[tj];
-        const int cnt = b.aligned[tj] ? b.c_cnt[tj] : 0;
-        for (int base = 0; base < cnt; base += 1024) {
-            const int q = base + tid;
-            const size_t at = (size_t)tj * b.cap + q;
-            const int flag = (q < cnt && b.inlier[at]) ? 1 : 0;
-            int chunk_total;
-            const int incl = block_scan_1024(flag, s_scan, &chunk_total);
-            if (flag) {
-                const size_t dst = (size_t)e * b.cap + s_carry + incl - 1;
-                const int c = b.c_src[at], k = c / st.cells, f = c - k * st.cells;
-                st.kf_obs_id[dst] = st.kf_mp0[job.stream * st.R + job.entry[k]] + f;
-                st.kf_obs_px[2 * dst] = b.c_px[2 * at];
-                st.kf_obs_px[2 * dst + 1] = b.c_px[2 * at + 1];
-            }
-            __syncthreads();
-            if (tid == 0) s_carry += chunk_total;
-            __syncthreads();
-        }
-        total = s_carry;
+        long long* obs_id = st.kf_obs_id + (size_t)e * b.cap;
+        double* obs_px = st.kf_obs_px + 2 * (size_t)e * b.cap;
+        total = for_each_inlier(
+            st, b, kj.track_job, s_scan,
+            [&](int row, int, size_t at, long long id) {
+                obs_id[row] = id;
+                obs_px[2 * row] = b.c_px[2 * at];
+                obs_px[2 * row + 1] = b.c_px[2 * at + 1];
+            },
+            [](int, int) {});
     }
     if (tid == 0) st.kf_nobs[e] = total;
+}
+
+// the observations of job blockIdx.x (batch position) behind its pose-only: its inliers as rows (map point id, measured
+// pixel, world point), written straight into the caller's page-locked buffer `out` (a mapped device pointer) at the rows
+// of the caller's job index -- only the live rows cross PCIe.  The rows of a chunk of candidates are assembled in shared
+// memory and leave as one contiguous run of 16-byte stores (full lines over PCIe, not 8-byte pieces 48 bytes apart).
+constexpr size_t kObsSmem = 1024 * sizeof(ygzb_observation);   // dynamic shared memory of track_obs_kernel: one chunk of rows
+__global__ void __launch_bounds__(1024) track_obs_kernel(TrackStore st, TrackBatch b, ygzb_observation* __restrict__ out) {
+    extern __shared__ int4 s_rows[];   // [1024 * 3]: the chunk's rows
+    __shared__ int s_scan[33];
+    const int j = blockIdx.x;
+    ygzb_observation* rows = out + (size_t)(b.orig ? b.orig[j] : j) * b.cap;
+    ygzb_observation* s_obs = reinterpret_cast<ygzb_observation*>(s_rows);
+    for_each_inlier(
+        st, b, j, s_scan,
+        [&](int, int r, size_t at, long long id) {
+            ygzb_observation& o = s_obs[r];
+            o.id = id;
+            o.px[0] = b.c_px[2 * at];
+            o.px[1] = b.c_px[2 * at + 1];
+            o.pw[0] = b.c_pw[3 * at];
+            o.pw[1] = b.c_pw[3 * at + 1];
+            o.pw[2] = b.c_pw[3 * at + 2];
+        },
+        [&](int first, int n) {   // (the next chunk's scan begins with a barrier: s_rows is read before it is rewritten)
+            __syncthreads();
+            int4* dst = reinterpret_cast<int4*>(rows + first);   // 48-byte rows: every row starts 16-byte aligned
+            for (int i = threadIdx.x; i < 3 * n; i += 1024) dst[i] = s_rows[i];
+        });
 }
 
 // previous-frame reference of job blockIdx.x after its pose-only refinement, into the stream's other buffer: its pose and its
@@ -624,6 +668,16 @@ int tracker_xfer(ygzb_tracker* t, MapXfer& X) {
     return YGZB_OK;
 }
 
+// the observation rows of a whole batch (all its jobs have been through pose-only), when the caller asked for them
+int launch_track_obs(ygzb_tracker* t, const TrackBatch& b) {
+    if (!t->d_obs) return YGZB_OK;
+    ygzb_ctx* ctx = t->ctx;
+    ProfScope ps(ctx, kStageOther);
+    track_obs_kernel<<<(unsigned)b.J, 1024, kObsSmem, ctx->stream>>>(t->st, b, t->d_obs);
+    YGZB_LAUNCHED(ctx);
+    return YGZB_OK;
+}
+
 // distinct ring entries in range (and distinct frame slots in range when `slots` is given)
 int check_entries(ygzb_tracker* t, int n, const int32_t* entries, const int32_t* slots, const char* what) {
     ygzb_ctx* ctx = t->ctx;
@@ -724,6 +778,8 @@ int track_previous(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, ygzb
         track_ref_write_kernel<<<(unsigned)wb.J, 256, 0, ctx->stream>>>(t->st, wb);
         YGZB_LAUNCHED(ctx);
     }
+    const int rc = launch_track_obs(t, b);   // every wave's jobs keep their rows of the batch arrays
+    if (rc != YGZB_OK) return rc;
     {
         ProfScope ps(ctx, kStageOther);
         track_finish_kernel<<<(n_jobs + 63) / 64, 64, 0, ctx->stream>>>(b);
@@ -1026,6 +1082,7 @@ int ygzb_tracker_track(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, 
     rc = launch_track_chain_mid(t->f, t->st, b);
     if (rc != YGZB_OK) return rc;
     rc = launch_pose_only_dev(ctx, n_jobs, b.c_off, b.c_cnt, b.c_pw, b.c_px, b.T_cur, b.inlier, b.c_depth, b.n_inl, b.enable, b.pose_ws, cl, b.cap);
+    if (rc == YGZB_OK) rc = launch_track_obs(t, b);
     if (rc != YGZB_OK) return rc;
     {
         ProfScope ps(ctx, kStageOther);
@@ -1143,6 +1200,39 @@ int ygzb_tracker_make_keyframes(ygzb_tracker* t, int n, const ygzb_keyframe_job*
         YGZB_CUDA(ctx, cudaEventRecord(t->e_fill, ctx->stream));
     }
     YGZB_CUDA(ctx, cudaMemcpyAsync(results, t->d_kfres, sizeof(ygzb_keyframe_result) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+    return YGZB_OK;
+}
+
+int ygzb_tracker_set_observations(ygzb_tracker* t, ygzb_observation* host, size_t capacity) {
+    if (!t) return YGZB_ERR_INVALID;
+    ygzb_ctx* ctx = t->ctx;
+    if (!host) {
+        t->d_obs = nullptr;
+        return YGZB_OK;
+    }
+    const size_t need = (size_t)t->max_jobs * t->b.cap;
+    if (capacity < need) return set_error(ctx, YGZB_ERR_INVALID, "set_observations: capacity %zu rows below max_jobs * %d * cells = %zu", capacity,
+                                          YGZB_TRACK_RING, need);
+    cudaSetDevice(ctx->device);
+    // the kernel writes through the device view of the allocation: both ends of the rows it may write must be page-locked
+    // host memory with a device mapping (ygzb_host_alloc); pageable memory has neither
+    void* dev[2] = {nullptr, nullptr};
+    const char* ends[2] = {reinterpret_cast<const char*>(host), reinterpret_cast<const char*>(host + need) - 1};
+    for (int k = 0; k < 2; ++k) {
+        cudaPointerAttributes a{};
+        if (cudaPointerGetAttributes(&a, ends[k]) != cudaSuccess) {
+            cudaGetLastError();
+            return set_error(ctx, YGZB_ERR_INVALID, "set_observations: not a page-locked host buffer");
+        }
+        if (a.type != cudaMemoryTypeHost || !a.devicePointer)
+            return set_error(ctx, YGZB_ERR_INVALID, "set_observations: not a page-locked host buffer (ygzb_host_alloc)");
+        dev[k] = a.devicePointer;
+    }
+    if (static_cast<char*>(dev[1]) - static_cast<char*>(dev[0]) != ends[1] - ends[0])
+        return set_error(ctx, YGZB_ERR_INVALID, "set_observations: the rows span more than one page-locked allocation");
+    if (reinterpret_cast<uintptr_t>(dev[0]) % 16) return set_error(ctx, YGZB_ERR_INVALID, "set_observations: rows not 16-byte aligned");
+    YGZB_CUDA(ctx, cudaFuncSetAttribute(track_obs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kObsSmem));
+    t->d_obs = static_cast<ygzb_observation*>(dev[0]);
     return YGZB_OK;
 }
 

@@ -573,7 +573,12 @@ struct EStream : Counters {
 
 class Engine {
     struct Win { int stream, first, count, job0; };   // a window in flight: frames [first, first + count) of a stream (job0 < 0: first frame)
-    struct KfFrame { int frame, n_inliers; int64_t tag; const double* depth; };   // the frame behind a pending key-frame job
+    struct KfFrame {   // the frame behind a pending key-frame job
+        int frame, n_inliers;
+        int64_t tag;
+        const double* depth;
+        size_t obs0, n_obs;   // its tracking job's observation rows in kf_rows_ (observations on)
+    };
   public:
     Engine(ygzb_ctx* ctx, int n_streams, int window, const Params& p) : ctx_(ctx), S_(n_streams), F_(std::max(1, window)), prm_(p), st_(n_streams) {
         for (int i = 0; i < S_; ++i) order_.push_back(i);
@@ -587,6 +592,7 @@ class Engine {
         if (fr_) ygzb_frames_destroy(fr_);
         if (h_res_) ygzb_host_free(h_res_);
         if (h_kres_) ygzb_host_free(h_kres_);
+        if (h_obs_) ygzb_host_free(h_obs_);
     }
     // order[i] = the caller's index of tracker stream i (images, depth maps, trajectory rows); identity unless set
     void set_order(const std::vector<int>& order) { order_ = order; }
@@ -662,8 +668,75 @@ class Engine {
         for (size_t k = 0; k < n; ++k) {
             out[k] = results_.front();
             results_.pop_front();
+            if (observations()) drop_rows(1);   // (ygz_vo_poll: the rows go with their result)
         }
         return n;
+    }
+    // whole results with their observation rows, oldest first, while both fit; YGZB_ERR_CAPACITY with *n = 0 and
+    // *n_obs = its row count when the first one's rows do not
+    int pop_results(ygz_vo_result* out, int capacity, int* n, ygzb_observation* obs, size_t obs_capacity, size_t* n_obs) {
+        *n = 0;
+        *n_obs = 0;
+        if (capacity > 0 && !results_.empty() && row_count_.front() > obs_capacity) {
+            *n_obs = row_count_.front();
+            return YGZB_ERR_CAPACITY;
+        }
+        size_t used = 0;
+        while (*n < capacity && *n < (int)results_.size() && used + row_count_[*n] <= obs_capacity) used += row_count_[(*n)++];
+        if (used) std::memcpy(obs, rows_.data() + rows_head_, used * sizeof(ygzb_observation));
+        std::copy(results_.begin(), results_.begin() + *n, out);
+        results_.erase(results_.begin(), results_.begin() + *n);
+        drop_rows(*n);
+        *n_obs = used;
+        return YGZB_OK;
+    }
+    // nothing queued, no key-frame insertion pending, no result waiting to be polled
+    bool idle() const {
+        for (const EStream& s : st_)
+            if (!s.queue.empty()) return false;
+        return kjobs_.empty() && results_.empty();
+    }
+    bool observations() const { return h_obs_ != nullptr; }
+    // the rows of the k oldest results have been polled: one buffer keeps its capacity across rounds, so a round neither
+    // allocates nor touches fresh pages once it has grown
+    void drop_rows(size_t k) {
+        for (size_t q = 0; q < k; ++q) {
+            rows_head_ += row_count_.front();
+            row_count_.pop_front();
+        }
+        if (rows_head_ == rows_.size()) {
+            rows_.clear();
+            rows_head_ = 0;
+        } else if (rows_head_ > rows_.size() / 2) {
+            rows_.erase(rows_.begin(), rows_.begin() + (ptrdiff_t)rows_head_);
+            rows_head_ = 0;
+        }
+    }
+    // on: every result from here on carries the observation rows of its frame (the tracker writes each job's rows into a
+    // page-locked buffer, allocated here: max_jobs * YGZB_TRACK_RING * cells rows); off: none, and the buffer is freed.
+    // Call only when idle()
+    int set_observations(bool on) {
+        if (on == observations()) return YGZB_OK;
+        if (!on) {
+            CHK(ygzb_tracker_set_observations(tr_, nullptr, 0));
+            CHK(ygzb_synchronize(ctx_));
+            ygzb_host_free(h_obs_);
+            h_obs_ = nullptr;
+            return YGZB_OK;
+        }
+        int rows = 0, cols = 0;
+        CHK(ygzb_grid_dims(ctx_, &rows, &cols));
+        obs_stride_ = (size_t)YGZB_TRACK_RING * rows * cols;
+        const size_t cap = (size_t)S_ * F_ * obs_stride_;
+        void* p = nullptr;
+        CHK(ygzb_host_alloc(&p, cap * sizeof(ygzb_observation)));
+        const int rc = ygzb_tracker_set_observations(tr_, static_cast<ygzb_observation*>(p), cap);
+        if (rc != YGZB_OK) {
+            ygzb_host_free(p);
+            return rc;
+        }
+        h_obs_ = static_cast<ygzb_observation*>(p);
+        return YGZB_OK;
     }
 
     // Batch feed: queues frames [queued, limit) of every stream from the stacked sequences images[caller stream] (with the
@@ -784,10 +857,12 @@ class Engine {
                 const double kbar = r.ba_points ? (double)r.ba_observations / r.ba_points : 0.0, dim = 6.0 * (kj.n_local - 1);
                 s.ba_flops += r.ba_trials * (300.0 * r.ba_observations + r.ba_points * (216.0 * kbar * kbar + 108.0 * kbar + 50.0) + dim * dim * dim / 3.0);
             }
-            emit(kj.stream, kframes_[q].frame, kframes_[q].tag, YGZ_VO_KEYFRAME, kframes_[q].n_inliers);
+            emit(kj.stream, kframes_[q].frame, kframes_[q].tag, YGZ_VO_KEYFRAME, kframes_[q].n_inliers, kf_rows_.data() + kframes_[q].obs0,
+                 kframes_[q].n_obs);
         }
         kjobs_.clear();
         kframes_.clear();
+        kf_rows_.clear();
         // ---- 4. results of the tracking batch
         for (const Win& b : wins_) {
             EStream& s = st_[b.stream];
@@ -808,6 +883,7 @@ class Engine {
             }
             for (int t = 0; t < b.count; ++t) {
                 const ygzb_track_result& r = h_res_[b.job0 + t];
+                const ygzb_observation* rows = job_rows(b.job0 + t);   // (exactly r.n_inliers of them)
                 if (!r.aligned) {   // Matcher::SparseImageAlignment returned false (Matcher.cpp:482-488)
                     s.lost = true;
                     emit_front(b.stream, YGZ_VO_LOST, 0);
@@ -817,17 +893,17 @@ class Engine {
                 s.n_projected += r.n_projected;
                 if (r.n_inliers < prm_.min_inliers) {
                     s.lost = true;
-                    emit_front(b.stream, YGZ_VO_LOST, r.n_inliers);
+                    emit_front(b.stream, YGZ_VO_LOST, r.n_inliers, rows);
                     break;
                 }
                 std::memcpy(s.T.m, r.T_cw, sizeof(s.T.m));
                 s.frames_since_kf += 1;
                 s.n_inliers += r.n_inliers;
                 if (need_keyframe(prm_, s.frames_since_kf, s.T, s.kfs.back().T)) {
-                    pend_keyframe(b.stream, b.stream * F_ + t, b.job0 + t, r.n_inliers);
+                    pend_keyframe(b.stream, b.stream * F_ + t, b.job0 + t, r.n_inliers, rows);
                     break;   // frames of the window behind the key-frame (speculative ones) stay queued: tracked again next round
                 }
-                emit_front(b.stream, YGZ_VO_TRACKED, r.n_inliers);
+                emit_front(b.stream, YGZ_VO_TRACKED, r.n_inliers, rows);
             }
         }
         wins_.clear();
@@ -891,23 +967,28 @@ class Engine {
         for (int t = 0; t < w; ++t) CHK(ygzb_tracker_upload(tr_, i * F_ + t, 1, q[t].image, fb));
         return YGZB_OK;
     }
+    // observation rows of job j of the tracking batch that has just come back (observations on), else NULL
+    const ygzb_observation* job_rows(int j) const { return h_obs_ ? h_obs_ + (size_t)j * obs_stride_ : nullptr; }
     // the stream's oldest queued frame becomes a key-frame: its insertion is enqueued at the start of the next round, its
-    // result is emitted once the insertion's local BA has come back
-    void pend_keyframe(int stream, int frame_slot, int track_job, int n_inliers) {
+    // result is emitted once the insertion's local BA has come back; its n_inliers observation rows (rows: its tracking
+    // job's, or NULL) are held with it until then, since the next round's batch reuses the buffer
+    void pend_keyframe(int stream, int frame_slot, int track_job, int n_inliers, const ygzb_observation* rows = nullptr) {
         EStream& s = st_[stream];
         const QFrame f = s.queue.front();
         s.queue.pop_front();
         kjobs_.push_back(make_kf_job(stream, frame_slot, track_job));
-        kframes_.push_back({s.next_frame++, n_inliers, f.tag, f.depth});
+        const size_t n_rows = rows ? (size_t)n_inliers : 0;
+        kframes_.push_back({s.next_frame++, n_inliers, f.tag, f.depth, kf_rows_.size(), n_rows});
+        if (n_rows) kf_rows_.insert(kf_rows_.end(), rows, rows + n_rows);
     }
-    // the stream's oldest queued frame is final with the stream's current pose
-    void emit_front(int stream, int status, int n_inliers) {
+    // the stream's oldest queued frame is final with the stream's current pose; rows: its n_inliers observation rows, or NULL
+    void emit_front(int stream, int status, int n_inliers, const ygzb_observation* rows = nullptr) {
         EStream& s = st_[stream];
         const int64_t tag = s.queue.front().tag;
         s.queue.pop_front();
-        emit(stream, s.next_frame++, tag, status, n_inliers);
+        emit(stream, s.next_frame++, tag, status, n_inliers, rows, rows ? (size_t)n_inliers : 0);
     }
-    void emit(int stream, int frame, int64_t tag, int status, int n_inliers) {
+    void emit(int stream, int frame, int64_t tag, int status, int n_inliers, const ygzb_observation* rows = nullptr, size_t n_rows = 0) {
         const EStream& s = st_[stream];
         if (traj_) {
             double* out = traj_ + ((size_t)order_[stream] * traj_frames_ + frame) * 12;
@@ -922,6 +1003,10 @@ class Engine {
             r.n_inliers = n_inliers;
             std::memcpy(r.T_cw, s.T.m, sizeof(r.T_cw));
             results_.push_back(r);
+            if (observations()) {
+                if (n_rows) rows_.insert(rows_.end(), rows, rows + n_rows);
+                row_count_.push_back(n_rows);
+            }
         }
     }
     ygzb_keyframe_job make_kf_job(int stream, int frame_slot, int track_job) const {
@@ -967,6 +1052,13 @@ class Engine {
     int traj_frames_ = 0;
     bool collect_ = false;
     std::deque<ygz_vo_result> results_;
+    // observations (set_observations): the tracker's page-locked rows, obs_stride_ rows per job; the rows of the results
+    // in results_, back to back from rows_head_ (row_count_: how many each); the rows of the pending key-frames
+    ygzb_observation* h_obs_ = nullptr;
+    size_t obs_stride_ = 0;
+    std::vector<ygzb_observation> rows_, kf_rows_;
+    size_t rows_head_ = 0;
+    std::deque<size_t> row_count_;
     bool blocking_sync_ = false;
 };
 
@@ -1581,6 +1673,17 @@ int ygz_vo_poll(ygz_vo* vo, ygz_vo_result* out, int capacity, int* n) {
     if (!vo || !n || capacity < 0 || (capacity > 0 && !out)) return YGZB_ERR_INVALID;
     *n = (int)vo->eng->pop_results(out, (size_t)capacity);
     return YGZB_OK;
+}
+
+int ygz_vo_set_observations(ygz_vo* vo, int on) {
+    if (!vo || !vo->eng->idle()) return YGZB_ERR_INVALID;
+    return vo->eng->set_observations(on != 0);
+}
+
+int ygz_vo_poll_observations(ygz_vo* vo, ygz_vo_result* out, int capacity, int* n, ygzb_observation* obs, size_t obs_capacity, size_t* n_obs) {
+    if (!vo || !n || !n_obs || capacity < 0 || (capacity > 0 && !out) || (obs_capacity > 0 && !obs) || !vo->eng->observations())
+        return YGZB_ERR_INVALID;
+    return vo->eng->pop_results(out, capacity, n, obs, obs_capacity, n_obs);
 }
 
 int ygz_vo_stream_stats(ygz_vo* vo, int stream, int64_t stats[16]) {

@@ -40,6 +40,8 @@ def _lib():
         _LIB.ygz_vo_step.argtypes = [C.c_void_p]
         _LIB.ygz_vo_flush.argtypes = [C.c_void_p]
         _LIB.ygz_vo_poll.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+        _LIB.ygz_vo_set_observations.argtypes = [C.c_void_p, C.c_int]
+        _LIB.ygz_vo_poll_observations.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
         _LIB.ygz_vo_stream_stats.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         _LIB.ygz_vo_export_map.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         _LIB.ygz_vo_stream_record_bound.argtypes = [C.c_void_p, C.c_void_p]
@@ -144,6 +146,8 @@ class VoConfig(C.Structure):
 STATUS = ("tracked", "keyframe", "lost")   # YGZ_VO_TRACKED / _KEYFRAME / _LOST
 RESULT_DTYPE = np.dtype([("stream", np.int32), ("frame", np.int32), ("tag", np.int64), ("status", np.int32), ("n_inliers", np.int32),
                          ("T_cw", np.float64, (12,))])   # ygz_vo_result
+OBS_DTYPE = np.dtype([("id", np.int64), ("px", np.float64, (2,)), ("pw", np.float64, (3,))])   # ygzb_observation
+_ERR_CAPACITY = -4   # YGZB_ERR_CAPACITY
 
 
 # the int64 counters of a stream record's host state, in order (include/ygz_vo.h)
@@ -215,10 +219,12 @@ class Engine:
     """The device-resident engine fed frame by frame (include/ygz_vo.h): push frames per stream as they arrive, step or
     flush, poll the final results.  The image size is the context's; K (fx, fy, cx, cy in double) defaults to the
     context's camera at the shortest decimal that rounds to it (520.9 for the float 520.9f), which is the TUM camera the
-    batch functions (run) use.  The pushed arrays are kept alive here until their results have been polled."""
+    batch functions (run) use.  The pushed arrays are kept alive here until their results have been polled.
+    observations=True: every result carries the map points its pose rests on (ygz_vo_set_observations), and poll
+    returns them too."""
 
     def __init__(self, ctx, n_streams, window=8, ref_mode="keyframe", kf_min_frames=10, kf_min_rot=0.1, kf_min_trans=0.1,
-                 min_inliers=30, K=None):
+                 min_inliers=30, K=None, observations=False):
         if ref_mode not in _REF_MODES:
             raise ValueError(f"ref_mode must be 'keyframe' or 'previous', not {ref_mode!r}")
         p = ctx.params
@@ -232,6 +238,16 @@ class Engine:
         ctx.check(self.lib.ygz_vo_create(ctx.h, C.byref(self.cfg), C.byref(self.h)), "ygz_vo_create")
         self._pushed = [0] * self.n_streams
         self._alive = {}   # (stream, frame) -> the arrays its result still needs
+        self.observations = False
+        self._obs = np.zeros(0, OBS_DTYPE)   # rows of one ygz_vo_poll_observations call, grown on demand
+        if observations:
+            self.set_observations(True)
+
+    def set_observations(self, on):
+        """Switch the observation rows of the results on or off (ygz_vo_set_observations): only while the engine is
+        idle -- nothing queued or pending, every result polled."""
+        self.ctx.check(self.lib.ygz_vo_set_observations(self.h, int(bool(on))), "ygz_vo_set_observations")
+        self.observations = bool(on)
 
     def push(self, stream, image, depth=None, tag=None):
         """Queue grey `image` (H, W) uint8 of `stream` with its depth map (H, W) float64, or None to keep the stream's current
@@ -266,7 +282,10 @@ class Engine:
         self.ctx.check(self.lib.ygz_vo_flush(self.h), "ygz_vo_flush")
 
     def poll(self, capacity=4096):
-        """Final results since the last poll, oldest first: a RESULT_DTYPE array (status indexes STATUS)."""
+        """Final results since the last poll, oldest first: a RESULT_DTYPE array (status indexes STATUS).  With
+        observations on, (results, rows): rows[k] is an OBS_DTYPE array of result k's n_inliers observations."""
+        if self.observations:
+            return self._poll_observations(capacity)
         out = []
         while True:
             buf = np.zeros(capacity, RESULT_DTYPE)
@@ -275,10 +294,35 @@ class Engine:
             out.append(buf[:n.value])
             if n.value < capacity:
                 break
-        res = np.concatenate(out)
+        return self._release(np.concatenate(out))
+
+    def _release(self, res):
         for s_, f in zip(res["stream"].tolist(), res["frame"].tolist()):
             self._alive.pop((s_, f), None)
         return res
+
+    def _poll_observations(self, capacity):
+        out, rows = [], []
+        if len(self._obs) == 0:
+            self._obs = np.zeros(4 * 4096, OBS_DTYPE)
+        while True:
+            buf = np.zeros(capacity, RESULT_DTYPE)
+            n, n_obs = C.c_int(0), C.c_size_t(0)
+            rc = self.lib.ygz_vo_poll_observations(self.h, buf.ctypes.data, capacity, C.byref(n), self._obs.ctypes.data, len(self._obs),
+                                                   C.byref(n_obs))
+            if rc == _ERR_CAPACITY:   # the next result's rows do not fit: grow the row buffer and ask again
+                self._obs = np.zeros(max(2 * len(self._obs), n_obs.value), OBS_DTYPE)
+                continue
+            self.ctx.check(rc, "ygz_vo_poll_observations")
+            if n.value == 0:
+                break
+            res = buf[:n.value]
+            ends = np.cumsum(res["n_inliers"])
+            assert ends[-1] == n_obs.value
+            out.append(res)
+            rows.extend(np.split(self._obs[:n_obs.value].copy(), ends[:-1]))
+        res = np.concatenate(out) if out else np.zeros(0, RESULT_DTYPE)
+        return self._release(res), rows
 
     def _stat_row(self, stream):
         row = np.zeros(16, np.int64)
