@@ -288,6 +288,18 @@ int ygzb_sparse_align(ygzb_frames* f, int n_problems, const int32_t* ref_slot, c
                       const int32_t* offsets, const double* px, const double* depth, const uint8_t* has_mappoint,
                       const double* T_cw_ref, double* T_cw_cur, int max_level, int min_level, int n_iter, double eps,
                       int32_t* n_meas, int32_t* iters_per_level /* n_problems x YGZB_MAX_LEVELS or NULL */);
+/* ygzb_sparse_align plus SparseImgAlign::getFisherInformation() (SparseImageAlign.cpp:52-57): fisher[21 p ..] = H_ of
+ * problem p divided by 5e-4 * 255 * 255 (in double), as the packed upper triangle of the symmetric 6x6 matrix, row by row
+ * (H00 H01 .. H05 H11 .. H55).  H_ is the one the last linearisation at min_level built (NLSSolver_impl.hpp:29-37):
+ * at the pose before the last update when the level stopped on eps, at the rejected trial pose when its step was rolled
+ * back (chi2 rose, or the LDL^T failed), at the last iterate when the level ran out of iterations.  Coordinates are those of
+ * the update T_cur_from_ref <- T_cur_from_ref * exp(-x), Sophus order [upsilon; omega].  With n_iter = 0, or a problem
+ * without features, the reference keeps a stale H_ of an earlier run; here it is all zeros.  fisher may be NULL; the
+ * poses, n_meas and iterations are bit-identical to ygzb_sparse_align's.                                               */
+int ygzb_sparse_align_fisher(ygzb_frames* f, int n_problems, const int32_t* ref_slot, const int32_t* cur_slot,
+                             const int32_t* offsets, const double* px, const double* depth, const uint8_t* has_mappoint,
+                             const double* T_cw_ref, double* T_cw_cur, int max_level, int min_level, int n_iter, double eps,
+                             int32_t* n_meas, int32_t* iters_per_level, double* fisher /* n_problems x 21 or NULL */);
 
 /* ---- ba:: ---------------------------------------------------------------------------------------
  * replaces ba::LocalBAG2O (src/Algorithm/BA.cpp:386-543; include/ygz/Algorithm/BA.h:60-66) with
@@ -494,6 +506,29 @@ typedef struct {
  * NULL switches the writes off (the next batch launches nothing for them).  YGZB_ERR_INVALID, with the tracker
  * unchanged, for pageable memory or a capacity below that.                                                           */
 int ygzb_tracker_set_observations(ygzb_tracker* t, ygzb_observation* host, size_t capacity);
+
+/* ---- pose information: how well a tracked frame's pose is determined ---------------------------------------------------
+ * Two symmetric 6x6 matrices per tracking job, each as its packed upper triangle, row by row (H00 H01 .. H05 H11 .. H55):
+ *   align_fisher  SparseImgAlign::getFisherInformation() of the job's sparse alignment (SparseImageAlign.cpp:52-57), with
+ *                 the rules of ygzb_sparse_align_fisher; the reference frame is the key-frame (YGZB_TRACK_REF_KEYFRAME)
+ *                 or the previous frame (YGZB_TRACK_REF_PREVIOUS).  Reported whatever `aligned` (the 0.2 motion rule)
+ *                 says.
+ *   pose_info     sum_i J_i^T J_i over the job's pose-only inliers -- exactly its observation rows, in candidate order --
+ *                 with J_i = d r_i / d delta at delta = 0, r_i = pi(exp(delta) T_cw P_w,i) - px_i in pixels (unit pixel
+ *                 noise), a left perturbation delta = [upsilon; omega] (Sophus exp), pi the context's camera (float
+ *                 fx, fy promoted to double, as the tracker projects), T_cw = results[j].T_cw and P_w / px the values
+ *                 the observation rows carry.  Zero for a job that did not align (it has no rows).
+ * Information, not covariance: a caller inverts what it needs, and a degenerate frame needs no special case.           */
+typedef struct {
+    double align_fisher[21];
+    double pose_info[21];
+} ygzb_pose_information;   /* 336 bytes */
+/* From the next ygzb_tracker_track on, every batch writes job j's record into host[j]; valid after ygzb_synchronize(ctx).
+ * A kernel behind pose-only writes it straight into `host`, which must be page-locked (ygzb_host_alloc): no further copy
+ * and no further synchronisation.  capacity (records) >= max_jobs.  A job's record does not depend on the batch it is
+ * in.  NULL switches the records off (the next batch launches nothing for them).  YGZB_ERR_INVALID, with the tracker
+ * unchanged, for pageable memory or a capacity below max_jobs.                                                        */
+int ygzb_tracker_set_information(ygzb_tracker* t, ygzb_pose_information* host, size_t capacity);
 
 /* ---- map record: the local map of one stream, out of a tracker and back into one ----------------------------------
  * The reference keeps its map in Memory / MapPoint objects any caller can read, and its System declares SaveMap /

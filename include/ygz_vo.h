@@ -92,8 +92,8 @@ int ygz_vo_restart(ygz_vo* vo, int stream, const double T_cw[12]);
 int ygz_vo_step(ygz_vo* vo);
 /* rounds until nothing is queued or in flight: every pushed frame has its result                                    */
 int ygz_vo_flush(ygz_vo* vo);
-/* moves up to `capacity` final results, oldest first, into `out`; *n = how many.  With observations on, the rows of
- * the results it returns are discarded.                                                                            */
+/* moves up to `capacity` final results, oldest first, into `out`; *n = how many.  With observations or information on,
+ * the rows and records of the results it returns are discarded.                                                    */
 int ygz_vo_poll(ygz_vo* vo, ygz_vo_result* out, int capacity, int* n);
 
 /* ---- observations: the map points each result's pose rests on (ygzb_observation, ygz_b200.h) --------------------------
@@ -112,6 +112,26 @@ int ygz_vo_set_observations(ygz_vo* vo, int on);
  * count.  YGZB_ERR_INVALID for a NULL vo, n or n_obs, a NULL out or obs with a capacity, or observations off.       */
 int ygz_vo_poll_observations(ygz_vo* vo, ygz_vo_result* out, int capacity, int* n, ygzb_observation* obs, size_t obs_capacity,
                              size_t* n_obs);
+
+/* ---- pose information: how well each result's pose is determined (ygzb_pose_information, ygz_b200.h) -----------------
+ * on != 0: every result final from here on carries an information record: the sparse alignment's Fisher information
+ * (SparseImgAlign::getFisherInformation) and pose-only's information matrix of the returned T_cw, both as packed upper
+ * triangles of symmetric 6x6 matrices.  Which record a result carries:
+ *   YGZ_VO_TRACKED    its tracking job's;
+ *   YGZ_VO_KEYFRAME   its tracking job's, computed at the tracked pose BEFORE the key-frame's local BA (the result's
+ *                     T_cw is the pose after it);
+ *   a sequence's first key-frame and every YGZ_VO_LOST result: all zeros.
+ * The records do not depend on the window or the pacing.  The tracker writes them into a page-locked buffer of
+ * n_streams * window records (336 bytes each), allocated when switched on and freed when switched off.  Stream records
+ * do not carry them.  YGZB_ERR_INVALID, changing nothing, unless the engine is idle (as ygz_vo_set_observations).     */
+int ygz_vo_set_information(ygz_vo* vo, int on);
+/* one poll for both attachments: moves whole results, oldest first, into `out`; info[k] is out[k]'s record.  info must
+ * be non-NULL exactly when information is on (room for `capacity` records).  With observations on, obs, obs_capacity and
+ * n_obs follow ygz_vo_poll_observations (YGZB_ERR_CAPACITY included); with observations off obs must be NULL and
+ * obs_capacity 0, and n_obs (may be NULL) is set to 0.  YGZB_ERR_INVALID for a NULL vo or n, a NULL out with a capacity,
+ * or attachments that do not match what is switched on.                                                            */
+int ygz_vo_poll_ex(ygz_vo* vo, ygz_vo_result* out, int capacity, int* n, ygzb_pose_information* info, ygzb_observation* obs,
+                   size_t obs_capacity, size_t* n_obs);
 /* the 16 counters ygz_vo_run reports per stream: lost, key-frames, local BAs, candidates, projected, inliers, BA
  * observations, BA points, BA key-frames, BA LM trials, BA iterations, BA model FLOP, restarts (ygz_vo_restart),
  * 0, 0, 0                                                                                                         */

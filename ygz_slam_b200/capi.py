@@ -46,6 +46,7 @@ EXPORTS = [
     "ygzb_tracker_export", "ygzb_tracker_import", "ygzb_tracker_debug_job", "ygzb_tracker_set_reference_mode", "ygzb_tracker_debug_reference",
     "ygzb_tracker_export_reference", "ygzb_tracker_import_reference", "ygzb_undistort_map", "ygzb_frames_set_undistort",
     "ygzb_tracker_set_start_pose", "ygzb_tracker_get_depth", "ygzb_tracker_set_observations",
+    "ygzb_sparse_align_fisher", "ygzb_tracker_set_information",
 ]
 
 
@@ -103,6 +104,9 @@ class _Pinned:
             self.lib.ygzb_host_free(self.ptr)
         except Exception:
             pass
+
+
+INFO_DTYPE = np.dtype([("align_fisher", np.float64, (21,)), ("pose_info", np.float64, (21,))])   # ygzb_pose_information
 
 
 def pinned_empty(shape, dtype):
@@ -441,18 +445,34 @@ def _project_align(self, ref_slot, cur_slot, poses, ref_pose, cur_pose, ref_px, 
     return cur, lvl.astype(np.int32), ok.astype(bool)
 
 
-def _sparse_align(self, ref_slot, cur_slot, offsets, px, depth, has_mp, T_ref, T_cur, max_level=2, min_level=0, n_iter=30, eps=1e-6):
+def _sparse_align(self, ref_slot, cur_slot, offsets, px, depth, has_mp, T_ref, T_cur, max_level=2, min_level=0, n_iter=30, eps=1e-6,
+                  fisher=False):
+    """fisher=True: ygzb_sparse_align_fisher, which also returns each problem's getFisherInformation() as [P, 6, 6]."""
     ref_slot = np.ascontiguousarray(ref_slot, np.int32)
     P = len(ref_slot)
     T = np.ascontiguousarray(T_cur, np.float64).reshape(P, 12).copy()
     nm = np.zeros(P, np.int32)
     iters = np.zeros((P, MAX_LEVELS), np.int32)
-    self.ctx.check(self.lib.ygzb_sparse_align(
-        self.h, P, _p(ref_slot), _p(np.ascontiguousarray(cur_slot, np.int32)), _p(np.ascontiguousarray(offsets, np.int32)),
-        _p(np.ascontiguousarray(px, np.float64)), _p(np.ascontiguousarray(depth, np.float64)),
-        _p(np.ascontiguousarray(has_mp, np.uint8)), _p(np.ascontiguousarray(T_ref, np.float64).reshape(P, 12)), _p(T),
-        max_level, min_level, n_iter, C.c_double(eps), _p(nm), _p(iters)), "ygzb_sparse_align")
-    return T.reshape(P, 3, 4), nm, iters
+    args = (self.h, P, _p(ref_slot), _p(np.ascontiguousarray(cur_slot, np.int32)), _p(np.ascontiguousarray(offsets, np.int32)),
+            _p(np.ascontiguousarray(px, np.float64)), _p(np.ascontiguousarray(depth, np.float64)),
+            _p(np.ascontiguousarray(has_mp, np.uint8)), _p(np.ascontiguousarray(T_ref, np.float64).reshape(P, 12)), _p(T),
+            max_level, min_level, n_iter, C.c_double(eps), _p(nm), _p(iters))
+    if not fisher:
+        self.ctx.check(self.lib.ygzb_sparse_align(*args), "ygzb_sparse_align")
+        return T.reshape(P, 3, 4), nm, iters
+    packed = np.zeros((P, 21), np.float64)
+    self.ctx.check(self.lib.ygzb_sparse_align_fisher(*args, _p(packed)), "ygzb_sparse_align_fisher")
+    return T.reshape(P, 3, 4), nm, iters, unpack_sym6(packed)
+
+
+def unpack_sym6(packed):
+    """[..., 21] packed upper triangles (row by row) -> [..., 6, 6] symmetric matrices."""
+    packed = np.asarray(packed, np.float64)
+    out = np.zeros(packed.shape[:-1] + (6, 6))
+    r, c = np.triu_indices(6)
+    out[..., r, c] = packed
+    out[..., c, r] = packed
+    return out
 
 
 def _align1d(self, slot, level, direction, ref_border, ref, uv, n_iter=10):
@@ -889,6 +909,13 @@ class Tracker:
             self.close()
         except Exception:
             pass
+
+    def set_information(self, buf, capacity=None):
+        """ygzb_tracker_set_information: from the next track on, job j's record goes to buf[j] (a page-locked INFO_DTYPE
+        array, pinned_empty; None switches the records off).  Returns the C status."""
+        self.lib.ygzb_tracker_set_information.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+        return self.lib.ygzb_tracker_set_information(self.h, None if buf is None else buf.ctypes.data,
+                                                     (0 if buf is None else len(buf)) if capacity is None else capacity)
 
     def export(self, stream: int, entries, images: bool = True, out: MapBuffers | None = None) -> MapBuffers:
         """Map record of ring entries `entries` of `stream`, complete (the call synchronises the context)."""

@@ -354,6 +354,7 @@ struct SparseArgs {
     int32_t* iters_out;         // [n_problems][kMaxLevels] or null
     void* feat_scratch;         // global fall-back of the per-feature staging, feat_stride bytes per problem
     size_t feat_stride;
+    double* H_out;              // [n_problems][21] or null: H of the last linearisation at min_level (zeroed before the launch)
 };
 
 // ---- SparseImgAlign (ygzb_sparse_align and the tracking engine's batches) ----------------------------------------------
@@ -605,6 +606,8 @@ __global__ void __launch_bounds__(kSA2Threads) sparse_align2_kernel(const Sparse
                     n_meas += (unsigned long long)pr[kSA2Terms];
                 }
                 s_last_nmeas = n_meas;
+                if (a.H_out && lvl == a.min_level)   // (every iteration stores; the last linearisation's H stays)
+                    for (int k = 0; k < 21; ++k) a.H_out[21 * (size_t)prob + k] = tot[k];
                 double H[6][6], b[6], x[6];
                 int t = 0;
                 for (int r = 0; r < 6; ++r)
@@ -880,6 +883,7 @@ int launch_sparse_align2(ygzb_ctx* ctx, const SparseArgs& a, int n_problems, int
     });
     const int max_features = (int)(a.feat_stride / sizeof(SA2Feat));
     const int feat_cap = std::min(max_dyn / (int)sizeof(SA2Feat), (max_features + cluster - 1) / cluster);
+    if (a.H_out) YGZB_CUDA(ctx, cudaMemsetAsync(a.H_out, 0, sizeof(double) * 21 * (size_t)n_problems, ctx->stream));
     ProfScope ps(ctx, kStageSparseAlign);
     YGZB_CUDA(ctx, launch_cluster(sparse_align2_kernel, (unsigned)(n_problems * cluster), kSA2Threads, cluster,
                                   (size_t)feat_cap * sizeof(SA2Feat), ctx->stream, a, feat_cap));
@@ -892,7 +896,7 @@ int launch_sparse_align2(ygzb_ctx* ctx, const SparseArgs& a, int n_problems, int
 int launch_sparse_align(ygzb_frames* f, int n_problems, const int32_t* d_ref_slot, const int32_t* d_cur_slot,
                         const int32_t* d_offsets, const double* d_px, const double* d_depth, const uint8_t* d_has_mp,
                         const double* d_T_ref, double* d_T_cur, int max_level, int min_level, int n_iter, double eps,
-                        int32_t* d_n_meas, int32_t* d_iters, void* d_feat_scratch, size_t feat_stride) {
+                        int32_t* d_n_meas, int32_t* d_iters, void* d_feat_scratch, size_t feat_stride, double* d_H) {
     ygzb_ctx* ctx = f->ctx;
     if (n_problems <= 0) return YGZB_OK;
     SparseArgs a;
@@ -918,6 +922,7 @@ int launch_sparse_align(ygzb_frames* f, int n_problems, const int32_t* d_ref_slo
     a.iters_out = d_iters;
     a.feat_scratch = d_feat_scratch;
     a.feat_stride = feat_stride;
+    a.H_out = d_H;
     return launch_sparse_align2(ctx, a, n_problems, cluster_knob("YGZB_TRACK_CLUSTER", kTrackCluster, false));
 }
 
@@ -955,6 +960,7 @@ int launch_track_chain_front(ygzb_frames* f, const TrackStore& st, const TrackBa
     a.iters_out = nullptr;
     a.feat_scratch = b.sa2_scratch;
     a.feat_stride = sparse_align2_scratch_bytes(1, feat_cap);
+    a.H_out = b.align_H;
     return launch_sparse_align2(ctx, a, b.J, sparse_cluster);
 }
 

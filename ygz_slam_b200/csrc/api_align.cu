@@ -148,6 +148,14 @@ int ygzb_project_align(ygzb_frames* f, int n, const int32_t* ref_slot, const int
 int ygzb_sparse_align(ygzb_frames* f, int n_problems, const int32_t* ref_slot, const int32_t* cur_slot, const int32_t* offsets,
                       const double* px, const double* depth, const uint8_t* has_mappoint, const double* T_cw_ref, double* T_cw_cur,
                       int max_level, int min_level, int n_iter, double eps, int32_t* n_meas, int32_t* iters_per_level) {
+    return ygzb_sparse_align_fisher(f, n_problems, ref_slot, cur_slot, offsets, px, depth, has_mappoint, T_cw_ref, T_cw_cur, max_level,
+                                    min_level, n_iter, eps, n_meas, iters_per_level, nullptr);
+}
+
+int ygzb_sparse_align_fisher(ygzb_frames* f, int n_problems, const int32_t* ref_slot, const int32_t* cur_slot, const int32_t* offsets,
+                             const double* px, const double* depth, const uint8_t* has_mappoint, const double* T_cw_ref, double* T_cw_cur,
+                             int max_level, int min_level, int n_iter, double eps, int32_t* n_meas, int32_t* iters_per_level,
+                             double* fisher) {
     if (!f || n_problems < 1 || !ref_slot || !cur_slot || !offsets || !T_cw_ref || !T_cw_cur || !n_meas) return YGZB_ERR_INVALID;
     ygzb_ctx* ctx = f->ctx;
     cudaSetDevice(ctx->device);
@@ -163,7 +171,7 @@ int ygzb_sparse_align(ygzb_frames* f, int n_problems, const int32_t* ref_slot, c
     for (int p = 0; p < n_problems; ++p) max_nf = std::max(max_nf, offsets[p + 1] - offsets[p]);
     const size_t feat_stride = sparse_align2_scratch_bytes(1, max_nf);
     int32_t *d_slots, *d_off, *d_nmeas, *d_iters;
-    double *d_px, *d_depth, *d_Tref, *d_Tcur;
+    double *d_px, *d_depth, *d_Tref, *d_Tcur, *d_H;
     uint8_t *d_mp, *d_feat;
     void* buf = carve_scratch(ctx, 6, [&](Carver& c) {
         d_slots = c.take<int32_t>(2 * P);
@@ -176,6 +184,7 @@ int ygzb_sparse_align(ygzb_frames* f, int n_problems, const int32_t* ref_slot, c
         d_nmeas = c.take<int32_t>(P);
         d_iters = c.take<int32_t>(P * kMaxLevels);
         d_feat = c.take<uint8_t>(P * feat_stride);
+        d_H = c.take<double>(21 * P);
     });
     if (!buf) return YGZB_ERR_CUDA;
     {   // the inputs are the first seven sub-buffers of `buf`: one staged copy instead of eight pageable ones
@@ -193,11 +202,14 @@ int ygzb_sparse_align(ygzb_frames* f, int n_problems, const int32_t* ref_slot, c
     }
     YGZB_CUDA(ctx, cudaMemsetAsync(d_iters, 0, P * kMaxLevels * sizeof(int32_t), ctx->stream));
     TRY(launch_sparse_align(f, n_problems, d_slots, d_slots + P, d_off, d_px, d_depth, d_mp, d_Tref, d_Tcur, max_level, min_level,
-                            n_iter, eps, d_nmeas, d_iters, d_feat, feat_stride));
+                            n_iter, eps, d_nmeas, d_iters, d_feat, feat_stride, fisher ? d_H : nullptr));
     TRY(d2h(ctx, T_cw_cur, d_Tcur, 12 * P));
     TRY(d2h(ctx, n_meas, d_nmeas, P));
     if (iters_per_level) TRY(d2h(ctx, iters_per_level, d_iters, P * kMaxLevels));
+    if (fisher) TRY(d2h(ctx, fisher, d_H, 21 * P));
     YGZB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (fisher)   // SparseImgAlign::getFisherInformation: H_ / (5e-4 * 255 * 255), the image noise
+        for (size_t k = 0; k < 21 * P; ++k) fisher[k] /= kFisherNoise;
     return YGZB_OK;
 }
 

@@ -202,11 +202,12 @@ int launch_project_align(ygzb_frames* f, int n, const int32_t* d_ref_slot, const
 int launch_sparse_align(ygzb_frames* f, int n_problems, const int32_t* d_ref_slot, const int32_t* d_cur_slot,
                         const int32_t* d_offsets, const double* d_px, const double* d_depth, const uint8_t* d_has_mp,
                         const double* d_T_ref, double* d_T_cur, int max_level, int min_level, int n_iter, double eps,
-                        int32_t* d_n_meas, int32_t* d_iters, void* d_feat_scratch, size_t feat_stride);
+                        int32_t* d_n_meas, int32_t* d_iters, void* d_feat_scratch, size_t feat_stride, double* d_H = nullptr);
 // sparse_align2_kernel on kTrackCluster CTAs per problem (YGZB_TRACK_CLUSTER, as in the tracker).  d_feat_scratch holds feat_stride bytes per problem, at least
 // sparse_align2_scratch_bytes(1, features of the largest problem): the global fall-back for CTAs whose share of the features
 // does not fit shared memory.
 size_t sparse_align2_scratch_bytes(int n_problems, int max_features);
+constexpr double kFisherNoise = 5e-4 * 255 * 255;   // SparseImgAlign::getFisherInformation's sigma_i_sq (SparseImageAlign.cpp:54)
 constexpr int kTrackCluster = 4;   // CTAs per problem of the tracker's sparse alignment and pose-only (YGZB_TRACK_CLUSTER: 1, 2, 4 or 8)
 
 // bump allocator over one scratch buffer (all sub-buffers 256-byte aligned)

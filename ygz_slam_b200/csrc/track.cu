@@ -65,11 +65,13 @@ struct ygzb_tracker {
     int32_t* h_aux;                // pinned [2][max_jobs]: job_ref_slot, orig
     int32_t* d_aux;
     ygzb_observation* d_obs;       // device view of the caller's page-locked observation rows (ygzb_tracker_set_observations), or NULL
+    ygzb_pose_information* d_info; // device view of the caller's page-locked information records (ygzb_tracker_set_information), or NULL
 };
 
 namespace {
 
 static_assert(sizeof(ygzb_observation) == 48, "an observation row is 48 bytes");
+static_assert(sizeof(ygzb_pose_information) == 336, "an information record is 336 bytes");
 constexpr size_t kf_stage_bytes = sizeof(ygzb_keyframe_job) + 12 * sizeof(double);   // a key-frame job and its start pose
 static_assert(sizeof(ygzb_keyframe_job) % sizeof(double) == 0, "the start poses behind the key-frame jobs are 8-byte aligned");
 
@@ -237,6 +239,59 @@ __global__ void __launch_bounds__(1024) track_obs_kernel(TrackStore st, TrackBat
         });
 }
 
+// the pose information of job blockIdx.x (batch position) behind its pose-only, written straight into the caller's
+// page-locked record `out` (a mapped device pointer) of the caller's job index: the alignment's H scaled to
+// getFisherInformation, and sum J^T J over the job's inliers -- the set its observation rows hold (for_each_inlier) -- with
+// J = d pi(exp(delta) T_cw P_w) / d delta at delta = 0 (left perturbation [upsilon; omega]) at the job's pose-only result.
+// Each thread sums the candidates it visits in candidate order, the warps and then the 32 warp sums are added in a fixed
+// order: a record depends on its job alone, not on the batch, the wave or the pacing.
+__global__ void __launch_bounds__(1024) track_info_kernel(TrackStore st, TrackBatch b, double fx, double fy,
+                                                         ygzb_pose_information* __restrict__ out) {
+    __shared__ int s_scan[33];
+    __shared__ double s_T[12];
+    __shared__ double s_red[32][21];
+    const int j = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid < 12) s_T[tid] = b.T_cur[12 * (size_t)j + tid];
+    __syncthreads();
+    double acc[21];
+#pragma unroll
+    for (int k = 0; k < 21; ++k) acc[k] = 0.0;
+    for_each_inlier(
+        st, b, j, s_scan,
+        [&](int, int, size_t at, long long) {
+            const double* P = b.c_pw + 3 * at;
+            const double x = s_T[0] * P[0] + s_T[1] * P[1] + s_T[2] * P[2] + s_T[3];
+            const double y = s_T[4] * P[0] + s_T[5] * P[1] + s_T[6] * P[2] + s_T[7];
+            const double z = s_T[8] * P[0] + s_T[9] * P[1] + s_T[10] * P[2] + s_T[11];
+            const double zi = 1.0 / z, u = x * zi, v = y * zi;
+            // d pi / d P_c times d P_c / d delta = [I | -P_c^]
+            const double Ju[6] = {fx * zi, 0.0, -fx * u * zi, -fx * u * v, fx * (1.0 + u * u), -fx * v};
+            const double Jv[6] = {0.0, fy * zi, -fy * v * zi, -fy * (1.0 + v * v), fy * u * v, fy * u};
+            int t = 0;
+#pragma unroll
+            for (int r = 0; r < 6; ++r)
+#pragma unroll
+                for (int c = r; c < 6; ++c, ++t) acc[t] += Ju[r] * Ju[c] + Jv[r] * Jv[c];
+        },
+        [](int, int) {});
+#pragma unroll
+    for (int k = 0; k < 21; ++k) {
+        double v = acc[k];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xFFFFFFFFu, v, o);
+        if (lane == 0) s_red[warp][k] = v;
+    }
+    __syncthreads();
+    ygzb_pose_information* rec = out + (b.orig ? b.orig[j] : j);
+    if (tid < 21) {
+        double v = 0.0;
+        for (int w = 0; w < 32; ++w) v += s_red[w][tid];
+        rec->pose_info[tid] = v;
+    } else if (tid < 42) {
+        rec->align_fisher[tid - 21] = b.align_H[21 * (size_t)j + tid - 21] / kFisherNoise;
+    }
+}
+
 // previous-frame reference of job blockIdx.x after its pose-only refinement, into the stream's other buffer: its pose and its
 // projected candidates in candidate order; an inlier at the depth of its map point under that pose (OptimizeCurrent,
 // LocalMapping.cpp:130-134), an outlier at the depth pose-only left it (its last inlier round's, or -1).  Outliers stay:
@@ -314,6 +369,7 @@ TrackBatch wave_batch(const TrackBatch& b, int j0, int J) {
     w.cand_ok += c; w.cand_px += 2 * c; w.n_cand += j0; w.c_cnt += j0; w.c_off += j0; w.c_src += c;
     w.c_pw += 3 * c; w.c_px += 2 * c; w.c_depth += c; w.inlier += c; w.enable += c; w.n_inl += j0;
     w.results += j0; w.job_ref_slot += j0; w.orig += j0;
+    if (w.align_H) w.align_H += 21 * (size_t)j0;
     return w;
 }
 
@@ -678,6 +734,38 @@ int launch_track_obs(ygzb_tracker* t, const TrackBatch& b) {
     return YGZB_OK;
 }
 
+// the information records of a whole batch (all its jobs have been through pose-only), when the caller asked for them
+int launch_track_info(ygzb_tracker* t, const TrackBatch& b) {
+    if (!t->d_info) return YGZB_OK;
+    ygzb_ctx* ctx = t->ctx;
+    ProfScope ps(ctx, kStageOther);
+    track_info_kernel<<<(unsigned)b.J, 1024, 0, ctx->stream>>>(t->st, b, (double)ctx->prm.fx, (double)ctx->prm.fy, t->d_info);
+    YGZB_LAUNCHED(ctx);
+    return YGZB_OK;
+}
+
+// the device view of `bytes` bytes of page-locked host memory at `host` (ygzb_host_alloc), which a kernel writes through:
+// both ends must be page-locked host memory with a device mapping, in one allocation; pageable memory has neither
+int mapped_view(ygzb_ctx* ctx, const void* host, size_t bytes, size_t align, const char* what, void** out) {
+    void* dev[2] = {nullptr, nullptr};
+    const char* ends[2] = {static_cast<const char*>(host), static_cast<const char*>(host) + bytes - 1};
+    for (int k = 0; k < 2; ++k) {
+        cudaPointerAttributes a{};
+        if (cudaPointerGetAttributes(&a, ends[k]) != cudaSuccess) {
+            cudaGetLastError();
+            return set_error(ctx, YGZB_ERR_INVALID, "%s: not a page-locked host buffer", what);
+        }
+        if (a.type != cudaMemoryTypeHost || !a.devicePointer)
+            return set_error(ctx, YGZB_ERR_INVALID, "%s: not a page-locked host buffer (ygzb_host_alloc)", what);
+        dev[k] = a.devicePointer;
+    }
+    if (static_cast<char*>(dev[1]) - static_cast<char*>(dev[0]) != ends[1] - ends[0])
+        return set_error(ctx, YGZB_ERR_INVALID, "%s: the buffer spans more than one page-locked allocation", what);
+    if (reinterpret_cast<uintptr_t>(dev[0]) % align) return set_error(ctx, YGZB_ERR_INVALID, "%s: buffer not %zu-byte aligned", what, align);
+    *out = dev[0];
+    return YGZB_OK;
+}
+
 // distinct ring entries in range (and distinct frame slots in range when `slots` is given)
 int check_entries(ygzb_tracker* t, int n, const int32_t* entries, const int32_t* slots, const char* what) {
     ygzb_ctx* ctx = t->ctx;
@@ -753,6 +841,7 @@ int track_previous(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, ygzb
     }
     TrackBatch b = t->b;
     b.J = n_jobs;
+    if (!t->d_info) b.align_H = nullptr;
     b.prev = 1;
     b.job_ref_slot = t->d_aux;
     b.orig = t->d_aux + t->max_jobs;
@@ -778,7 +867,8 @@ int track_previous(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, ygzb
         track_ref_write_kernel<<<(unsigned)wb.J, 256, 0, ctx->stream>>>(t->st, wb);
         YGZB_LAUNCHED(ctx);
     }
-    const int rc = launch_track_obs(t, b);   // every wave's jobs keep their rows of the batch arrays
+    int rc = launch_track_obs(t, b);   // every wave's jobs keep their rows of the batch arrays
+    if (rc == YGZB_OK) rc = launch_track_info(t, b);
     if (rc != YGZB_OK) return rc;
     {
         ProfScope ps(ctx, kStageOther);
@@ -852,6 +942,7 @@ int ygzb_tracker_create(ygzb_frames* f, int n_streams, int max_jobs, const doubl
             b.inlier = c.take<uint8_t>(Cn); b.enable = c.take<uint8_t>(Cn); b.n_inl = c.take<int32_t>(J);
             b.pose_ws = c.take<double>(pose_only_ws_doubles((int)J));
             b.results = c.take<ygzb_track_result>(J);
+            b.align_H = c.take<double>(J * 21);
         };
         Carver sz(nullptr);
         carve(sz);
@@ -1060,6 +1151,7 @@ int ygzb_tracker_track(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, 
     memcpy(t->h_jobs, jobs, sizeof(ygzb_track_job) * (size_t)n_jobs);
     TrackBatch b = t->b;
     b.J = n_jobs;
+    if (!t->d_info) b.align_H = nullptr;
     t->last_J = n_jobs;
     t->pos_of.clear();
     const int cl = t->cluster;
@@ -1083,6 +1175,7 @@ int ygzb_tracker_track(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, 
     if (rc != YGZB_OK) return rc;
     rc = launch_pose_only_dev(ctx, n_jobs, b.c_off, b.c_cnt, b.c_pw, b.c_px, b.T_cur, b.inlier, b.c_depth, b.n_inl, b.enable, b.pose_ws, cl, b.cap);
     if (rc == YGZB_OK) rc = launch_track_obs(t, b);
+    if (rc == YGZB_OK) rc = launch_track_info(t, b);
     if (rc != YGZB_OK) return rc;
     {
         ProfScope ps(ctx, kStageOther);
@@ -1214,25 +1307,26 @@ int ygzb_tracker_set_observations(ygzb_tracker* t, ygzb_observation* host, size_
     if (capacity < need) return set_error(ctx, YGZB_ERR_INVALID, "set_observations: capacity %zu rows below max_jobs * %d * cells = %zu", capacity,
                                           YGZB_TRACK_RING, need);
     cudaSetDevice(ctx->device);
-    // the kernel writes through the device view of the allocation: both ends of the rows it may write must be page-locked
-    // host memory with a device mapping (ygzb_host_alloc); pageable memory has neither
-    void* dev[2] = {nullptr, nullptr};
-    const char* ends[2] = {reinterpret_cast<const char*>(host), reinterpret_cast<const char*>(host + need) - 1};
-    for (int k = 0; k < 2; ++k) {
-        cudaPointerAttributes a{};
-        if (cudaPointerGetAttributes(&a, ends[k]) != cudaSuccess) {
-            cudaGetLastError();
-            return set_error(ctx, YGZB_ERR_INVALID, "set_observations: not a page-locked host buffer");
-        }
-        if (a.type != cudaMemoryTypeHost || !a.devicePointer)
-            return set_error(ctx, YGZB_ERR_INVALID, "set_observations: not a page-locked host buffer (ygzb_host_alloc)");
-        dev[k] = a.devicePointer;
-    }
-    if (static_cast<char*>(dev[1]) - static_cast<char*>(dev[0]) != ends[1] - ends[0])
-        return set_error(ctx, YGZB_ERR_INVALID, "set_observations: the rows span more than one page-locked allocation");
-    if (reinterpret_cast<uintptr_t>(dev[0]) % 16) return set_error(ctx, YGZB_ERR_INVALID, "set_observations: rows not 16-byte aligned");
+    void* dev = nullptr;   // (16-byte aligned: the kernel writes the rows as 16-byte stores)
+    TRY(mapped_view(ctx, host, need * sizeof(ygzb_observation), 16, "set_observations", &dev));
     YGZB_CUDA(ctx, cudaFuncSetAttribute(track_obs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kObsSmem));
-    t->d_obs = static_cast<ygzb_observation*>(dev[0]);
+    t->d_obs = static_cast<ygzb_observation*>(dev);
+    return YGZB_OK;
+}
+
+int ygzb_tracker_set_information(ygzb_tracker* t, ygzb_pose_information* host, size_t capacity) {
+    if (!t) return YGZB_ERR_INVALID;
+    ygzb_ctx* ctx = t->ctx;
+    if (!host) {
+        t->d_info = nullptr;
+        return YGZB_OK;
+    }
+    const size_t need = (size_t)t->max_jobs;
+    if (capacity < need) return set_error(ctx, YGZB_ERR_INVALID, "set_information: capacity %zu records below max_jobs = %zu", capacity, need);
+    cudaSetDevice(ctx->device);
+    void* dev = nullptr;
+    TRY(mapped_view(ctx, host, need * sizeof(ygzb_pose_information), alignof(double), "set_information", &dev));
+    t->d_info = static_cast<ygzb_pose_information*>(dev);
     return YGZB_OK;
 }
 

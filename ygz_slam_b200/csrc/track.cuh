@@ -48,6 +48,7 @@ struct TrackBatch {
     double *T_ref, *T_cur;      // [J][12]; T_cur: reference pose in, aligned pose, then pose-only result
     double* T_aligned;          // [J][12]  the aligned pose (pose-only's start), kept for ygzb_tracker_debug_job
     void* sa2_scratch;          // global fall-back of sparse_align2_kernel's per-feature staging
+    double* align_H;            // [J][21] H of the alignment's last linearisation at level 0 (pose information on), or null
     // Matcher::SparseImageAlignment's motion check, poses relative to the local key-frames
     int32_t* aligned;           // [J]
     double* rel;                // [J][kTrackMaxLocal][12]

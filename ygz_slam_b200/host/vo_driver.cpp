@@ -578,6 +578,7 @@ class Engine {
         int64_t tag;
         const double* depth;
         size_t obs0, n_obs;   // its tracking job's observation rows in kf_rows_ (observations on)
+        ygzb_pose_information info;   // its tracking job's information record (information on; zeros for a first key-frame)
     };
   public:
     Engine(ygzb_ctx* ctx, int n_streams, int window, const Params& p) : ctx_(ctx), S_(n_streams), F_(std::max(1, window)), prm_(p), st_(n_streams) {
@@ -593,6 +594,7 @@ class Engine {
         if (h_res_) ygzb_host_free(h_res_);
         if (h_kres_) ygzb_host_free(h_kres_);
         if (h_obs_) ygzb_host_free(h_obs_);
+        if (h_info_) ygzb_host_free(h_info_);
     }
     // order[i] = the caller's index of tracker stream i (images, depth maps, trajectory rows); identity unless set
     void set_order(const std::vector<int>& order) { order_ = order; }
@@ -669,25 +671,39 @@ class Engine {
             out[k] = results_.front();
             results_.pop_front();
             if (observations()) drop_rows(1);   // (ygz_vo_poll: the rows go with their result)
+            if (information()) info_.pop_front();
         }
         return n;
     }
-    // whole results with their observation rows, oldest first, while both fit; YGZB_ERR_CAPACITY with *n = 0 and
-    // *n_obs = its row count when the first one's rows do not
-    int pop_results(ygz_vo_result* out, int capacity, int* n, ygzb_observation* obs, size_t obs_capacity, size_t* n_obs) {
+    // whole results, oldest first, with their information records (info; NULL: discarded) and, with observations on,
+    // their observation rows while those fit; YGZB_ERR_CAPACITY with *n = 0 and *n_obs = its row count when the first
+    // one's rows do not.  n_obs is only touched with observations on
+    int pop_results(ygz_vo_result* out, int capacity, int* n, ygzb_pose_information* info, ygzb_observation* obs, size_t obs_capacity,
+                    size_t* n_obs) {
         *n = 0;
-        *n_obs = 0;
-        if (capacity > 0 && !results_.empty() && row_count_.front() > obs_capacity) {
-            *n_obs = row_count_.front();
-            return YGZB_ERR_CAPACITY;
-        }
+        const bool rows = observations();
         size_t used = 0;
-        while (*n < capacity && *n < (int)results_.size() && used + row_count_[*n] <= obs_capacity) used += row_count_[(*n)++];
-        if (used) std::memcpy(obs, rows_.data() + rows_head_, used * sizeof(ygzb_observation));
+        if (rows) {
+            *n_obs = 0;
+            if (capacity > 0 && !results_.empty() && row_count_.front() > obs_capacity) {
+                *n_obs = row_count_.front();
+                return YGZB_ERR_CAPACITY;
+            }
+            while (*n < capacity && *n < (int)results_.size() && used + row_count_[*n] <= obs_capacity) used += row_count_[(*n)++];
+            if (used) std::memcpy(obs, rows_.data() + rows_head_, used * sizeof(ygzb_observation));
+        } else {
+            *n = std::min(capacity, (int)results_.size());
+        }
         std::copy(results_.begin(), results_.begin() + *n, out);
         results_.erase(results_.begin(), results_.begin() + *n);
-        drop_rows(*n);
-        *n_obs = used;
+        if (information()) {
+            if (info) std::copy(info_.begin(), info_.begin() + *n, info);
+            info_.erase(info_.begin(), info_.begin() + *n);
+        }
+        if (rows) {
+            drop_rows(*n);
+            *n_obs = used;
+        }
         return YGZB_OK;
     }
     // nothing queued, no key-frame insertion pending, no result waiting to be polled
@@ -697,6 +713,7 @@ class Engine {
         return kjobs_.empty() && results_.empty();
     }
     bool observations() const { return h_obs_ != nullptr; }
+    bool information() const { return h_info_ != nullptr; }
     // the rows of the k oldest results have been polled: one buffer keeps its capacity across rounds, so a round neither
     // allocates nor touches fresh pages once it has grown
     void drop_rows(size_t k) {
@@ -736,6 +753,29 @@ class Engine {
             return rc;
         }
         h_obs_ = static_cast<ygzb_observation*>(p);
+        return YGZB_OK;
+    }
+    // on: every result from here on carries the information record of its frame (the tracker writes each job's record
+    // into a page-locked buffer, allocated here: max_jobs records); off: none, and the buffer is freed.  Call only when
+    // idle()
+    int set_information(bool on) {
+        if (on == information()) return YGZB_OK;
+        if (!on) {
+            CHK(ygzb_tracker_set_information(tr_, nullptr, 0));
+            CHK(ygzb_synchronize(ctx_));
+            ygzb_host_free(h_info_);
+            h_info_ = nullptr;
+            return YGZB_OK;
+        }
+        const size_t cap = (size_t)S_ * F_;
+        void* p = nullptr;
+        CHK(ygzb_host_alloc(&p, cap * sizeof(ygzb_pose_information)));
+        const int rc = ygzb_tracker_set_information(tr_, static_cast<ygzb_pose_information*>(p), cap);
+        if (rc != YGZB_OK) {
+            ygzb_host_free(p);
+            return rc;
+        }
+        h_info_ = static_cast<ygzb_pose_information*>(p);
         return YGZB_OK;
     }
 
@@ -858,7 +898,7 @@ class Engine {
                 s.ba_flops += r.ba_trials * (300.0 * r.ba_observations + r.ba_points * (216.0 * kbar * kbar + 108.0 * kbar + 50.0) + dim * dim * dim / 3.0);
             }
             emit(kj.stream, kframes_[q].frame, kframes_[q].tag, YGZ_VO_KEYFRAME, kframes_[q].n_inliers, kf_rows_.data() + kframes_[q].obs0,
-                 kframes_[q].n_obs);
+                 kframes_[q].n_obs, &kframes_[q].info);
         }
         kjobs_.clear();
         kframes_.clear();
@@ -900,10 +940,10 @@ class Engine {
                 s.frames_since_kf += 1;
                 s.n_inliers += r.n_inliers;
                 if (need_keyframe(prm_, s.frames_since_kf, s.T, s.kfs.back().T)) {
-                    pend_keyframe(b.stream, b.stream * F_ + t, b.job0 + t, r.n_inliers, rows);
+                    pend_keyframe(b.stream, b.stream * F_ + t, b.job0 + t, r.n_inliers, rows, job_info(b.job0 + t));
                     break;   // frames of the window behind the key-frame (speculative ones) stay queued: tracked again next round
                 }
-                emit_front(b.stream, YGZ_VO_TRACKED, r.n_inliers, rows);
+                emit_front(b.stream, YGZ_VO_TRACKED, r.n_inliers, rows, job_info(b.job0 + t));
             }
         }
         wins_.clear();
@@ -969,26 +1009,32 @@ class Engine {
     }
     // observation rows of job j of the tracking batch that has just come back (observations on), else NULL
     const ygzb_observation* job_rows(int j) const { return h_obs_ ? h_obs_ + (size_t)j * obs_stride_ : nullptr; }
+    // information record of job j of the tracking batch that has just come back (information on), else NULL
+    const ygzb_pose_information* job_info(int j) const { return h_info_ ? h_info_ + j : nullptr; }
     // the stream's oldest queued frame becomes a key-frame: its insertion is enqueued at the start of the next round, its
     // result is emitted once the insertion's local BA has come back; its n_inliers observation rows (rows: its tracking
-    // job's, or NULL) are held with it until then, since the next round's batch reuses the buffer
-    void pend_keyframe(int stream, int frame_slot, int track_job, int n_inliers, const ygzb_observation* rows = nullptr) {
+    // job's, or NULL) and its tracking job's information record (info, or NULL: zeros) are held with it until then, since
+    // the next round's batch reuses the buffers
+    void pend_keyframe(int stream, int frame_slot, int track_job, int n_inliers, const ygzb_observation* rows = nullptr,
+                       const ygzb_pose_information* info = nullptr) {
         EStream& s = st_[stream];
         const QFrame f = s.queue.front();
         s.queue.pop_front();
         kjobs_.push_back(make_kf_job(stream, frame_slot, track_job));
         const size_t n_rows = rows ? (size_t)n_inliers : 0;
-        kframes_.push_back({s.next_frame++, n_inliers, f.tag, f.depth, kf_rows_.size(), n_rows});
+        kframes_.push_back({s.next_frame++, n_inliers, f.tag, f.depth, kf_rows_.size(), n_rows, info ? *info : ygzb_pose_information{}});
         if (n_rows) kf_rows_.insert(kf_rows_.end(), rows, rows + n_rows);
     }
-    // the stream's oldest queued frame is final with the stream's current pose; rows: its n_inliers observation rows, or NULL
-    void emit_front(int stream, int status, int n_inliers, const ygzb_observation* rows = nullptr) {
+    // the stream's oldest queued frame is final with the stream's current pose; rows: its n_inliers observation rows, or NULL;
+    // info: its information record, or NULL (zeros)
+    void emit_front(int stream, int status, int n_inliers, const ygzb_observation* rows = nullptr, const ygzb_pose_information* info = nullptr) {
         EStream& s = st_[stream];
         const int64_t tag = s.queue.front().tag;
         s.queue.pop_front();
-        emit(stream, s.next_frame++, tag, status, n_inliers, rows, rows ? (size_t)n_inliers : 0);
+        emit(stream, s.next_frame++, tag, status, n_inliers, rows, rows ? (size_t)n_inliers : 0, info);
     }
-    void emit(int stream, int frame, int64_t tag, int status, int n_inliers, const ygzb_observation* rows = nullptr, size_t n_rows = 0) {
+    void emit(int stream, int frame, int64_t tag, int status, int n_inliers, const ygzb_observation* rows = nullptr, size_t n_rows = 0,
+              const ygzb_pose_information* info = nullptr) {
         const EStream& s = st_[stream];
         if (traj_) {
             double* out = traj_ + ((size_t)order_[stream] * traj_frames_ + frame) * 12;
@@ -1007,6 +1053,7 @@ class Engine {
                 if (n_rows) rows_.insert(rows_.end(), rows, rows + n_rows);
                 row_count_.push_back(n_rows);
             }
+            if (information()) info_.push_back(info ? *info : ygzb_pose_information{});
         }
     }
     ygzb_keyframe_job make_kf_job(int stream, int frame_slot, int track_job) const {
@@ -1059,6 +1106,9 @@ class Engine {
     std::vector<ygzb_observation> rows_, kf_rows_;
     size_t rows_head_ = 0;
     std::deque<size_t> row_count_;
+    // information (set_information): the tracker's page-locked records, one per job; the records of the results in results_
+    ygzb_pose_information* h_info_ = nullptr;
+    std::deque<ygzb_pose_information> info_;
     bool blocking_sync_ = false;
 };
 
@@ -1683,7 +1733,22 @@ int ygz_vo_set_observations(ygz_vo* vo, int on) {
 int ygz_vo_poll_observations(ygz_vo* vo, ygz_vo_result* out, int capacity, int* n, ygzb_observation* obs, size_t obs_capacity, size_t* n_obs) {
     if (!vo || !n || !n_obs || capacity < 0 || (capacity > 0 && !out) || (obs_capacity > 0 && !obs) || !vo->eng->observations())
         return YGZB_ERR_INVALID;
-    return vo->eng->pop_results(out, capacity, n, obs, obs_capacity, n_obs);
+    return vo->eng->pop_results(out, capacity, n, nullptr, obs, obs_capacity, n_obs);
+}
+
+int ygz_vo_set_information(ygz_vo* vo, int on) {
+    if (!vo || !vo->eng->idle()) return YGZB_ERR_INVALID;
+    return vo->eng->set_information(on != 0);
+}
+
+int ygz_vo_poll_ex(ygz_vo* vo, ygz_vo_result* out, int capacity, int* n, ygzb_pose_information* info, ygzb_observation* obs,
+                   size_t obs_capacity, size_t* n_obs) {
+    if (!vo || !n || capacity < 0 || (capacity > 0 && !out)) return YGZB_ERR_INVALID;
+    Engine& e = *vo->eng;
+    if (e.information() != (info != nullptr)) return YGZB_ERR_INVALID;
+    if (e.observations() ? (!n_obs || (obs_capacity > 0 && !obs)) : (obs || obs_capacity > 0)) return YGZB_ERR_INVALID;
+    if (!e.observations() && n_obs) *n_obs = 0;
+    return e.pop_results(out, capacity, n, info, obs, obs_capacity, n_obs);
 }
 
 int ygz_vo_stream_stats(ygz_vo* vo, int stream, int64_t stats[16]) {

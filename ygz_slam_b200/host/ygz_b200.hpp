@@ -506,6 +506,13 @@ inline bool Align2D(Frame* cur, int level, uint8_t* ref_patch_with_border, uint8
 }
 }  // namespace cvutils
 
+// Matrix<double,6,6> is a plain row-major array here (SparseImgAlign::getFisherInformation's return type)
+struct Matrix66d {
+    double m[6][6] = {};
+    double operator()(int r, int c) const { return m[r][c]; }
+    double& operator()(int r, int c) { return m[r][c]; }
+};
+
 class SparseImgAlign {  // include/ygz/Algorithm/SparseImageAlign.h:12-58
   public:
     enum Method { GaussNewton, LevenbergMarquardt };
@@ -514,6 +521,7 @@ class SparseImgAlign {  // include/ygz/Algorithm/SparseImageAlign.h:12-58
     size_t run(Frame* ref_frame, Frame* cur_frame) {
         auto& rt = b200::Runtime::Get();
         const int n = (int)ref_frame->_features.size();
+        fisher_ = Matrix66d{};
         if (!n) return 0;
         std::vector<double> px(2 * (size_t)n), depth(n);
         std::vector<uint8_t> has(n);
@@ -529,13 +537,21 @@ class SparseImgAlign {  // include/ygz/Algorithm/SparseImageAlign.h:12-58
         b200::PoseTo3x4(cur_frame->_TCW, Tc);
         const int32_t rs = b200::SlotOf(ref_frame), cs = b200::SlotOf(cur_frame), off[2] = {0, n};
         int32_t n_meas = 0;
-        rt.Check(ygzb_sparse_align(rt.frames(), 1, &rs, &cs, off, px.data(), depth.data(), has.data(), Tr, Tc, max_level_, min_level_, n_iter_,
-                                   0.000001, &n_meas, nullptr), "ygzb_sparse_align");
+        double packed[21];
+        rt.Check(ygzb_sparse_align_fisher(rt.frames(), 1, &rs, &cs, off, px.data(), depth.data(), has.data(), Tr, Tc, max_level_, min_level_,
+                                          n_iter_, 0.000001, &n_meas, nullptr, packed),
+                 "ygzb_sparse_align_fisher");
+        for (int r = 0, t = 0; r < 6; ++r)
+            for (int c = r; c < 6; ++c, ++t) fisher_(r, c) = fisher_(c, r) = packed[t];
         cur_frame->_TCW = SE3::from3x4(Tc);
         return (size_t)n_meas;
     }
+    // SparseImageAlign.cpp:52-57: H_ / (5e-4 * 255^2) of the last run (zeros before any run, or after one that had no feature
+    // or n_iter = 0, where the reference keeps a stale H_)
+    Matrix66d getFisherInformation() const { return fisher_; }
   private:
     int max_level_, min_level_, n_iter_;
+    Matrix66d fisher_;
 };
 
 class Matcher {  // include/ygz/Algorithm/Matcher.h

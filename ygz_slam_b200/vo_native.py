@@ -8,6 +8,7 @@ from pathlib import Path
 import numpy as np
 
 from . import build
+from .capi import INFO_DTYPE, unpack_sym6
 
 _LIB = None
 
@@ -42,6 +43,8 @@ def _lib():
         _LIB.ygz_vo_poll.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         _LIB.ygz_vo_set_observations.argtypes = [C.c_void_p, C.c_int]
         _LIB.ygz_vo_poll_observations.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+        _LIB.ygz_vo_set_information.argtypes = [C.c_void_p, C.c_int]
+        _LIB.ygz_vo_poll_ex.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
         _LIB.ygz_vo_stream_stats.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         _LIB.ygz_vo_export_map.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         _LIB.ygz_vo_stream_record_bound.argtypes = [C.c_void_p, C.c_void_p]
@@ -221,10 +224,12 @@ class Engine:
     context's camera at the shortest decimal that rounds to it (520.9 for the float 520.9f), which is the TUM camera the
     batch functions (run) use.  The pushed arrays are kept alive here until their results have been polled.
     observations=True: every result carries the map points its pose rests on (ygz_vo_set_observations), and poll
-    returns them too."""
+    returns them too.  information=True: every result carries how well its pose is determined (ygz_vo_set_information):
+    poll also returns an [n, 2, 6, 6] array, the sparse alignment's Fisher information and pose-only's information
+    matrix of each result as full symmetric matrices."""
 
     def __init__(self, ctx, n_streams, window=8, ref_mode="keyframe", kf_min_frames=10, kf_min_rot=0.1, kf_min_trans=0.1,
-                 min_inliers=30, K=None, observations=False):
+                 min_inliers=30, K=None, observations=False, information=False):
         if ref_mode not in _REF_MODES:
             raise ValueError(f"ref_mode must be 'keyframe' or 'previous', not {ref_mode!r}")
         p = ctx.params
@@ -242,12 +247,21 @@ class Engine:
         self._obs = np.zeros(0, OBS_DTYPE)   # rows of one ygz_vo_poll_observations call, grown on demand
         if observations:
             self.set_observations(True)
+        self.information = False
+        if information:
+            self.set_information(True)
 
     def set_observations(self, on):
         """Switch the observation rows of the results on or off (ygz_vo_set_observations): only while the engine is
         idle -- nothing queued or pending, every result polled."""
         self.ctx.check(self.lib.ygz_vo_set_observations(self.h, int(bool(on))), "ygz_vo_set_observations")
         self.observations = bool(on)
+
+    def set_information(self, on):
+        """Switch the information records of the results on or off (ygz_vo_set_information): only while the engine is
+        idle, as set_observations."""
+        self.ctx.check(self.lib.ygz_vo_set_information(self.h, int(bool(on))), "ygz_vo_set_information")
+        self.information = bool(on)
 
     def push(self, stream, image, depth=None, tag=None):
         """Queue grey `image` (H, W) uint8 of `stream` with its depth map (H, W) float64, or None to keep the stream's current
@@ -283,7 +297,11 @@ class Engine:
 
     def poll(self, capacity=4096):
         """Final results since the last poll, oldest first: a RESULT_DTYPE array (status indexes STATUS).  With
-        observations on, (results, rows): rows[k] is an OBS_DTYPE array of result k's n_inliers observations."""
+        observations on, (results, rows): rows[k] is an OBS_DTYPE array of result k's n_inliers observations.  With
+        information on, (results, info) or (results, rows, info): info[k] = [alignment Fisher, pose information] of
+        result k, [n, 2, 6, 6] (zeros for a sequence's first key-frame and for LOST results)."""
+        if self.information:
+            return self._poll_ex(capacity)
         if self.observations:
             return self._poll_observations(capacity)
         out = []
@@ -323,6 +341,34 @@ class Engine:
             rows.extend(np.split(self._obs[:n_obs.value].copy(), ends[:-1]))
         res = np.concatenate(out) if out else np.zeros(0, RESULT_DTYPE)
         return self._release(res), rows
+
+    def _poll_ex(self, capacity):
+        out, rows, infos = [], [], []
+        if self.observations and len(self._obs) == 0:
+            self._obs = np.zeros(4 * 4096, OBS_DTYPE)
+        while True:
+            buf = np.zeros(capacity, RESULT_DTYPE)
+            info = np.zeros(capacity, INFO_DTYPE)
+            n, n_obs = C.c_int(0), C.c_size_t(0)
+            obs, obs_cap = (self._obs.ctypes.data, len(self._obs)) if self.observations else (None, 0)
+            rc = self.lib.ygz_vo_poll_ex(self.h, buf.ctypes.data, capacity, C.byref(n), info.ctypes.data, obs, obs_cap, C.byref(n_obs))
+            if rc == _ERR_CAPACITY:   # the next result's rows do not fit: grow the row buffer and ask again
+                self._obs = np.zeros(max(2 * len(self._obs), n_obs.value), OBS_DTYPE)
+                continue
+            self.ctx.check(rc, "ygz_vo_poll_ex")
+            if n.value == 0:
+                break
+            res = buf[:n.value]
+            out.append(res)
+            infos.append(info[:n.value])
+            if self.observations:
+                ends = np.cumsum(res["n_inliers"])
+                assert ends[-1] == n_obs.value
+                rows.extend(np.split(self._obs[:n_obs.value].copy(), ends[:-1]))
+        res = self._release(np.concatenate(out) if out else np.zeros(0, RESULT_DTYPE))
+        info = np.concatenate(infos) if infos else np.zeros(0, INFO_DTYPE)
+        full = np.stack([unpack_sym6(info["align_fisher"]), unpack_sym6(info["pose_info"])], axis=1)
+        return (res, rows, full) if self.observations else (res, full)
 
     def _stat_row(self, stream):
         row = np.zeros(16, np.int64)
