@@ -530,6 +530,28 @@ typedef struct {
  * unchanged, for pageable memory or a capacity below max_jobs.                                                        */
 int ygzb_tracker_set_information(ygzb_tracker* t, ygzb_pose_information* host, size_t capacity);
 
+/* ---- map updates: the local map as each key-frame insertion leaves it -------------------------------------------------
+ * The reference's LocalMapping::LocalBA (LocalMapping.cpp:149-172) writes its result back into the KeyFrame and MapPoint
+ * objects any caller can read.  Here the map lives in the tracker's ring, and an insertion changes two sets of points:
+ *   moved  the local BA's points, the points of the older local key-frames that at least two local key-frames observe,
+ *          in the BA's landmark order (local key-frame, then feature); exactly results[j].ba_points of them (0 without a
+ *          BA).  The new key-frame's own points have one observation and are never among them.
+ *   new    the key-frame's own points, ids mp0 .. mp0 + n_features - 1 in feature order; exactly results[j].n_features.
+ * A map point row is a point's id (mp0 of its key-frame + feature index) and its world position as the ring holds it
+ * after the insertion's BA write-back, bit for bit.  The poses of the local key-frames after the insertion are
+ * results[j].T_cw.                                                                                                     */
+typedef struct {
+    int64_t id;            /* map point id: mp0 of its key-frame + feature index                                      */
+    double pw[3];          /* MapPoint::_pos_world after the insertion                                                 */
+} ygzb_map_point;          /* 32 bytes */
+/* From the next ygzb_tracker_make_keyframes on, every batch writes key-frame job j's rows into
+ * host[j * YGZB_TRACK_RING * C ...] (C = grid cells): results[j].ba_points moved rows, then results[j].n_features new
+ * rows.  They are valid after ygzb_synchronize(ctx).  A kernel behind the BA's write-back writes them straight into
+ * `host`, which must be page-locked (ygzb_host_alloc): no further copy and no further synchronisation.
+ * capacity (rows) >= n_streams * YGZB_TRACK_RING * C.  NULL switches the writes off (the next batch launches nothing
+ * for them).  YGZB_ERR_INVALID, with the tracker unchanged, for pageable memory or a capacity below that.           */
+int ygzb_tracker_set_map_updates(ygzb_tracker* t, ygzb_map_point* host, size_t capacity);
+
 /* ---- map record: the local map of one stream, out of a tracker and back into one ----------------------------------
  * The reference keeps its map in Memory / MapPoint objects any caller can read, and its System declares SaveMap /
  * LoadMap (include/ygz/system.h:63-67, never defined).  A map record is the tracker's side of that: `n_keyframes` ring

@@ -132,6 +132,50 @@ int ygz_vo_set_information(ygz_vo* vo, int on);
  * or attachments that do not match what is switched on.                                                            */
 int ygz_vo_poll_ex(ygz_vo* vo, ygz_vo_result* out, int capacity, int* n, ygzb_pose_information* info, ygzb_observation* obs,
                    size_t obs_capacity, size_t* n_obs);
+
+/* ---- map updates: the local map as each key-frame insertion leaves it (ygzb_map_point, ygz_b200.h) --------------------
+ * A YGZ_VO_KEYFRAME result gives the key-frame's pose after its own local BA, but the BA also moves the older local
+ * key-frames (all but the oldest, which fixes the gauge) and the points at least two local key-frames observe.  With map
+ * updates on, every key-frame insertion brings one update: what it changed in the stream's local map.
+ *   - n_local, local_frame, T_cw: the local key-frames after the insertion, oldest first, by frame index, and their poses
+ *     as the ring holds them (the BA's, or the start pose for a sequence's first key-frame).  The last one is the new
+ *     key-frame; its T_cw equals its YGZ_VO_KEYFRAME result's bit for bit.
+ *   - n_moved rows: the BA's points in its landmark order (local key-frame, then feature); 0 for a first key-frame.
+ *   - n_new rows: the new key-frame's points, ids mp0 .. mp0 + n_new - 1 in feature order.
+ *   - retired_frame: the key-frame that left the local key-frames with this insertion, or -1.  No later BA includes it,
+ *     so its pose and the points it created are final for the sequence.
+ * Rows carry the positions the ring holds after the BA's write-back.  The two row sets never overlap, and a caller who
+ * applies every update in order holds the engine's map -- every pose and point ygz_vo_export_map would give -- at any
+ * time.  Map point ids restart from 0 with each sequence (ygz_vo_restart): key points by (stream, sequence, id).  A
+ * restart retires nothing: the new sequence's first update has sequence + 1, n_local 1, and the old sequence's
+ * key-frames are final as they were last reported.  The engine never revises a result: a caller who wants a tracked
+ * frame to follow a later move of the key-frame it was tracked against (the newest key-frame before it) keeps the
+ * relative pose, T_cw' = T_cw * T_kf^-1 * T_kf', with T_kf that key-frame's pose when the frame's result was final and
+ * T_kf' its pose from a later update.  A lost stream inserts no key-frame, so it brings no update until it is restarted. */
+typedef struct {
+    int32_t stream;            /* the caller's stream index                                                        */
+    int32_t frame;             /* the key-frame's frame index, the same as its YGZ_VO_KEYFRAME result's            */
+    int64_t sequence;          /* restarts of the stream before this key-frame (ygz_vo_stream_stats counter 12)    */
+    int32_t n_local;           /* local key-frames after the insertion (1 .. 3)                                    */
+    int32_t retired_frame;     /* frame index of the key-frame that stopped being local, or -1                     */
+    int32_t local_frame[YGZB_TRACK_RING];   /* their frame indices, oldest first; -1 past n_local                  */
+    int32_t n_moved, n_new;    /* row counts: the BA's points, then the new key-frame's points                     */
+    double T_cw[YGZB_TRACK_RING][12];       /* their poses (3x4 row-major) after the insertion; zeros past n_local */
+} ygz_vo_map_update;           /* 432 bytes */
+/* on != 0: every key-frame insertion final from here on queues its update, in a queue of its own (ygz_vo_poll and
+ * ygz_vo_poll_ex neither return nor discard updates).  An update is queued when its YGZ_VO_KEYFRAME result is.  The
+ * tracker writes the rows into a page-locked buffer of n_streams * YGZB_TRACK_RING * cells rows (32 bytes each: 3.1 MB at
+ * 8 streams and 3,072 cells), allocated when switched on and freed when switched off.  Stream records and the batch
+ * entry points do not carry updates.  YGZB_ERR_INVALID, changing nothing, unless the engine is idle (as
+ * ygz_vo_set_observations); with updates on, idle also means no update waiting to be polled, for this call,
+ * ygz_vo_set_observations and ygz_vo_set_information alike.                                                          */
+int ygz_vo_set_map_updates(ygz_vo* vo, int on);
+/* moves whole updates, oldest first, while they fit in `capacity` updates and `row_capacity` rows; update k's
+ * out[k].n_moved + out[k].n_new rows follow those of update k - 1 in `rows`; *n updates, *n_rows rows.
+ * YGZB_ERR_CAPACITY, moving nothing (*n = 0), when the rows of the first waiting update do not fit: *n_rows = its row
+ * count.  YGZB_ERR_INVALID for a NULL vo, n or n_rows, a NULL out or rows with a capacity, or map updates off.     */
+int ygz_vo_poll_map_updates(ygz_vo* vo, ygz_vo_map_update* out, int capacity, int* n, ygzb_map_point* rows, size_t row_capacity,
+                            size_t* n_rows);
 /* the 16 counters ygz_vo_run reports per stream: lost, key-frames, local BAs, candidates, projected, inliers, BA
  * observations, BA points, BA key-frames, BA LM trials, BA iterations, BA model FLOP, restarts (ygz_vo_restart),
  * 0, 0, 0                                                                                                         */

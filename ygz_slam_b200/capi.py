@@ -46,7 +46,7 @@ EXPORTS = [
     "ygzb_tracker_export", "ygzb_tracker_import", "ygzb_tracker_debug_job", "ygzb_tracker_set_reference_mode", "ygzb_tracker_debug_reference",
     "ygzb_tracker_export_reference", "ygzb_tracker_import_reference", "ygzb_undistort_map", "ygzb_frames_set_undistort",
     "ygzb_tracker_set_start_pose", "ygzb_tracker_get_depth", "ygzb_tracker_set_observations",
-    "ygzb_sparse_align_fisher", "ygzb_tracker_set_information",
+    "ygzb_sparse_align_fisher", "ygzb_tracker_set_information", "ygzb_tracker_set_map_updates",
 ]
 
 
@@ -107,6 +107,7 @@ class _Pinned:
 
 
 INFO_DTYPE = np.dtype([("align_fisher", np.float64, (21,)), ("pose_info", np.float64, (21,))])   # ygzb_pose_information
+MAP_POINT_DTYPE = np.dtype([("id", np.int64), ("pw", np.float64, (3,))])   # ygzb_map_point
 
 
 def pinned_empty(shape, dtype):
@@ -915,6 +916,14 @@ class Tracker:
         array, pinned_empty; None switches the records off).  Returns the C status."""
         self.lib.ygzb_tracker_set_information.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
         return self.lib.ygzb_tracker_set_information(self.h, None if buf is None else buf.ctypes.data,
+                                                     (0 if buf is None else len(buf)) if capacity is None else capacity)
+
+    def set_map_updates(self, buf, capacity=None):
+        """ygzb_tracker_set_map_updates: from the next make_keyframes on, key-frame job j's map rows (ba_points moved, then
+        n_features new) go to buf[j * TRACK_RING * cells ...] (a page-locked MAP_POINT_DTYPE array, pinned_empty; None
+        switches the rows off).  Returns the C status."""
+        self.lib.ygzb_tracker_set_map_updates.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+        return self.lib.ygzb_tracker_set_map_updates(self.h, None if buf is None else buf.ctypes.data,
                                                      (0 if buf is None else len(buf)) if capacity is None else capacity)
 
     def export(self, stream: int, entries, images: bool = True, out: MapBuffers | None = None) -> MapBuffers:

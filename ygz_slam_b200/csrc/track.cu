@@ -13,6 +13,7 @@
 // (host/vo_driver.cpp, ygz_slam_b200/vo.py) operation by operation.
 #include <algorithm>
 #include <cmath>
+#include <cstddef>
 #include <cstdlib>
 #include <cstring>
 #include <new>
@@ -66,12 +67,14 @@ struct ygzb_tracker {
     int32_t* d_aux;
     ygzb_observation* d_obs;       // device view of the caller's page-locked observation rows (ygzb_tracker_set_observations), or NULL
     ygzb_pose_information* d_info; // device view of the caller's page-locked information records (ygzb_tracker_set_information), or NULL
+    ygzb_map_point* d_map;         // device view of the caller's page-locked map rows (ygzb_tracker_set_map_updates), or NULL
 };
 
 namespace {
 
 static_assert(sizeof(ygzb_observation) == 48, "an observation row is 48 bytes");
 static_assert(sizeof(ygzb_pose_information) == 336, "an information record is 336 bytes");
+static_assert(sizeof(ygzb_map_point) == 32 && offsetof(ygzb_map_point, pw) == 8, "a map point row is 32 bytes: id, pw[3]");
 constexpr size_t kf_stage_bytes = sizeof(ygzb_keyframe_job) + 12 * sizeof(double);   // a key-frame job and its start pose
 static_assert(sizeof(ygzb_keyframe_job) % sizeof(double) == 0, "the start poses behind the key-frame jobs are 8-byte aligned");
 
@@ -545,6 +548,44 @@ size_t babuild_carve(Carver& c, BABuild& B, size_t P, int cells, int n_jobs) {
     B.tab = c.take<int32_t>(P * kTrackMaxLocal * kTrackMaxLocal * cells);
     B.prob_of = c.take<int32_t>((size_t)n_jobs);
     return c.bytes();
+}
+
+// the map rows of key-frame job blockIdx.x behind its BA write-back (ygzb_tracker_set_map_updates): the BA's points in its
+// landmark order (B.owner), then the new key-frame's points in feature order, each with its id and the ring's kf_pw as the
+// write-back left it, written straight into the caller's page-locked buffer `out` (a mapped device pointer) at
+// out[blockIdx.x * YGZB_TRACK_RING * cells].  The rows of a chunk are assembled in shared memory and leave as one
+// contiguous run of 16-byte stores, as track_obs_kernel's do.
+__global__ void __launch_bounds__(1024) kf_points_kernel(TrackStore st, const ygzb_keyframe_job* __restrict__ jobs, BABuild B,
+                                                        ygzb_map_point* __restrict__ out) {
+    __shared__ int4 s_rows[1024 * sizeof(ygzb_map_point) / sizeof(int4)];   // one chunk of 1024 rows
+    const ygzb_keyframe_job* kj = jobs + blockIdx.x;   // (read in place: local_entry is indexed by k)
+    const int p = B.prob_of[blockIdx.x];
+    const int n_moved = p >= 0 ? B.n_pt[p] : 0, e_new = kj->stream * st.R + kj->entry;
+    const int total = n_moved + st.kf_n[e_new];
+    ygzb_map_point* rows = out + (size_t)blockIdx.x * YGZB_TRACK_RING * st.cells;
+    ygzb_map_point* s_pts = reinterpret_cast<ygzb_map_point*>(s_rows);
+    for (int base = 0; base < total; base += 1024) {
+        const int q = base + (int)threadIdx.x;
+        if (q < total) {
+            int e = e_new, g = q - n_moved;
+            if (q < n_moved) {
+                const int i = B.owner[(size_t)p * B.pcap + q], k = i / st.cells;
+                e = kj->stream * st.R + kj->local_entry[k];
+                g = i - k * st.cells;
+            }
+            const size_t fe = (size_t)e * st.cells + g;
+            ygzb_map_point& m = s_pts[threadIdx.x];
+            m.id = st.kf_mp0[e] + g;
+            m.pw[0] = st.kf_pw[3 * fe];
+            m.pw[1] = st.kf_pw[3 * fe + 1];
+            m.pw[2] = st.kf_pw[3 * fe + 2];
+        }
+        __syncthreads();
+        const int n = min(1024, total - base);
+        int4* dst = reinterpret_cast<int4*>(rows + base);   // 32-byte rows: every row starts 16-byte aligned
+        for (int i = threadIdx.x; i < 2 * n; i += 1024) dst[i] = s_rows[i];
+        __syncthreads();   // s_rows is read before the next chunk rewrites it
+    }
 }
 
 // ---- map records (ygzb_tracker_export / _import) -----------------------------------------------------------------------
@@ -1292,6 +1333,11 @@ int ygzb_tracker_make_keyframes(ygzb_tracker* t, int n, const ygzb_keyframe_job*
         for (int i = 0; i < n; ++i) t->cur_ref[jobs[i].stream] = jobs[i].kf_slot;
         YGZB_CUDA(ctx, cudaEventRecord(t->e_fill, ctx->stream));
     }
+    if (t->d_map) {   // (behind the reference, so that previous-frame mode's next alignment does not wait for the rows)
+        ProfScope ps(ctx, kStageOther);
+        kf_points_kernel<<<(unsigned)n, 1024, 0, ctx->stream>>>(t->st, t->d_kfjobs, B, t->d_map);
+        YGZB_LAUNCHED(ctx);
+    }
     YGZB_CUDA(ctx, cudaMemcpyAsync(results, t->d_kfres, sizeof(ygzb_keyframe_result) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
     return YGZB_OK;
 }
@@ -1327,6 +1373,24 @@ int ygzb_tracker_set_information(ygzb_tracker* t, ygzb_pose_information* host, s
     void* dev = nullptr;
     TRY(mapped_view(ctx, host, need * sizeof(ygzb_pose_information), alignof(double), "set_information", &dev));
     t->d_info = static_cast<ygzb_pose_information*>(dev);
+    return YGZB_OK;
+}
+
+int ygzb_tracker_set_map_updates(ygzb_tracker* t, ygzb_map_point* host, size_t capacity) {
+    if (!t) return YGZB_ERR_INVALID;
+    ygzb_ctx* ctx = t->ctx;
+    if (!host) {
+        t->d_map = nullptr;
+        return YGZB_OK;
+    }
+    const size_t need = (size_t)t->st.S * YGZB_TRACK_RING * t->st.cells;   // a key-frame batch has at most one job per stream
+    if (capacity < need)
+        return set_error(ctx, YGZB_ERR_INVALID, "set_map_updates: capacity %zu rows below n_streams * %d * cells = %zu", capacity,
+                         YGZB_TRACK_RING, need);
+    cudaSetDevice(ctx->device);
+    void* dev = nullptr;   // (16-byte aligned: the kernel writes the rows as 16-byte stores)
+    TRY(mapped_view(ctx, host, need * sizeof(ygzb_map_point), 16, "set_map_updates", &dev));
+    t->d_map = static_cast<ygzb_map_point*>(dev);
     return YGZB_OK;
 }
 

@@ -18,6 +18,7 @@
 #include <bit>
 #include <chrono>
 #include <cmath>
+#include <cstddef>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -41,6 +42,11 @@ constexpr int kLocalKeyframes = 3;                                 // LocalMappi
 constexpr int kSlotsPerStream = kLocalKeyframes + 2;
 constexpr int kMinInliers = 30;                                    // vo.keyframe.min_features (default.yaml:66)
 constexpr int kSpeculativeFrames = 3;                              // engine: frames tracked ahead once a key-frame may trigger any time
+static_assert(sizeof(ygzb_map_point) == 32 && offsetof(ygzb_map_point, pw) == 8, "a map point row is 32 bytes: id, pw[3]");
+static_assert(sizeof(ygz_vo_map_update) == 432 && offsetof(ygz_vo_map_update, sequence) == 8 &&
+                  offsetof(ygz_vo_map_update, local_frame) == 24 && offsetof(ygz_vo_map_update, n_moved) == 40 &&
+                  offsetof(ygz_vo_map_update, T_cw) == 48,
+              "ygz_vo_map_update is laid out as include/ygz_vo.h documents");
 
 struct Mat34 {
     double m[12];
@@ -595,6 +601,7 @@ class Engine {
         if (h_kres_) ygzb_host_free(h_kres_);
         if (h_obs_) ygzb_host_free(h_obs_);
         if (h_info_) ygzb_host_free(h_info_);
+        if (h_map_) ygzb_host_free(h_map_);
     }
     // order[i] = the caller's index of tracker stream i (images, depth maps, trajectory rows); identity unless set
     void set_order(const std::vector<int>& order) { order_ = order; }
@@ -706,14 +713,41 @@ class Engine {
         }
         return YGZB_OK;
     }
-    // nothing queued, no key-frame insertion pending, no result waiting to be polled
+    // nothing queued, no key-frame insertion pending, no result or map update waiting to be polled
     bool idle() const {
         for (const EStream& s : st_)
             if (!s.queue.empty()) return false;
-        return kjobs_.empty() && results_.empty();
+        return kjobs_.empty() && results_.empty() && updates_.empty();
     }
     bool observations() const { return h_obs_ != nullptr; }
     bool information() const { return h_info_ != nullptr; }
+    bool map_updates() const { return h_map_ != nullptr; }
+    // whole map updates with their rows, oldest first, while both fit; YGZB_ERR_CAPACITY with *n = 0 and *n_rows = its row
+    // count when the first one's rows do not
+    int pop_map_updates(ygz_vo_map_update* out, int capacity, int* n, ygzb_map_point* rows, size_t row_capacity, size_t* n_rows) {
+        *n = 0;
+        *n_rows = 0;
+        auto count = [](const ygz_vo_map_update& u) { return (size_t)u.n_moved + (size_t)u.n_new; };
+        if (capacity > 0 && !updates_.empty() && count(updates_.front()) > row_capacity) {
+            *n_rows = count(updates_.front());
+            return YGZB_ERR_CAPACITY;
+        }
+        size_t used = 0;
+        while (*n < capacity && *n < (int)updates_.size() && used + count(updates_[*n]) <= row_capacity) used += count(updates_[(*n)++]);
+        if (used) std::memcpy(rows, map_rows_.data() + map_head_, used * sizeof(ygzb_map_point));
+        std::copy(updates_.begin(), updates_.begin() + *n, out);
+        updates_.erase(updates_.begin(), updates_.begin() + *n);
+        map_head_ += used;
+        if (map_head_ == map_rows_.size()) {   // (one buffer keeps its capacity across rounds, as the observation rows')
+            map_rows_.clear();
+            map_head_ = 0;
+        } else if (map_head_ > map_rows_.size() / 2) {
+            map_rows_.erase(map_rows_.begin(), map_rows_.begin() + (ptrdiff_t)map_head_);
+            map_head_ = 0;
+        }
+        *n_rows = used;
+        return YGZB_OK;
+    }
     // the rows of the k oldest results have been polled: one buffer keeps its capacity across rounds, so a round neither
     // allocates nor touches fresh pages once it has grown
     void drop_rows(size_t k) {
@@ -776,6 +810,32 @@ class Engine {
             return rc;
         }
         h_info_ = static_cast<ygzb_pose_information*>(p);
+        return YGZB_OK;
+    }
+    // on: every key-frame insertion from here on queues its map update (the tracker writes each key-frame job's rows into a
+    // page-locked buffer, allocated here: n_streams * YGZB_TRACK_RING * cells rows); off: none, and the buffer is freed.
+    // Call only when idle()
+    int set_map_updates(bool on) {
+        if (on == map_updates()) return YGZB_OK;
+        if (!on) {
+            CHK(ygzb_tracker_set_map_updates(tr_, nullptr, 0));
+            CHK(ygzb_synchronize(ctx_));
+            ygzb_host_free(h_map_);
+            h_map_ = nullptr;
+            return YGZB_OK;
+        }
+        int rows = 0, cols = 0;
+        CHK(ygzb_grid_dims(ctx_, &rows, &cols));
+        map_stride_ = (size_t)YGZB_TRACK_RING * rows * cols;
+        const size_t cap = (size_t)S_ * map_stride_;
+        void* p = nullptr;
+        CHK(ygzb_host_alloc(&p, cap * sizeof(ygzb_map_point)));
+        const int rc = ygzb_tracker_set_map_updates(tr_, static_cast<ygzb_map_point*>(p), cap);
+        if (rc != YGZB_OK) {
+            ygzb_host_free(p);
+            return rc;
+        }
+        h_map_ = static_cast<ygzb_map_point*>(p);
         return YGZB_OK;
     }
 
@@ -899,6 +959,7 @@ class Engine {
             }
             emit(kj.stream, kframes_[q].frame, kframes_[q].tag, YGZ_VO_KEYFRAME, kframes_[q].n_inliers, kf_rows_.data() + kframes_[q].obs0,
                  kframes_[q].n_obs, &kframes_[q].info);
+            if (map_updates()) queue_map_update(kj, r, h_map_ + q * map_stride_);
         }
         kjobs_.clear();
         kframes_.clear();
@@ -1007,6 +1068,25 @@ class Engine {
         for (int t = 0; t < w; ++t) CHK(ygzb_tracker_upload(tr_, i * F_ + t, 1, q[t].image, fb));
         return YGZB_OK;
     }
+    // the map update of key-frame job kj, whose result r and rows (r.ba_points moved, then r.n_features new) have just come
+    // back: the rows are copied here, since the next round's insertions reuse the buffer.  Step 3 has applied r to the
+    // stream's key-frames, so the last kj.n_local of them are the local ones after the insertion
+    void queue_map_update(const ygzb_keyframe_job& kj, const ygzb_keyframe_result& r, const ygzb_map_point* rows) {
+        const EStream& s = st_[kj.stream];
+        ygz_vo_map_update u{};
+        u.stream = order_[kj.stream];
+        u.frame = s.kfs.back().frame_id;
+        u.sequence = s.n_restarts;
+        u.n_local = kj.n_local;
+        const size_t first = s.kfs.size() - (size_t)kj.n_local;
+        u.retired_frame = first > 0 ? s.kfs[first - 1].frame_id : -1;   // (the ring keeps the key-frame that has just left)
+        for (int k = 0; k < YGZB_TRACK_RING; ++k) u.local_frame[k] = k < kj.n_local ? s.kfs[first + k].frame_id : -1;
+        for (int k = 0; k < kj.n_local; ++k) std::memcpy(u.T_cw[k], r.T_cw[k], sizeof(u.T_cw[k]));
+        u.n_moved = r.ba_points;
+        u.n_new = r.n_features;
+        map_rows_.insert(map_rows_.end(), rows, rows + (size_t)u.n_moved + (size_t)u.n_new);
+        updates_.push_back(u);
+    }
     // observation rows of job j of the tracking batch that has just come back (observations on), else NULL
     const ygzb_observation* job_rows(int j) const { return h_obs_ ? h_obs_ + (size_t)j * obs_stride_ : nullptr; }
     // information record of job j of the tracking batch that has just come back (information on), else NULL
@@ -1109,6 +1189,13 @@ class Engine {
     // information (set_information): the tracker's page-locked records, one per job; the records of the results in results_
     ygzb_pose_information* h_info_ = nullptr;
     std::deque<ygzb_pose_information> info_;
+    // map updates (set_map_updates): the tracker's page-locked rows, map_stride_ rows per key-frame job; the updates waiting
+    // to be polled, their rows back to back from map_head_
+    ygzb_map_point* h_map_ = nullptr;
+    size_t map_stride_ = 0;
+    std::deque<ygz_vo_map_update> updates_;
+    std::vector<ygzb_map_point> map_rows_;
+    size_t map_head_ = 0;
     bool blocking_sync_ = false;
 };
 
@@ -1749,6 +1836,18 @@ int ygz_vo_poll_ex(ygz_vo* vo, ygz_vo_result* out, int capacity, int* n, ygzb_po
     if (e.observations() ? (!n_obs || (obs_capacity > 0 && !obs)) : (obs || obs_capacity > 0)) return YGZB_ERR_INVALID;
     if (!e.observations() && n_obs) *n_obs = 0;
     return e.pop_results(out, capacity, n, info, obs, obs_capacity, n_obs);
+}
+
+int ygz_vo_set_map_updates(ygz_vo* vo, int on) {
+    if (!vo || !vo->eng->idle()) return YGZB_ERR_INVALID;
+    return vo->eng->set_map_updates(on != 0);
+}
+
+int ygz_vo_poll_map_updates(ygz_vo* vo, ygz_vo_map_update* out, int capacity, int* n, ygzb_map_point* rows, size_t row_capacity,
+                            size_t* n_rows) {
+    if (!vo || !n || !n_rows || capacity < 0 || (capacity > 0 && !out) || (row_capacity > 0 && !rows) || !vo->eng->map_updates())
+        return YGZB_ERR_INVALID;
+    return vo->eng->pop_map_updates(out, capacity, n, rows, row_capacity, n_rows);
 }
 
 int ygz_vo_stream_stats(ygz_vo* vo, int stream, int64_t stats[16]) {

@@ -8,7 +8,7 @@ from pathlib import Path
 import numpy as np
 
 from . import build
-from .capi import INFO_DTYPE, unpack_sym6
+from .capi import INFO_DTYPE, MAP_POINT_DTYPE, unpack_sym6
 
 _LIB = None
 
@@ -45,6 +45,8 @@ def _lib():
         _LIB.ygz_vo_poll_observations.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
         _LIB.ygz_vo_set_information.argtypes = [C.c_void_p, C.c_int]
         _LIB.ygz_vo_poll_ex.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+        _LIB.ygz_vo_set_map_updates.argtypes = [C.c_void_p, C.c_int]
+        _LIB.ygz_vo_poll_map_updates.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
         _LIB.ygz_vo_stream_stats.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         _LIB.ygz_vo_export_map.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         _LIB.ygz_vo_stream_record_bound.argtypes = [C.c_void_p, C.c_void_p]
@@ -150,6 +152,9 @@ STATUS = ("tracked", "keyframe", "lost")   # YGZ_VO_TRACKED / _KEYFRAME / _LOST
 RESULT_DTYPE = np.dtype([("stream", np.int32), ("frame", np.int32), ("tag", np.int64), ("status", np.int32), ("n_inliers", np.int32),
                          ("T_cw", np.float64, (12,))])   # ygz_vo_result
 OBS_DTYPE = np.dtype([("id", np.int64), ("px", np.float64, (2,)), ("pw", np.float64, (3,))])   # ygzb_observation
+MAP_UPDATE_DTYPE = np.dtype([("stream", np.int32), ("frame", np.int32), ("sequence", np.int64), ("n_local", np.int32),
+                             ("retired_frame", np.int32), ("local_frame", np.int32, (4,)), ("n_moved", np.int32), ("n_new", np.int32),
+                             ("T_cw", np.float64, (4, 12))])   # ygz_vo_map_update
 _ERR_CAPACITY = -4   # YGZB_ERR_CAPACITY
 
 
@@ -226,10 +231,11 @@ class Engine:
     observations=True: every result carries the map points its pose rests on (ygz_vo_set_observations), and poll
     returns them too.  information=True: every result carries how well its pose is determined (ygz_vo_set_information):
     poll also returns an [n, 2, 6, 6] array, the sparse alignment's Fisher information and pose-only's information
-    matrix of each result as full symmetric matrices."""
+    matrix of each result as full symmetric matrices.  map_updates=True: every key-frame insertion queues what it changed
+    in the local map (ygz_vo_set_map_updates), which poll_map_updates returns."""
 
     def __init__(self, ctx, n_streams, window=8, ref_mode="keyframe", kf_min_frames=10, kf_min_rot=0.1, kf_min_trans=0.1,
-                 min_inliers=30, K=None, observations=False, information=False):
+                 min_inliers=30, K=None, observations=False, information=False, map_updates=False):
         if ref_mode not in _REF_MODES:
             raise ValueError(f"ref_mode must be 'keyframe' or 'previous', not {ref_mode!r}")
         p = ctx.params
@@ -250,6 +256,10 @@ class Engine:
         self.information = False
         if information:
             self.set_information(True)
+        self.map_updates = False
+        self._map_rows = np.zeros(0, MAP_POINT_DTYPE)   # rows of one ygz_vo_poll_map_updates call, grown on demand
+        if map_updates:
+            self.set_map_updates(True)
 
     def set_observations(self, on):
         """Switch the observation rows of the results on or off (ygz_vo_set_observations): only while the engine is
@@ -262,6 +272,37 @@ class Engine:
         idle, as set_observations."""
         self.ctx.check(self.lib.ygz_vo_set_information(self.h, int(bool(on))), "ygz_vo_set_information")
         self.information = bool(on)
+
+    def set_map_updates(self, on):
+        """Switch the map updates of key-frame insertions on or off (ygz_vo_set_map_updates): only while the engine is
+        idle, as set_observations, with no update waiting either."""
+        self.ctx.check(self.lib.ygz_vo_set_map_updates(self.h, int(bool(on))), "ygz_vo_set_map_updates")
+        self.map_updates = bool(on)
+
+    def poll_map_updates(self, capacity=256):
+        """Map updates since the last call, oldest first: (updates, rows) -- a MAP_UPDATE_DTYPE array and, per update, a
+        MAP_POINT_DTYPE array of its n_moved rows (the local BA's points) followed by its n_new rows (the new key-frame's
+        points).  Independent of poll: results and updates have queues of their own."""
+        out, rows = [], []
+        if len(self._map_rows) == 0:
+            self._map_rows = np.zeros(4 * 4096, MAP_POINT_DTYPE)
+        while True:
+            buf = np.zeros(capacity, MAP_UPDATE_DTYPE)
+            n, n_rows = C.c_int(0), C.c_size_t(0)
+            rc = self.lib.ygz_vo_poll_map_updates(self.h, buf.ctypes.data, capacity, C.byref(n), self._map_rows.ctypes.data,
+                                                  len(self._map_rows), C.byref(n_rows))
+            if rc == _ERR_CAPACITY:   # the next update's rows do not fit: grow the row buffer and ask again
+                self._map_rows = np.zeros(max(2 * len(self._map_rows), n_rows.value), MAP_POINT_DTYPE)
+                continue
+            self.ctx.check(rc, "ygz_vo_poll_map_updates")
+            if n.value == 0:
+                break
+            upd = buf[:n.value]
+            ends = np.cumsum(upd["n_moved"].astype(np.int64) + upd["n_new"])
+            assert ends[-1] == n_rows.value
+            out.append(upd)
+            rows.extend(np.split(self._map_rows[:n_rows.value].copy(), ends[:-1]))
+        return (np.concatenate(out) if out else np.zeros(0, MAP_UPDATE_DTYPE)), rows
 
     def push(self, stream, image, depth=None, tag=None):
         """Queue grey `image` (H, W) uint8 of `stream` with its depth map (H, W) float64, or None to keep the stream's current
