@@ -476,6 +476,17 @@ int ygzb_tracker_get_depth(ygzb_tracker* t, int stream, double* out);
  * enqueued.  YGZB_ERR_INVALID, with the tracker untouched, for a NULL tracker or pose, a stream out of range, an entry
  * that is not finite, or a rotation that is not orthonormal with determinant +1 (within 1e-6 per entry).           */
 int ygzb_tracker_set_start_pose(ygzb_tracker* t, int stream, const double T_cw[12]);
+/* K = {fx, fy, cx, cy} of `stream` for every job and key-frame insertion enqueued after the call; streams of one tracker
+ * may have different cameras and still share every launch.  Every stream starts with ygzb_tracker_create's K.  A stream
+ * with camera K computes what a one-camera tracker created with K on a context whose float fx..cy are (float)K computes:
+ * candidate projection and map points use K, the solvers (sparse alignment, pose-only, local BA) (float)K.  Until its
+ * first call a stream's solvers use the context's fx..cy, as before.  Map and reference records carry the stream's K
+ * (ygzb_tracker_export, _import).  The camera is not checked against the frames: a caller changes it between sequences.
+ * The new camera is enqueued like an upload (ygzb_tracker_upload): it waits for the jobs and key-frame insertions
+ * enqueued before, not for a local BA still in flight, so the next batch's alignment still overlaps that BA.
+ * YGZB_ERR_INVALID, with the tracker untouched, for a NULL tracker or K, a stream out of range, an entry that is not
+ * finite, or fx <= 0 or fy <= 0.                                                                                    */
+int ygzb_tracker_set_camera(ygzb_tracker* t, int stream, const double K[4]);
 /* host -> device copy of `count` grey frames into slots [first, first+count) and their pyramids, like ygzb_frames_upload,
  * but on the tracker's second CUDA stream: behind the last key-frame insertion and tracking chain (which still read the
  * slots), concurrent with a local BA in flight.  ygzb_tracker_track orders itself behind these uploads.              */
@@ -565,7 +576,7 @@ int ygzb_tracker_set_map_updates(ygzb_tracker* t, ygzb_map_point* host, size_t c
 #define YGZB_MAP_OBS_PER_CELL 4   /* observation capacity of a key-frame per grid cell */
 typedef struct {
     int32_t width, height, cells, n_levels;   /* image size, grid cells, pyramid levels                             */
-    double K[4];                              /* fx, fy, cx, cy of the tracker (ygzb_tracker_create)                */
+    double K[4];                              /* fx, fy, cx, cy of the stream (ygzb_tracker_set_camera)             */
     int32_t n_keyframes, pad;
     int32_t* entry;        /* [n_keyframes] ring entry the key-frame was exported from                                */
     double* T_cw;          /* [n_keyframes][12]                                                                      */

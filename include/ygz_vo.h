@@ -50,7 +50,8 @@ typedef struct {
     int kf_min_frames;      /* NeedNewKeyFrame (VisualOdometry.cpp:304-321): frames since the last key-frame ...       */
     double kf_min_rot, kf_min_trans;   /* ... and the rotation (rad) or translation (m) from it that make a key-frame */
     int min_inliers;        /* pose-only inliers below which a stream is lost (vo.keyframe.min_features, 30)         */
-    double K[4];            /* fx, fy, cx, cy in double; must round to the context's float fx..cy                   */
+    double K[4];            /* fx, fy, cx, cy in double; must round to the context's float fx..cy; the camera of
+                               every stream until ygz_vo_set_camera gives it another                                 */
 } ygz_vo_config;
 
 #define YGZ_VO_TRACKED 0
@@ -87,6 +88,30 @@ int ygz_vo_push(ygz_vo* vo, int stream, const uint8_t* image, const double* dept
  * The engine never restarts a stream by itself.  YGZB_ERR_INVALID, changing nothing, for a NULL vo, a stream out of
  * range, a non-finite entry, or a rotation that is not orthonormal with determinant +1 (within 1e-6 per entry).      */
 int ygz_vo_restart(ygz_vo* vo, int stream, const double T_cw[12]);
+/* K = {fx, fy, cx, cy} of `stream`'s next sequence, so that the streams of one engine may come from different cameras
+ * (undistorted, with the context's image size).  A camera belongs to a sequence:
+ *  - Accepted before the stream's first push, or while a restart is pending (ygz_vo_restart called, nothing pushed
+ *    since).  Of two calls with no push in between, the last one counts.
+ *  - Barrier: frames pushed before ygz_vo_restart are tracked with the old camera, whatever is set afterwards; the new
+ *    camera applies from the new sequence's first key-frame.
+ *  - A stream with camera K gives the results, observation rows (in its own pixel frame), information records and map
+ *    updates of a one-stream engine created with K on a context whose float fx..cy are (float)K.  K need not round to
+ *    the context's camera.
+ *  - ygz_vo_export_map carries the camera of the key-frames it holds (that of the stream's current sequence).  Stream
+ *    records carry the stream's camera (the one its next push uses) in their header K, and ygz_vo_load_stream accepts a
+ *    record only if that K equals the destination stream's camera bit for bit: to hand a stream with another camera
+ *    over into a stream that has tracked, call ygz_vo_flush, ygz_vo_restart(stream) (a restart is then pending),
+ *    ygz_vo_set_camera, then ygz_vo_load_stream.  The load replaces the whole state, the pending restart included; if it
+ *    fails, the stream keeps the camera that was set and the restart stays pending.  A stream saved while a restart is
+ *    pending after ygz_vo_set_camera carries the new camera, while its ring still holds the old sequence's key-frames;
+ *    the loaded stream's ygz_vo_export_map reports them with the new camera until its next push restarts it (they are
+ *    never tracked again).
+ * YGZB_ERR_INVALID, changing nothing, for a NULL vo or K, a stream out of range, an entry that is not finite, fx <= 0 or
+ * fy <= 0, or a call at any other time (the stream has pushed frames and no restart is pending).                 */
+int ygz_vo_set_camera(ygz_vo* vo, int stream, const double K[4]);
+/* the camera ygz_vo_set_camera last gave `stream` (the config's K until then): that of its current sequence, or of the
+ * next one while a restart is pending.  YGZB_ERR_INVALID for a NULL vo or K or a stream out of range.               */
+int ygz_vo_get_camera(const ygz_vo* vo, int stream, double K[4]);
 /* one round over what is queued, with one host synchronisation: the results of the windows it tracks are final on
  * return, except a frame that triggers a key-frame, whose insertion is enqueued by the next round.                 */
 int ygz_vo_step(ygz_vo* vo);
@@ -181,7 +206,8 @@ int ygz_vo_poll_map_updates(ygz_vo* vo, ygz_vo_map_update* out, int capacity, in
  * 0, 0, 0                                                                                                         */
 int ygz_vo_stream_stats(ygz_vo* vo, int stream, int64_t stats[16]);
 /* the local map of `stream` (every key-frame still in its ring, oldest first) into `out`, sized for YGZB_TRACK_RING
- * key-frames (ygzb_tracker_export): asynchronous, valid after ygzb_synchronize(ctx); call after ygz_vo_flush         */
+ * key-frames (ygzb_tracker_export), with the stream's camera in out->K (ygz_vo_set_camera): asynchronous, valid after
+ * ygzb_synchronize(ctx); call after ygz_vo_flush                                                                   */
 int ygz_vo_export_map(ygz_vo* vo, int stream, ygzb_map_record* out);
 
 /* ---- stream records: a live stream as plain bytes, to move it to another engine, context, device or process ----------
@@ -191,7 +217,7 @@ int ygz_vo_export_map(ygz_vo* vo, int stream, ygzb_map_record* out);
  *
  * Layout: little-endian, packed (no padding; fields are not aligned), every count before the rows it describes.
  *   1. header      u8 magic[4] = "YGZS", u32 version = 1, u64 size (of the whole record),
- *                  i32 width, height, cells, n_levels, f64 K[4], i32 ref_mode                                 (68 bytes)
+ *                  i32 width, height, cells, n_levels, f64 K[4] (the stream's camera), i32 ref_mode           (68 bytes)
  *   2. host state  i32 n_kf, then per key-frame of the stream's ring, oldest first:
  *                      i32 entry, i32 n, i32 frame_id, i64 mp0, f64 T_cw[12]                               (116 bytes)
  *                  f64 T_cw[12] (current pose), f64 start[12] (pose of the next sequence's first key-frame),
@@ -224,7 +250,8 @@ int ygz_vo_save_stream(ygz_vo* vo, int stream, void* buf, size_t capacity, size_
  *    the result queue stay there for ygz_vo_poll.
  *  - The engine may differ from the saved one in n_streams, window, key-frame policy and min_inliers (the destination's
  *    apply from here on), in the stream index and in its context and device.  It must match it in image size, grid
- *    cells, pyramid levels, K (bit for bit) and ref_mode.
+ *    cells, pyramid levels and ref_mode, and the destination stream's camera (ygz_vo_get_camera) must equal the
+ *    record's K bit for bit.
  *  - The record is checked whole on the host before anything is enqueued.
  * Asynchronous like ygzb_tracker_import; `buf` may be released when the call returns.  YGZB_ERR_INVALID, with the
  * stream exactly as before, for a NULL vo or buf, a stream out of range or with queued frames or a pending insertion,

@@ -46,7 +46,7 @@ EXPORTS = [
     "ygzb_tracker_export", "ygzb_tracker_import", "ygzb_tracker_debug_job", "ygzb_tracker_set_reference_mode", "ygzb_tracker_debug_reference",
     "ygzb_tracker_export_reference", "ygzb_tracker_import_reference", "ygzb_undistort_map", "ygzb_frames_set_undistort",
     "ygzb_tracker_set_start_pose", "ygzb_tracker_get_depth", "ygzb_tracker_set_observations",
-    "ygzb_sparse_align_fisher", "ygzb_tracker_set_information", "ygzb_tracker_set_map_updates",
+    "ygzb_sparse_align_fisher", "ygzb_tracker_set_information", "ygzb_tracker_set_map_updates", "ygzb_tracker_set_camera",
 ]
 
 
@@ -886,6 +886,7 @@ class Tracker:
         self.lib.ygzb_tracker_set_depth.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         self.lib.ygzb_tracker_get_depth.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         self.lib.ygzb_tracker_set_start_pose.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        self.lib.ygzb_tracker_set_camera.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         self.lib.ygzb_tracker_upload.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
         self.lib.ygzb_tracker_track.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         self.lib.ygzb_tracker_make_keyframes.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -974,6 +975,11 @@ class Tracker:
         """T_cw (3, 4) that `stream`'s next first key-frame (a key-frame job with track_job = -1) takes; identity by default."""
         T = np.ascontiguousarray(T_cw, np.float64).reshape(12)
         self.ctx.check(self.lib.ygzb_tracker_set_start_pose(self.h, int(stream), _p(T)), "ygzb_tracker_set_start_pose")
+
+    def set_camera(self, stream: int, K):
+        """K = (fx, fy, cx, cy) of `stream` for every later job and key-frame insertion (ygzb_tracker_set_camera)."""
+        K = np.ascontiguousarray(K, np.float64).reshape(4)
+        self.ctx.check(self.lib.ygzb_tracker_set_camera(self.h, int(stream), _p(K)), "ygzb_tracker_set_camera")
 
     def upload(self, first: int, images):
         """Grey frames (n, H, W) into slots [first, first + n)."""

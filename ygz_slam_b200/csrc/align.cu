@@ -355,6 +355,7 @@ struct SparseArgs {
     void* feat_scratch;         // global fall-back of the per-feature staging, feat_stride bytes per problem
     size_t feat_stride;
     double* H_out;              // [n_problems][21] or null: H of the last linearisation at min_level (zeroed before the launch)
+    const float* cam_p;         // optional [n_problems][4]: fx, fy, cx, cy of each problem (default: cam)
 };
 
 // ---- SparseImgAlign (ygzb_sparse_align and the tracking engine's batches) ----------------------------------------------
@@ -435,6 +436,7 @@ __global__ void __launch_bounds__(kSA2Threads) sparse_align2_kernel(const Sparse
     __shared__ int s_flag;
     __shared__ double s_chi2;
     __shared__ unsigned long long s_last_nmeas;
+    __shared__ CamF s_cam;
 
     const int rank = (int)cluster.block_rank(), C = (int)cluster.num_blocks();
     const int prob = blockIdx.x / C, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -457,12 +459,14 @@ __global__ void __launch_bounds__(kSA2Threads) sparse_align2_kernel(const Sparse
         s_T = se3_mul(se3_from_mat(a.T_cur + 12 * (size_t)prob), se3_inverse(Tref));
         s_chi2 = 1e10;
         s_last_nmeas = 0;
+        s_cam = a.cam_p ? CamF{a.cam_p[4 * prob], a.cam_p[4 * prob + 1], a.cam_p[4 * prob + 2], a.cam_p[4 * prob + 3]} : a.cam;
     }
+    __syncthreads();
     for (int j = tid; j < nl; j += kSA2Threads) {
         SA2Feat& ft = F[j];
         const long gi = f0 + j_lo + j + din;
         ft.state = 0;
-        const V3d xyz = pixel2camera(a.cam, a.px[2 * gi], a.px[2 * gi + 1], a.depth[gi]);
+        const V3d xyz = pixel2camera(s_cam, a.px[2 * gi], a.px[2 * gi + 1], a.depth[gi]);
         ft.xyz[0] = xyz.x; ft.xyz[1] = xyz.y; ft.xyz[2] = xyz.z;
         for (int k = 0; k < 16; ++k) ft.patch[k] = 0.f;   // (the reference's patch cache starts out zero-filled)
     }
@@ -473,7 +477,7 @@ __global__ void __launch_bounds__(kSA2Threads) sparse_align2_kernel(const Sparse
         const LevelImg rim = level_img(a.pyr, a.slot_stride, a.ref_slot[prob], g, lvl);
         const LevelImg cim = level_img(a.pyr, a.slot_stride, a.cur_slot[prob], g, lvl);
         const float scale = 1.0f / (float)(1 << lvl);
-        const double focal = (double)(float)((a.cam.fx + a.cam.fy) / 2);  // PinholeCamera::_f is a float
+        const double focal = (double)(float)((s_cam.fx + s_cam.fy) / 2);  // PinholeCamera::_f is a float
         const double jscale = focal / (1 << lvl);
         // precomputeReferencePatches (features that are not cached at this level keep their stale patch with a zero Jacobian)
         for (int j = tid; j < nl; j += kSA2Threads) {
@@ -529,7 +533,7 @@ __global__ void __launch_bounds__(kSA2Threads) sparse_align2_kernel(const Sparse
                 const double y = s_Tm[4] * ft.xyz[0] + s_Tm[5] * ft.xyz[1] + s_Tm[6] * ft.xyz[2] + s_Tm[7];
                 const double z = s_Tm[8] * ft.xyz[0] + s_Tm[9] * ft.xyz[1] + s_Tm[10] * ft.xyz[2] + s_Tm[11];
                 double pu, pv;
-                camera2pixel(a.cam, V3d{x, y, z}, &pu, &pv);
+                camera2pixel(s_cam, V3d{x, y, z}, &pu, &pv);
                 const float u_cur = (float)pu * scale, v_cur = (float)pv * scale;
                 const int ui = (int)floorf(u_cur), vi = (int)floorf(v_cur);
                 if (ui < 0 || vi < 0 || ui - 3 < 0 || vi - 3 < 0 || ui + 3 >= cim.w || vi + 3 >= cim.h) continue;
@@ -667,6 +671,7 @@ __global__ void track_prep_kernel(TrackStore st, TrackBatch b) {
     if (j >= b.J) return;
     const ygzb_track_job job = b.jobs[j];
     b.cur_slot[j] = job.cur_slot;
+    for (int c = 0; c < 4; ++c) b.cam[4 * (size_t)j + c] = st.cam_F[4 * job.stream + c];
     b.n_cand[j] = 0;
     b.c_off[j] = j * b.cap;
     if (j == 0) b.c_off[b.J] = b.J * b.cap;
@@ -732,9 +737,9 @@ __global__ void track_motion_kernel(TrackStore st, TrackBatch b) {
 }
 
 // LocalMapping::FindCandidates (LocalMapping.cpp:47-80) + Matcher::FindDirectProjection (:82-111) for dense candidate
-// c = local key-frame k * cells + feature g of job blockIdx.y
-__global__ void __launch_bounds__(128) track_project_kernel(const uint8_t* __restrict__ pyr, size_t slot_stride, Geometry g, CamF cam,
-                                                            TrackStore st, TrackBatch b) {
+// c = local key-frame k * cells + feature g of job blockIdx.y, with the camera of the job's stream
+__global__ void __launch_bounds__(128) track_project_kernel(const uint8_t* __restrict__ pyr, size_t slot_stride, Geometry g, TrackStore st,
+                                                            TrackBatch b) {
     const int j = blockIdx.y, c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= b.cap) return;
     const size_t at = (size_t)j * b.cap + c;
@@ -750,10 +755,13 @@ __global__ void __launch_bounds__(128) track_project_kernel(const uint8_t* __res
     const double x = T[0] * X[0] + T[1] * X[1] + T[2] * X[2] + T[3];
     const double y = T[4] * X[0] + T[5] * X[1] + T[6] * X[2] + T[7];
     const double z = T[8] * X[0] + T[9] * X[1] + T[10] * X[2] + T[11];
-    double u = st.fx * x / z + st.cx, v = st.fy * y / z + st.cy;
+    const double* K = st.cam_K + 4 * job.stream;
+    double u = K[0] * x / z + K[2], v = K[1] * y / z + K[3];
     if (!(z > 0 && u >= 20 && u < st.W - 20 && v >= 20 && v < st.H - 20)) return;
     atomicAdd(&b.n_cand[j], 1);
     const double eye[12] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0};
+    const float* cf = b.cam + 4 * (size_t)j;
+    const CamF cam{cf[0], cf[1], cf[2], cf[3]};
     uint8_t sl;
     const size_t fe = (size_t)e * st.cells + f;
     const bool ok = find_direct_projection_dev(pyr, slot_stride, g, cam, st.kf_slot[e], job.cur_slot, eye,
@@ -904,6 +912,7 @@ int launch_sparse_align(ygzb_frames* f, int n_problems, const int32_t* d_ref_slo
     a.slot_stride = ctx->slot_stride;
     a.g = ctx->geo;
     a.cam = CamF{ctx->prm.fx, ctx->prm.fy, ctx->prm.cx, ctx->prm.cy};
+    a.cam_p = nullptr;
     a.ref_slot = d_ref_slot;
     a.cur_slot = d_cur_slot;
     a.offsets = d_offsets;
@@ -942,6 +951,7 @@ int launch_track_chain_front(ygzb_frames* f, const TrackStore& st, const TrackBa
     a.slot_stride = ctx->slot_stride;
     a.g = ctx->geo;
     a.cam = CamF{ctx->prm.fx, ctx->prm.fy, ctx->prm.cx, ctx->prm.cy};
+    a.cam_p = b.cam;               // the camera of each job's stream
     a.ref_slot = b.ref_slot;
     a.cur_slot = b.cur_slot;
     a.offsets = b.offsets;
@@ -980,10 +990,9 @@ int launch_track_chain_mid(ygzb_frames* f, const TrackStore& st, const TrackBatc
         YGZB_LAUNCHED(ctx);
     }
     {
-        const CamF cam{ctx->prm.fx, ctx->prm.fy, ctx->prm.cx, ctx->prm.cy};
         ProfScope ps(ctx, kStageProjectAlign);
         track_project_kernel<<<dim3((unsigned)((b.cap + 127) / 128), (unsigned)b.J), 128, 0, ctx->stream>>>(f->d_pyr, ctx->slot_stride, ctx->geo,
-                                                                                                          cam, st, b);
+                                                                                                          st, b);
         YGZB_LAUNCHED(ctx);
     }
     {

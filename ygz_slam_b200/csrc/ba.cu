@@ -798,6 +798,7 @@ struct PoseOnlyArgs {
     uint8_t* enable;          // scratch [total]
     double* ws;               // (unused since the partial sums travel through distributed shared memory; kept for the scratch layout)
     float fx, fy, cx, cy;
+    const float* cam;         // optional [n_problems][4]: fx, fy, cx, cy of each problem (default: fx..cy above)
     int stage_k;              // points per thread the dynamic shared memory can stage (0: read the points from global memory)
 };
 
@@ -856,11 +857,14 @@ __global__ void __launch_bounds__(kPoseThreads) pose_only_kernel(const PoseOnlyA
     __shared__ double s_pub[4][kPoseRed];                    // this CTA's partial sums of the last four reductions (read by the peers)
     __shared__ double s_pose[6], s_cand[6], s_scale[6], s_sum[kPoseRed];
     __shared__ double s_R[9], s_dR[27], s_Rpose[6];          // rotation (row major), dR[3 * (3 j + k) + m] = d R_jk / d aa_m, and their pose
+    __shared__ float s_cam[4];                               // the problem's fx, fy, cx, cy
     const int rank = (int)cluster.block_rank(), C = (int)cluster.num_blocks();
     const int prob = blockIdx.x / C, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int CT = C * kPoseThreads, ct = rank * kPoseThreads + tid;   // cluster-wide thread id
     const int i0 = a.offsets[prob], n = a.counts ? a.counts[prob] : a.offsets[prob + 1] - i0;
-    const double fx = a.fx, fy = a.fy, cx = a.cx, cy = a.cy;
+    if (tid < 4) s_cam[tid] = a.cam ? a.cam[4 * (size_t)prob + tid] : tid == 0 ? a.fx : tid == 1 ? a.fy : tid == 2 ? a.cx : a.cy;
+    __syncthreads();
+    const double fx = s_cam[0], fy = s_cam[1], cx = s_cam[2], cy = s_cam[3];
     const int K = (n + CT - 1) / CT;                         // points per thread: i = ct + k * CT
     const bool staged = K <= a.stage_k && K <= 32;
     unsigned en_mask = 0;                                    // (staged) enable flag of this thread's k-th point
@@ -1145,7 +1149,8 @@ __global__ void __launch_bounds__(kPoseThreads) pose_only_kernel(const PoseOnlyA
 size_t pose_only_ws_doubles(int n_problems) { return (size_t)n_problems * 4 * kPoseCluster * kPoseRed; }
 
 // ba::OptimizeCurrentPoseOnly on device-resident problems (the tracking engine): problem p owns points
-// [d_offsets[p], d_offsets[p] + d_counts[p]); cluster = CTAs per problem (1, 2, 4 or 8)
+// [d_offsets[p], d_offsets[p] + d_counts[p]); cluster = CTAs per problem (1, 2, 4 or 8); d_cam: [n_problems][4] float
+// fx, fy, cx, cy of every problem, or null for the context's camera
 // points per thread the kernel may stage in shared memory for problems of at most max_points points on `cluster` CTAs
 // (0 = more than fits: the kernel then reads the points from global memory); sets the kernel's shared-memory opt-in once
 static int pose_only_stage_k(int max_points, int cluster) {
@@ -1165,12 +1170,13 @@ static int pose_only_stage_k(int max_points, int cluster) {
 
 int launch_pose_only_dev(ygzb_ctx* ctx, int n_problems, const int32_t* d_offsets, const int32_t* d_counts, const double* d_pw,
                          const double* d_px, double* d_T_cw, uint8_t* d_inlier, double* d_depth, int32_t* d_n_inlier, uint8_t* d_enable,
-                         double* d_ws, int cluster, int max_points) {
+                         double* d_ws, int cluster, int max_points, const float* d_cam) {
     if (n_problems <= 0) return YGZB_OK;
     PoseOnlyArgs a;
     a.offsets = d_offsets; a.counts = d_counts; a.pw = d_pw; a.px = d_px; a.T_cw = d_T_cw; a.inlier = d_inlier; a.depth = d_depth;
     a.n_inlier = d_n_inlier; a.enable = d_enable; a.ws = d_ws;
     a.fx = ctx->prm.fx; a.fy = ctx->prm.fy; a.cx = ctx->prm.cx; a.cy = ctx->prm.cy;
+    a.cam = d_cam;
     cluster = std::max(1, std::min(cluster, kPoseCluster));
     a.stage_k = pose_only_stage_k(max_points, cluster);
     ProfScope ps(ctx, kStagePoseOnly);
@@ -1679,7 +1685,7 @@ int ygzb_pose_only(ygzb_ctx* ctx, int n_problems, const int32_t* offsets, const 
     int max_points = 0;
     for (size_t q = 0; q < P; ++q) max_points = std::max(max_points, offsets[q + 1] - offsets[q]);
     TRY(launch_pose_only_dev(ctx, n_problems, d_off, nullptr, d_pw, d_px, d_T_cw, d_inlier, d_depth, d_n_inlier, d_enable, d_ws, kPoseCluster,
-                             max_points));
+                             max_points, nullptr));
     TRY(d2h(ctx, T_cw, d_T_cw, 12 * P));
     TRY(d2h(ctx, inlier, d_inlier, N));
     TRY(d2h(ctx, depth, d_depth, N));

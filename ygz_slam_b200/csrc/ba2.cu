@@ -479,10 +479,11 @@ __global__ void __launch_bounds__(kT) local_ba2_kernel(const BA2Args a) {
     __shared__ int s_gstart[kBA2MaxFree * (kBA2MaxFree + 1) / 2 + kBA2MaxFree + 1];   // first 32-lane work group of every task
 
     const int rank = (int)cluster.block_rank(), C = (int)cluster.num_blocks();
-    const int prob = blockIdx.x / C, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int prob = a.prob0 + blockIdx.x / C, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    // (read where it is used, straight from the parameter bank: held in registers it would spill the LM trial's state)
+    const auto cam = [&](int c) -> double { return a.cam[(blockIdx.x / C) % kBA2Cams][c]; };
     const int k0 = a.kf_off[prob], n_kf = a.n_kf ? a.n_kf[prob] : a.kf_off[prob + 1] - k0;
     const int p0 = a.pt_off[prob], n_pt = a.n_pt ? a.n_pt[prob] : a.pt_off[prob + 1] - p0;
-    const double fx = a.fx, fy = a.fy, cx = a.cx, cy = a.cy;
     const double dsqr = a.huber_delta * a.huber_delta;
 
     if (tid == 0) {
@@ -653,13 +654,13 @@ __global__ void __launch_bounds__(kT) local_ba2_kernel(const BA2Args a) {
                 const double y = Tm[4] * X0 + Tm[5] * X1 + Tm[6] * X2 + Tm[7];
                 const double z = Tm[8] * X0 + Tm[9] * X1 + Tm[10] * X2 + Tm[11];
                 const double iz = 1.0 / z;
-                const double e0 = st.uv[2 * (size_t)(q - q_lo)] - (x * iz * fx + cx), e1 = st.uv[2 * (size_t)(q - q_lo) + 1] - (y * iz * fy + cy);
+                const double e0 = st.uv[2 * (size_t)(q - q_lo)] - (x * iz * cam(0) + cam(2)), e1 = st.uv[2 * (size_t)(q - q_lo) + 1] - (y * iz * cam(1) + cam(3));
                 double w;
                 chi += robust(e0 * e0 + e1 * e1, &w);
                 double* rec = st.lin[buf] + 6 * (size_t)(q - q_lo);
                 rec[0] = x; rec[1] = y; rec[2] = iz; rec[3] = e0; rec[4] = e1; rec[5] = w;
                 double l0[3], l1[3];
-                point_jac(x, y, iz, fx, fy, Tm, l0, l1);
+                point_jac(x, y, iz, cam(0), cam(1), Tm, l0, l1);
                 H[0] += w * (l0[0] * l0[0] + l1[0] * l1[0]); H[1] += w * (l0[0] * l0[1] + l1[0] * l1[1]);
                 H[2] += w * (l0[0] * l0[2] + l1[0] * l1[2]); H[3] += w * (l0[1] * l0[1] + l1[1] * l1[1]);
                 H[4] += w * (l0[1] * l0[2] + l1[1] * l1[2]); H[5] += w * (l0[2] * l0[2] + l1[2] * l1[2]);
@@ -721,7 +722,7 @@ __global__ void __launch_bounds__(kT) local_ba2_kernel(const BA2Args a) {
                     const int qa = st.qa[jj];
                     const double* Di = st.Dinv + 6 * jj;
                     double H1[6][3], BD[6][3];
-                    make_hpl(lin + 6 * (size_t)(qa + s1), R1, fx, fy, H1);
+                    make_hpl(lin + 6 * (size_t)(qa + s1), R1, cam(0), cam(1), H1);
 #pragma unroll
                     for (int r = 0; r < 6; ++r) sym_mul3(Di, H1[r], BD[r]);   // (Hpl D)_r = D Hpl_r (D symmetric)
                     if (f1 == f2) {
@@ -734,7 +735,7 @@ __global__ void __launch_bounds__(kT) local_ba2_kernel(const BA2Args a) {
                             for (int c = 0; c < 6; ++c) accS[r * 6 + c] += BD[r][0] * H1[c][0] + BD[r][1] * H1[c][1] + BD[r][2] * H1[c][2];
                     } else {
                         double H2[6][3];
-                        make_hpl(lin + 6 * (size_t)(qa + s2), R2, fx, fy, H2);
+                        make_hpl(lin + 6 * (size_t)(qa + s2), R2, cam(0), cam(1), H2);
 #pragma unroll
                         for (int r = 0; r < 6; ++r)
 #pragma unroll
@@ -771,7 +772,7 @@ __global__ void __launch_bounds__(kT) local_ba2_kernel(const BA2Args a) {
                     }
                     const double* rec = lin + 6 * (size_t)(st.qa[jj] + s1);
                     double q0[6], q1[6];
-                    pose_jac(rec[0], rec[1], rec[2], fx, fy, q0, q1);
+                    pose_jac(rec[0], rec[1], rec[2], cam(0), cam(1), q0, q1);
                     const double w = rec[5];
                     int t = 0;
 #pragma unroll
@@ -962,7 +963,7 @@ __global__ void __launch_bounds__(kT) local_ba2_kernel(const BA2Args a) {
                         const int kf = st.kf[q], fi = s_free[kf];
                         if (fi < 0) continue;
                         double H1[6][3];
-                        make_hpl(st.lin[cur] + 6 * (size_t)q, s_Rlin[kf], fx, fy, H1);
+                        make_hpl(st.lin[cur] + 6 * (size_t)q, s_Rlin[kf], cam(0), cam(1), H1);
 #pragma unroll
                         for (int c = 0; c < 3; ++c)
 #pragma unroll
@@ -1194,7 +1195,6 @@ int launch_local_ba2(ygzb_ctx* ctx, const BA2Problem& in, void* scratch, const y
     a.kf_off = in.kf_off; a.pt_off = in.pt_off; a.obs_off = in.obs_off;
     a.n_kf = in.n_kf; a.n_pt = in.n_pt;
     a.poses = in.poses; a.fixed = in.fixed; a.pts = in.pts;
-    a.fx = ctx->prm.fx; a.fy = ctx->prm.fy; a.cx = ctx->prm.cx; a.cy = ctx->prm.cy;
     a.max_iters = prm->max_iters; a.max_trials = prm->max_trials; a.huber_delta = prm->huber_delta;
     a.chi2_outlier = prm->chi2_outlier; a.tau = prm->tau;
 
@@ -1228,11 +1228,21 @@ int launch_local_ba2(ygzb_ctx* ctx, const BA2Problem& in, void* scratch, const y
     const size_t dyn = std::min(cap, sys + 2 * (size_t)V + stage);
     a.dyn_doubles = (long long)dyn;
 
-    {
+    // one launch when every problem has the context's camera or all have one camera; else launches of kBA2Cams problems
+    const float ctx_cam[4] = {ctx->prm.fx, ctx->prm.fy, ctx->prm.cx, ctx->prm.cy};
+    auto cam_of = [&](size_t p) { return in.cam ? in.cam[p] : ctx_cam; };
+    bool one_cam = true;
+    for (size_t p = 1; p < P && one_cam; ++p) one_cam = std::memcmp(cam_of(p), cam_of(0), sizeof(ctx_cam)) == 0;
+    const size_t chunk = one_cam ? P : (size_t)kBA2Cams;
+    for (size_t p0 = 0; p0 < P; p0 += chunk) {
+        const size_t n = std::min(chunk, P - p0);
+        a.prob0 = (int)p0;
+        for (int k = 0; k < kBA2Cams; ++k)
+            for (int c = 0; c < 4; ++c) a.cam[k][c] = cam_of(one_cam ? 0 : p0 + std::min<size_t>(k, n - 1))[c];
         ProfScope ps(ctx, kStageLocalBA);
-        YGZB_CUDA(ctx, launch_cluster(local_ba2_kernel, (unsigned)(P * cluster), kT, cluster, dyn * sizeof(double), ctx->stream, a));
+        YGZB_CUDA(ctx, launch_cluster(local_ba2_kernel, (unsigned)(n * cluster), kT, cluster, dyn * sizeof(double), ctx->stream, a));
+        YGZB_LAUNCHED(ctx);
     }
-    YGZB_LAUNCHED(ctx);
     if (a.debug) {   // YGZB_BA_DEBUG: phase cycles of problem 0 (blocking; diagnostics only)
         double h[16];
         double hs[8];

@@ -12,6 +12,7 @@ namespace ygzb {
 constexpr int kBA2Threads = 256;
 constexpr int kBA2MaxFree = 16;    // free poses per problem: the reduced system is at most 96 x 96
 constexpr int kBA2MaxPoses = 64;
+constexpr int kBA2Cams = 32;       // cameras in the kernel's parameters: problems of one launch (fewer problems than that, or one camera)
 
 struct BA2Args {
     // problem p owns poses [kf_off[p], kf_off[p+1]), points [pt_off[p], ..), observations [obs_off[p], ..)
@@ -34,7 +35,10 @@ struct BA2Args {
     double* debug;             // optional [n_problems][8]: cycles per phase (YGZB_BA_DEBUG)
     int solver;                // 0 = 6 x 6 block LDL^T (default), 1 = scalar LDL^T (YGZB_BA_SOLVER=1, kept for comparison)
     long long dyn_doubles;     // dynamic shared memory of the launch, in doubles
-    float fx, fy, cx, cy;
+    // fx, fy, cx, cy of problem p = prob0 + blockIdx.x / cluster in cam[(p - prob0) % kBA2Cams]: a kernel parameter, so that the
+    // kernel multiplies by it straight from the constant bank (the LM trial has no registers to spare for it)
+    float cam[kBA2Cams][4];
+    int prob0;
     int max_iters, max_trials;
     double huber_delta, chi2_outlier, tau;
 };
@@ -55,6 +59,7 @@ struct BA2Problem {
     size_t total_pts, total_obs;                // sizes of the batch (bounds are fine: they size scratch)
     size_t max_pts, max_obs;                    // largest problem (bounds)
     int max_free, max_kf;
+    const float (*cam)[4];                      // HOST, optional [n_problems]: fx, fy, cx, cy of every problem (default: the context's)
 };
 
 size_t ba2_scratch_bytes(size_t total_pts, size_t total_obs, size_t n_problems);

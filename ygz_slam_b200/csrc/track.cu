@@ -68,6 +68,10 @@ struct ygzb_tracker {
     ygzb_observation* d_obs;       // device view of the caller's page-locked observation rows (ygzb_tracker_set_observations), or NULL
     ygzb_pose_information* d_info; // device view of the caller's page-locked information records (ygzb_tracker_set_information), or NULL
     ygzb_map_point* d_map;         // device view of the caller's page-locked map rows (ygzb_tracker_set_map_updates), or NULL
+    // the camera table (ygzb_tracker_set_camera): st.cam_K / st.cam_F on the device, and the host's copy of both
+    void* d_cam;
+    std::vector<double> cam_K;     // [S][4]
+    std::vector<float> cam_F;      // [S][4]
 };
 
 namespace {
@@ -167,11 +171,12 @@ __global__ void __launch_bounds__(1024) kf_fill_kernel(TrackStore st, TrackBatch
                                                       const int16_t* __restrict__ f_x, const int16_t* __restrict__ f_y,
                                                       const uint8_t* __restrict__ f_level, int n_cells, ygzb_keyframe_result* __restrict__ res) {
     __shared__ int s_scan[33];
-    __shared__ double s_T[12], s_Tin[12];
+    __shared__ double s_T[12], s_Tin[12], s_K[4];
     const ygzb_keyframe_job kj = jobs[blockIdx.x];
     const int tid = threadIdx.x, e = kj.stream * st.R + kj.entry;
     const int n = min(f_count[kj.frame_slot], st.cells);
     if (tid < 12) s_T[tid] = kj.track_job >= 0 ? b.T_cur[12 * (size_t)kj.track_job + tid] : start_T[12 * (size_t)blockIdx.x + tid];
+    if (tid >= 32 && tid < 36) s_K[tid - 32] = st.cam_K[4 * kj.stream + tid - 32];   // the camera of the key-frame's stream
     __syncthreads();
     if (tid == 0) mat34_inv(s_T, s_Tin);
     __syncthreads();
@@ -192,7 +197,8 @@ __global__ void __launch_bounds__(1024) kf_fill_kernel(TrackStore st, TrackBatch
         st.kf_px[2 * fe + 1] = y;
         st.kf_level[fe] = (uint8_t)L;
         st.kf_depth[fe] = d;
-        const double pc0 = (x - st.cx) * d / st.fx, pc1 = (y - st.cy) * d / st.fy, pc2 = d;
+        const volatile double* K = s_K;   // (read where it is used: held in registers across the loop, it spills more)
+        const double pc0 = (x - K[2]) * d / K[0], pc1 = (y - K[3]) * d / K[1], pc2 = d;
         for (int r = 0; r < 3; ++r)
             st.kf_pw[3 * fe + r] = s_Tin[4 * r] * pc0 + s_Tin[4 * r + 1] * pc1 + s_Tin[4 * r + 2] * pc2 + s_Tin[4 * r + 3];
     }
@@ -248,14 +254,15 @@ __global__ void __launch_bounds__(1024) track_obs_kernel(TrackStore st, TrackBat
 // J = d pi(exp(delta) T_cw P_w) / d delta at delta = 0 (left perturbation [upsilon; omega]) at the job's pose-only result.
 // Each thread sums the candidates it visits in candidate order, the warps and then the 32 warp sums are added in a fixed
 // order: a record depends on its job alone, not on the batch, the wave or the pacing.
-__global__ void __launch_bounds__(1024) track_info_kernel(TrackStore st, TrackBatch b, double fx, double fy,
-                                                         ygzb_pose_information* __restrict__ out) {
+__global__ void __launch_bounds__(1024) track_info_kernel(TrackStore st, TrackBatch b, ygzb_pose_information* __restrict__ out) {
     __shared__ int s_scan[33];
-    __shared__ double s_T[12];
+    __shared__ double s_T[12], s_f[2];
     __shared__ double s_red[32][21];
     const int j = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     if (tid < 12) s_T[tid] = b.T_cur[12 * (size_t)j + tid];
+    if (tid >= 32 && tid < 34) s_f[tid - 32] = b.cam[4 * (size_t)j + tid - 32];   // the float focal lengths of the job's stream
     __syncthreads();
+    const double fx = s_f[0], fy = s_f[1];
     double acc[21];
 #pragma unroll
     for (int k = 0; k < 21; ++k) acc[k] = 0.0;
@@ -368,7 +375,7 @@ TrackBatch wave_batch(const TrackBatch& b, int j0, int J) {
     w.J = J;
     w.jobs += j0; w.ref_slot += j0; w.cur_slot += j0; w.offsets += j0; w.in_off += j0; w.n_feat += j0; w.n_meas += j0;
     w.T_ref += 12 * (size_t)j0; w.T_cur += 12 * (size_t)j0; w.T_aligned += 12 * (size_t)j0;
-    w.aligned += j0; w.rel += 12 * (size_t)kTrackMaxLocal * j0;
+    w.aligned += j0; w.rel += 12 * (size_t)kTrackMaxLocal * j0; w.cam += 4 * (size_t)j0;
     w.cand_ok += c; w.cand_px += 2 * c; w.n_cand += j0; w.c_cnt += j0; w.c_off += j0; w.c_src += c;
     w.c_pw += 3 * c; w.c_px += 2 * c; w.c_depth += c; w.inlier += c; w.enable += c; w.n_inl += j0;
     w.results += j0; w.job_ref_slot += j0; w.orig += j0;
@@ -780,7 +787,7 @@ int launch_track_info(ygzb_tracker* t, const TrackBatch& b) {
     if (!t->d_info) return YGZB_OK;
     ygzb_ctx* ctx = t->ctx;
     ProfScope ps(ctx, kStageOther);
-    track_info_kernel<<<(unsigned)b.J, 1024, 0, ctx->stream>>>(t->st, b, (double)ctx->prm.fx, (double)ctx->prm.fy, t->d_info);
+    track_info_kernel<<<(unsigned)b.J, 1024, 0, ctx->stream>>>(t->st, b, t->d_info);
     YGZB_LAUNCHED(ctx);
     return YGZB_OK;
 }
@@ -902,7 +909,7 @@ int track_previous(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, ygzb
         if (rc == YGZB_OK) rc = launch_track_chain_mid(t->f, t->st, wb);
         if (rc == YGZB_OK)
             rc = launch_pose_only_dev(ctx, wb.J, wb.c_off, wb.c_cnt, wb.c_pw, wb.c_px, wb.T_cur, wb.inlier, wb.c_depth, wb.n_inl, wb.enable,
-                                      wb.pose_ws, cl, wb.cap);
+                                      wb.pose_ws, cl, wb.cap, wb.cam);
         if (rc != YGZB_OK) return rc;
         ProfScope ps(ctx, kStageOther);
         track_ref_write_kernel<<<(unsigned)wb.J, 256, 0, ctx->stream>>>(t->st, wb);
@@ -945,8 +952,22 @@ int ygzb_tracker_create(ygzb_frames* f, int n_streams, int max_jobs, const doubl
     const size_t S = (size_t)n_streams, R = YGZB_TRACK_RING, cells = (size_t)g.n_cells, E = S * R, cap = kTrackMaxLocal * cells;
     TrackStore& st = t->st;
     st.S = n_streams; st.R = (int)R; st.cells = (int)cells; st.W = g.W; st.H = g.H;
-    st.fx = K[0]; st.fy = K[1]; st.cx = K[2]; st.cy = K[3];
-    int rc = YGZB_OK;
+    // every stream starts with K, and with the context's float camera in the solvers
+    t->cam_K.resize(4 * S);
+    t->cam_F.resize(4 * S);
+    for (size_t s = 0; s < S; ++s) {
+        std::copy(K, K + 4, &t->cam_K[4 * s]);
+        t->cam_F[4 * s] = ctx->prm.fx; t->cam_F[4 * s + 1] = ctx->prm.fy; t->cam_F[4 * s + 2] = ctx->prm.cx; t->cam_F[4 * s + 3] = ctx->prm.cy;
+    }
+    int rc = check_cuda(ctx, cudaMalloc(&t->d_cam, 4 * S * (sizeof(double) + sizeof(float))), "cudaMalloc(tracker cameras)");
+    if (rc == YGZB_OK) {
+        st.cam_K = static_cast<double*>(t->d_cam);
+        st.cam_F = reinterpret_cast<float*>(static_cast<double*>(t->d_cam) + 4 * S);
+        rc = check_cuda(ctx, cudaMemcpyAsync(t->d_cam, t->cam_K.data(), 4 * S * sizeof(double), cudaMemcpyHostToDevice, ctx->stream), "H2D");
+    }
+    if (rc == YGZB_OK)
+        rc = check_cuda(ctx, cudaMemcpyAsync(const_cast<float*>(st.cam_F), t->cam_F.data(), 4 * S * sizeof(float), cudaMemcpyHostToDevice, ctx->stream),
+                        "H2D");
     {
         auto carve = [&](Carver& c) {
             st.kf_T = c.take<double>(E * 12); st.kf_n = c.take<int32_t>(E); st.kf_slot = c.take<int32_t>(E); st.kf_mp0 = c.take<long long>(E);
@@ -956,7 +977,7 @@ int ygzb_tracker_create(ygzb_frames* f, int n_streams, int max_jobs, const doubl
         };
         Carver sz(nullptr);
         carve(sz);
-        rc = check_cuda(ctx, cudaMalloc(&t->d_store, sz.bytes()), "cudaMalloc(tracker store)");
+        if (rc == YGZB_OK) rc = check_cuda(ctx, cudaMalloc(&t->d_store, sz.bytes()), "cudaMalloc(tracker store)");
         if (rc == YGZB_OK) rc = check_cuda(ctx, cudaMemsetAsync(t->d_store, 0, sz.bytes(), ctx->stream), "memset");
         if (rc == YGZB_OK) {
             Carver c(t->d_store);
@@ -984,6 +1005,7 @@ int ygzb_tracker_create(ygzb_frames* f, int n_streams, int max_jobs, const doubl
             b.pose_ws = c.take<double>(pose_only_ws_doubles((int)J));
             b.results = c.take<ygzb_track_result>(J);
             b.align_H = c.take<double>(J * 21);
+            b.cam = c.take<float>(J * 4);
         };
         Carver sz(nullptr);
         carve(sz);
@@ -1049,6 +1071,7 @@ void ygzb_tracker_destroy(ygzb_tracker* t) {
     if (t->d_ref) cudaFree(t->d_ref);
     if (t->h_aux) cudaFreeHost(t->h_aux);
     if (t->d_aux) cudaFree(t->d_aux);
+    if (t->d_cam) cudaFree(t->d_cam);
     if (t->staged) cudaEventDestroy(t->staged);
     if (t->front) {
         cudaStreamSynchronize(t->front);
@@ -1158,6 +1181,32 @@ int ygzb_tracker_set_start_pose(ygzb_tracker* t, int stream, const double T_cw[1
     return YGZB_OK;
 }
 
+int ygzb_tracker_set_camera(ygzb_tracker* t, int stream, const double K[4]) {
+    if (!t || !K) return YGZB_ERR_INVALID;
+    ygzb_ctx* ctx = t->ctx;
+    if (stream < 0 || stream >= t->st.S) return set_error(ctx, YGZB_ERR_INVALID, "set_camera: stream %d out of range", stream);
+    for (int c = 0; c < 4; ++c)
+        if (!std::isfinite(K[c])) return set_error(ctx, YGZB_ERR_INVALID, "set_camera: entry %d is not finite", c);
+    if (!(K[0] > 0 && K[1] > 0)) return set_error(ctx, YGZB_ERR_INVALID, "set_camera: focal lengths %g, %g must be positive", K[0], K[1]);
+    cudaSetDevice(ctx->device);
+    double* hk = &t->cam_K[4 * (size_t)stream];
+    float* hf = &t->cam_F[4 * (size_t)stream];
+    for (int c = 0; c < 4; ++c) {
+        hk[c] = K[c];
+        hf[c] = (float)K[c];
+    }
+    // ordered as an upload (ygzb_tracker_upload): on the front stream, behind the last key-frame insertion's kf_fill_kernel
+    // and the last tracking chain, the table's readers on the context's stream, but NOT behind a local BA in flight (its
+    // cameras are kernel parameters); the next tracking chain is on the front stream, and a key-frame insertion, an import
+    // and previous-frame tracking wait for e_up
+    YGZB_CUDA(ctx, cudaStreamWaitEvent(t->front, t->e_fill, 0));
+    YGZB_CUDA(ctx, cudaStreamWaitEvent(t->front, t->e_main, 0));
+    YGZB_CUDA(ctx, cudaMemcpyAsync(const_cast<double*>(t->st.cam_K) + 4 * stream, hk, 4 * sizeof(double), cudaMemcpyHostToDevice, t->front));
+    YGZB_CUDA(ctx, cudaMemcpyAsync(const_cast<float*>(t->st.cam_F) + 4 * stream, hf, 4 * sizeof(float), cudaMemcpyHostToDevice, t->front));
+    YGZB_CUDA(ctx, cudaEventRecord(t->e_up, t->front));
+    return YGZB_OK;
+}
+
 int ygzb_tracker_upload(ygzb_tracker* t, int first, int count, const uint8_t* host, size_t frame_stride) {
     if (!t) return YGZB_ERR_INVALID;
     ygzb_ctx* ctx = t->ctx;
@@ -1214,7 +1263,8 @@ int ygzb_tracker_track(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, 
     }
     rc = launch_track_chain_mid(t->f, t->st, b);
     if (rc != YGZB_OK) return rc;
-    rc = launch_pose_only_dev(ctx, n_jobs, b.c_off, b.c_cnt, b.c_pw, b.c_px, b.T_cur, b.inlier, b.c_depth, b.n_inl, b.enable, b.pose_ws, cl, b.cap);
+    rc = launch_pose_only_dev(ctx, n_jobs, b.c_off, b.c_cnt, b.c_pw, b.c_px, b.T_cur, b.inlier, b.c_depth, b.n_inl, b.enable, b.pose_ws, cl, b.cap,
+                              b.cam);
     if (rc == YGZB_OK) rc = launch_track_obs(t, b);
     if (rc == YGZB_OK) rc = launch_track_info(t, b);
     if (rc != YGZB_OK) return rc;
@@ -1315,6 +1365,10 @@ int ygzb_tracker_make_keyframes(ygzb_tracker* t, int n, const ygzb_keyframe_job*
         in.max_obs = (size_t)max_local * in.max_pts;
         in.max_free = max_local - 1;
         in.max_kf = max_local;
+        std::vector<float> cams(4 * (size_t)P);   // the float camera of every problem's stream
+        for (int i = 0; i < n; ++i)
+            if (prob_of[i] >= 0) std::copy_n(&t->cam_F[4 * (size_t)jobs[i].stream], 4, &cams[4 * (size_t)prob_of[i]]);
+        in.cam = reinterpret_cast<const float(*)[4]>(cams.data());
         void* scratch = static_cast<uint8_t*>(t->d_ba) + ((head + 255) & ~(size_t)255);
         rc = launch_local_ba2(ctx, in, scratch, ba, nullptr, &d_ba_stats);
         if (rc != YGZB_OK) return rc;
@@ -1408,7 +1462,7 @@ int ygzb_tracker_export(ygzb_tracker* t, int stream, int n_entries, const int32_
     if (rc != YGZB_OK) return rc;
     cudaSetDevice(ctx->device);
     out->width = st.W; out->height = st.H; out->cells = st.cells; out->n_levels = ctx->geo.n_levels;
-    out->K[0] = st.fx; out->K[1] = st.fy; out->K[2] = st.cx; out->K[3] = st.cy;
+    std::copy_n(&t->cam_K[4 * (size_t)stream], 4, out->K);
     out->n_keyframes = n_entries;
     out->pad = 0;
     for (int k = 0; k < n_entries; ++k) out->entry[k] = entries[k];
@@ -1458,8 +1512,9 @@ int ygzb_tracker_import(ygzb_tracker* t, int stream, const int32_t* entries, con
     if (in->width != st.W || in->height != st.H || in->cells != st.cells || in->n_levels != ctx->geo.n_levels)
         return set_error(ctx, YGZB_ERR_INVALID, "import: record geometry %dx%d, %d cells, %d levels; tracker %dx%d, %d cells, %d levels", in->width,
                          in->height, in->cells, in->n_levels, st.W, st.H, st.cells, ctx->geo.n_levels);
-    if (!(in->K[0] == st.fx && in->K[1] == st.fy && in->K[2] == st.cx && in->K[3] == st.cy))
-        return set_error(ctx, YGZB_ERR_INVALID, "import: record intrinsics differ from the tracker's");
+    const double* K = &t->cam_K[4 * (size_t)stream];
+    if (!(in->K[0] == K[0] && in->K[1] == K[1] && in->K[2] == K[2] && in->K[3] == K[3]))
+        return set_error(ctx, YGZB_ERR_INVALID, "import: record intrinsics differ from the stream's camera");
     const int n = in->n_keyframes;
     if (n < 0 || n > YGZB_TRACK_RING) return set_error(ctx, YGZB_ERR_INVALID, "import: %d key-frames (at most %d)", n, YGZB_TRACK_RING);
     if (n == 0) return YGZB_OK;
@@ -1530,7 +1585,7 @@ int ygzb_tracker_export_reference(ygzb_tracker* t, int stream, ygzb_reference_re
     if (slot < 0) return set_error(ctx, YGZB_ERR_INVALID, "export_reference: stream %d has no reference yet", stream);
     cudaSetDevice(ctx->device);
     out->width = st.W; out->height = st.H; out->cells = st.cells; out->n_levels = ctx->geo.n_levels;
-    out->K[0] = st.fx; out->K[1] = st.fy; out->K[2] = st.cx; out->K[3] = st.cy;
+    std::copy_n(&t->cam_K[4 * (size_t)stream], 4, out->K);
     MapXfer X;
     rc = tracker_xfer(t, X);
     if (rc != YGZB_OK) return rc;
@@ -1569,8 +1624,9 @@ int ygzb_tracker_import_reference(ygzb_tracker* t, int stream, const ygzb_refere
     if (in->width != st.W || in->height != st.H || in->cells != st.cells || in->n_levels != ctx->geo.n_levels)
         return set_error(ctx, YGZB_ERR_INVALID, "import_reference: record geometry %dx%d, %d cells, %d levels; tracker %dx%d, %d cells, %d levels",
                          in->width, in->height, in->cells, in->n_levels, st.W, st.H, st.cells, ctx->geo.n_levels);
-    if (!(in->K[0] == st.fx && in->K[1] == st.fy && in->K[2] == st.cx && in->K[3] == st.cy))
-        return set_error(ctx, YGZB_ERR_INVALID, "import_reference: record intrinsics differ from the tracker's");
+    const double* K = &t->cam_K[4 * (size_t)stream];
+    if (!(in->K[0] == K[0] && in->K[1] == K[1] && in->K[2] == K[2] && in->K[3] == K[3]))
+        return set_error(ctx, YGZB_ERR_INVALID, "import_reference: record intrinsics differ from the stream's camera");
     const int n = in->n;
     if (n < 0 || n > st.ref_cap) return set_error(ctx, YGZB_ERR_INVALID, "import_reference: %d features (capacity %d)", n, st.ref_cap);
     // ---- enqueue on the context's stream, behind the front stream's uploads and sparse alignment, like an import of a map;

@@ -15,7 +15,10 @@ constexpr int kTrackMaxLocal = 4;   // ring entries per stream = local key-frame
 
 struct TrackStore {
     int S, R, cells, W, H;
-    double fx, fy, cx, cy;      // caller-side intrinsics in double (config/default.yaml camera.*): candidate projection, map points
+    // the camera of every stream (ygzb_tracker_set_camera): K in double for candidate projection and map points, and the
+    // float camera of the solvers (the context's for a stream whose camera was never set, else (float)K)
+    const double* cam_K;        // [S][4] fx, fy, cx, cy
+    const float* cam_F;         // [S][4]
     // ring entry e = stream * R + entry
     double* kf_T;               // [S*R][12]   T_cw
     int32_t* kf_n;              // [S*R]       features = map points created by the key-frame
@@ -52,6 +55,7 @@ struct TrackBatch {
     // Matcher::SparseImageAlignment's motion check, poses relative to the local key-frames
     int32_t* aligned;           // [J]
     double* rel;                // [J][kTrackMaxLocal][12]
+    float* cam;                 // [J][4] float camera of the job's stream (track_prep_kernel): the solvers' per-problem camera
     // FindCandidates + FindDirectProjection, dense over (local key-frame, feature)
     uint8_t* cand_ok;           // [J][cap]
     double* cand_px;            // [J][cap][2]
@@ -77,7 +81,7 @@ int launch_track_chain_mid(ygzb_frames* f, const TrackStore& st, const TrackBatc
 // ba.cu
 int launch_pose_only_dev(ygzb_ctx* ctx, int n_problems, const int32_t* d_offsets, const int32_t* d_counts, const double* d_pw,
                          const double* d_px, double* d_T_cw, uint8_t* d_inlier, double* d_depth, int32_t* d_n_inlier, uint8_t* d_enable,
-                         double* d_ws, int cluster, int max_points);
+                         double* d_ws, int cluster, int max_points, const float* d_cam);
 size_t pose_only_ws_doubles(int n_problems);
 
 }  // namespace ygzb

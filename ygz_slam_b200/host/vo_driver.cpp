@@ -14,6 +14,7 @@
 //
 // Build: host C++ only (g++), links libygz_b200.so; see ygz_slam_b200/build.py (libygz_vo.so).
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <bit>
 #include <chrono>
@@ -565,12 +566,18 @@ struct QFrame {
     bool stacked;          // image lies in the caller's stacked sequence of the stream (one allocation, batch entry points)
     bool restart = false;  // first frame of a new sequence (ygz_vo_restart): it becomes a first key-frame
 };
+using Camera = std::array<double, 4>;   // fx, fy, cx, cy
+struct SeqStart {
+    Mat34 T;                  // pose of the sequence's first key-frame
+    Camera K;                 // camera of the sequence
+};
 struct EStream : Counters {
     std::deque<KfInfo> kfs;   // at most YGZB_TRACK_RING, the newest is the reference key-frame; the last kLocalKeyframes are local
     std::deque<QFrame> queue; // frames without a final result, oldest first; the first one is frame next_frame
     Mat34 T = identity();
     Mat34 start = identity(); // pose of the next sequence's first key-frame (ygz_vo_restart)
-    std::deque<Mat34> starts; // poses of the queued frames that start a sequence (the stream's first, restarts), in order
+    Camera cam{};             // camera of the current sequence, or of the next one while a restart is pending (ygz_vo_set_camera)
+    std::deque<SeqStart> starts;   // the queued frames that start a sequence (the stream's first, restarts), in order
     bool has_pose = false, lost = false, has_depth = false;
     bool restart_pending = false;   // the next push starts a new sequence at `start`
     int frames_since_kf = 0, next_frame = 0;
@@ -589,6 +596,8 @@ class Engine {
   public:
     Engine(ygzb_ctx* ctx, int n_streams, int window, const Params& p) : ctx_(ctx), S_(n_streams), F_(std::max(1, window)), prm_(p), st_(n_streams) {
         for (int i = 0; i < S_; ++i) order_.push_back(i);
+        for (EStream& s : st_) std::copy_n(prm_.K, 4, s.cam.begin());
+        tr_cam_.assign(S_, st_[0].cam);
         // YGZ_VO_BLOCKING_SYNC=1: sleep instead of spinning in the one synchronisation per round (hosts with fewer CPUs than
         // engine threads; bench.py sets it when the threads of all ranks outnumber the CPUs it may use)
         const char* e = std::getenv("YGZ_VO_BLOCKING_SYNC");
@@ -646,7 +655,7 @@ class Engine {
         QFrame f{image, depth, tag, stacked};
         if (pushed(i) == 0 || s.restart_pending) {
             f.restart = s.restart_pending;
-            s.starts.push_back(s.start);
+            s.starts.push_back({s.start, s.cam});
             s.restart_pending = false;
         }
         s.queue.push_back(f);
@@ -663,6 +672,14 @@ class Engine {
         EStream& s = st_[i];
         s.start = T;
         s.restart_pending = pushed(i) > 0;
+        return YGZB_OK;
+    }
+    // the camera of stream i's next sequence: only before its first push or while a restart is pending (the caller has
+    // checked K); it reaches the tracker when that sequence's first key-frame is decided (use_camera)
+    int set_camera(int i, const Camera& K) {
+        EStream& s = st_[i];
+        if (pushed(i) > 0 && !s.restart_pending) return YGZB_ERR_INVALID;
+        s.cam = K;
         return YGZB_OK;
     }
     // final results go to `traj` (this group's [S][n_frames][12], rows in the caller's stream order; NULL: none) and, with
@@ -976,7 +993,8 @@ class Engine {
                     s.next_mp = 0;
                     s.n_restarts += 1;
                 }
-                s.T = s.starts.front();
+                s.T = s.starts.front().T;
+                CHK(use_camera(b.stream, s.starts.front().K));   // (nothing of the old sequence is left to run)
                 s.starts.pop_front();
                 s.has_pose = true;
                 pend_keyframe(b.stream, b.stream * F_, -1, 0);
@@ -1034,6 +1052,7 @@ class Engine {
             slots.push_back(S_ * F_ + i * YGZB_TRACK_RING + kf.entry);
         }
         if (rec->n_keyframes != (int)entries.size()) return YGZB_ERR_INVALID;
+        CHK(use_camera(i, s.cam));
         CHK(ygzb_tracker_import(tr_, i, entries.data(), slots.data(), rec));
         if (ref) CHK(ygzb_tracker_import_reference(tr_, i, ref));
         st_[i] = s;
@@ -1054,6 +1073,13 @@ class Engine {
     int check_start_pose(int i, const Mat34& T) { return ygzb_tracker_set_start_pose(tr_, i, T.m); }
 
   private:
+    // the tracker's camera of stream i becomes K for everything enqueued from here on (nothing is enqueued when it is K already)
+    int use_camera(int i, const Camera& K) {
+        if (tr_cam_[i] == K) return YGZB_OK;
+        CHK(ygzb_tracker_set_camera(tr_, i, K.data()));
+        tr_cam_[i] = K;
+        return YGZB_OK;
+    }
     // the first w queued frames of stream i into its frame slots: one strided copy when they are equally spaced in one
     // stacked sequence, one copy per frame otherwise (frames pushed one by one may sit in separate allocations, which one
     // strided copy cannot span even when their addresses happen to be equally spaced)
@@ -1175,6 +1201,7 @@ class Engine {
     std::vector<ygzb_keyframe_job> kjobs_;   // key-frame insertions for the next round ...
     std::vector<KfFrame> kframes_;           // ... and their frames
     std::vector<int> order_;
+    std::vector<Camera> tr_cam_;   // the tracker's camera of every stream (ygzb_tracker_set_camera), as last set
     double* traj_ = nullptr;
     int traj_frames_ = 0;
     bool collect_ = false;
@@ -1795,6 +1822,21 @@ int ygz_vo_restart(ygz_vo* vo, int stream, const double T_cw[12]) {
     return vo->eng->restart(stream, T);
 }
 
+int ygz_vo_set_camera(ygz_vo* vo, int stream, const double K[4]) {
+    if (!vo || !K || stream < 0 || stream >= vo->n_streams) return YGZB_ERR_INVALID;
+    for (int c = 0; c < 4; ++c)
+        if (!std::isfinite(K[c])) return YGZB_ERR_INVALID;
+    if (!(K[0] > 0 && K[1] > 0)) return YGZB_ERR_INVALID;
+    return vo->eng->set_camera(stream, Camera{K[0], K[1], K[2], K[3]});
+}
+
+int ygz_vo_get_camera(const ygz_vo* vo, int stream, double K[4]) {
+    if (!vo || !K || stream < 0 || stream >= vo->n_streams) return YGZB_ERR_INVALID;
+    const Camera& c = vo->eng->streams()[stream].cam;
+    std::copy(c.begin(), c.end(), K);
+    return YGZB_OK;
+}
+
 int ygz_vo_step(ygz_vo* vo) {
     if (!vo) return YGZB_ERR_INVALID;
     bool idle = false;
@@ -1875,6 +1917,8 @@ int ygz_vo_save_stream(ygz_vo* vo, int stream, void* buf, size_t capacity, size_
     if (!e.settled(stream)) return YGZB_ERR_INVALID;
     if (!vo->stage.mem) CHK(vo->stage.init(vo->geom));
     const EStream& s = e.streams()[stream];
+    RecordGeom g = vo->geom;   // with the stream's own camera
+    std::copy(s.cam.begin(), s.cam.end(), g.K);
     SaveStage& st = vo->stage;
     CHK(e.export_map(stream, &st.map));
     const bool ref = e.has_reference(stream);
@@ -1882,11 +1926,11 @@ int ygz_vo_save_stream(ygz_vo* vo, int stream, void* buf, size_t capacity, size_
     if (s.has_depth) CHK(e.get_depth(stream, st.depth));
     CHK(ygzb_synchronize(vo->ctx));
     RecordWriter count{nullptr};
-    write_record(count, vo->geom, s, st.map, ref ? &st.ref : nullptr, s.has_depth ? st.depth : nullptr);
+    write_record(count, g, s, st.map, ref ? &st.ref : nullptr, s.has_depth ? st.depth : nullptr);
     *size = count.n;
     if (count.n > capacity) return YGZB_ERR_CAPACITY;
     RecordWriter w{static_cast<uint8_t*>(buf)};
-    write_record(w, vo->geom, s, st.map, ref ? &st.ref : nullptr, s.has_depth ? st.depth : nullptr);
+    write_record(w, g, s, st.map, ref ? &st.ref : nullptr, s.has_depth ? st.depth : nullptr);
     return YGZB_OK;
 }
 
@@ -1896,8 +1940,12 @@ int ygz_vo_load_stream(ygz_vo* vo, int stream, const void* buf, size_t size) {
     if (!vo || !buf || stream < 0 || stream >= vo->n_streams) return YGZB_ERR_INVALID;
     Engine& e = *vo->eng;
     if (!e.settled(stream)) return YGZB_ERR_INVALID;
-    StreamRecord rec(vo->geom);
-    CHK(read_record(static_cast<const uint8_t*>(buf), size, vo->geom, rec));
+    const Camera cam = e.streams()[stream].cam;   // the record's K must be the destination stream's camera
+    RecordGeom g = vo->geom;
+    std::copy(cam.begin(), cam.end(), g.K);
+    StreamRecord rec(g);
+    CHK(read_record(static_cast<const uint8_t*>(buf), size, g, rec));
+    rec.s.cam = cam;
     CHK(e.check_start_pose(stream, rec.s.start));
     CHK(e.adopt(stream, rec.s, &rec.map.rec, rec.has_ref ? &rec.ref.rec : nullptr));
     if (rec.s.has_depth) CHK(e.set_depth(stream, rec.depth.data()));

@@ -77,16 +77,19 @@ class VisualOdometry:
     SLOTS_PER_STREAM = LOCAL_KEYFRAMES + 2
 
     def __init__(self, backend, n_streams: int, stream_ids=None, kf_min_frames: int | None = None, kf_min_rot: float | None = None,
-                 kf_min_trans: float | None = None, ref_mode: str = "keyframe"):
+                 kf_min_trans: float | None = None, ref_mode: str = "keyframe", camera=None):
         """ref_mode: what a frame is aligned against by the sparse alignment.  "previous" is the reference's rule
         (VisualOdometry.cpp:66 and :88-90: the previous tracked frame, or the key-frame it became); "keyframe" aligns every
-        frame against the newest key-frame, which makes the frames between two key-frames independent of each other."""
+        frame against the newest key-frame, which makes the frames between two key-frames independent of each other.
+        camera: (fx, fy, cx, cy) in double of the candidate projection and the key-frames' map points (default: the TUM
+        camera, synth.FX..CY); the backend's solvers use their own camera, which must be this one rounded to float."""
         if ref_mode not in ("keyframe", "previous"):
             raise ValueError(f"ref_mode must be 'keyframe' or 'previous', not {ref_mode!r}")
         params = inspect.signature(backend.pose_only).parameters.values() if ref_mode == "previous" else ()
         if ref_mode == "previous" and not any(p.name == "return_depth" or p.kind is p.VAR_KEYWORD for p in params):
             raise TypeError("ref_mode='previous' needs a backend whose pose_only(..., return_depth=True) returns pose-only's depths")
         self.ref_mode = ref_mode
+        self.K = tuple(float(v) for v in (camera if camera is not None else (synth.FX, synth.FY, synth.CX, synth.CY)))
         self.be = backend
         self.streams = [Stream(sid=(stream_ids[i] if stream_ids else i),
                                slots=tuple(range(i * self.SLOTS_PER_STREAM, (i + 1) * self.SLOTS_PER_STREAM)))
@@ -174,8 +177,8 @@ class VisualOdometry:
                 pc = (T[:, :3] @ kf.pw.T).T + T[:, 3]
                 z = pc[:, 2]
                 with np.errstate(divide="ignore", invalid="ignore"):
-                    u = synth.FX * pc[:, 0] / z + synth.CX
-                    v = synth.FY * pc[:, 1] / z + synth.CY
+                    u = self.K[0] * pc[:, 0] / z + self.K[2]
+                    v = self.K[1] * pc[:, 1] / z + self.K[3]
                 good = np.nonzero((z > 0) & (u >= 20) & (u < synth.W - 20) & (v >= 20) & (v < synth.H - 20))[0]
                 kf_of.append(np.full(len(good), k, np.int32)); n_of.append(good.astype(np.int32))
                 uu.append(u[good]); vv.append(v[good]); ids.append(kf.mp_id[good])
@@ -246,7 +249,8 @@ class VisualOdometry:
             d = depths[i][f["py"].astype(int), f["px"].astype(int)]
             T = st.T_cw
             Tin = se3.inv(T)
-            pc = np.stack([(px[:, 0] - synth.CX) * d / synth.FX, (px[:, 1] - synth.CY) * d / synth.FY, d], 1)
+            fx, fy, cx, cy = self.K
+            pc = np.stack([(px[:, 0] - cx) * d / fx, (px[:, 1] - cy) * d / fy, d], 1)
             pw = (Tin[:, :3] @ pc.T).T + Tin[:, 3]
             ids = np.arange(st.next_mp, st.next_mp + len(d))
             st.next_mp += len(d)

@@ -38,6 +38,8 @@ def _lib():
         _LIB.ygz_vo_create.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         _LIB.ygz_vo_push.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int64]
         _LIB.ygz_vo_restart.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        _LIB.ygz_vo_set_camera.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        _LIB.ygz_vo_get_camera.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         _LIB.ygz_vo_step.argtypes = [C.c_void_p]
         _LIB.ygz_vo_flush.argtypes = [C.c_void_p]
         _LIB.ygz_vo_poll.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
@@ -232,10 +234,11 @@ class Engine:
     returns them too.  information=True: every result carries how well its pose is determined (ygz_vo_set_information):
     poll also returns an [n, 2, 6, 6] array, the sparse alignment's Fisher information and pose-only's information
     matrix of each result as full symmetric matrices.  map_updates=True: every key-frame insertion queues what it changed
-    in the local map (ygz_vo_set_map_updates), which poll_map_updates returns."""
+    in the local map (ygz_vo_set_map_updates), which poll_map_updates returns.  cameras: None, or one (fx, fy, cx, cy)
+    per stream (None: K), set before any push (ygz_vo_set_camera)."""
 
     def __init__(self, ctx, n_streams, window=8, ref_mode="keyframe", kf_min_frames=10, kf_min_rot=0.1, kf_min_trans=0.1,
-                 min_inliers=30, K=None, observations=False, information=False, map_updates=False):
+                 min_inliers=30, K=None, observations=False, information=False, map_updates=False, cameras=None):
         if ref_mode not in _REF_MODES:
             raise ValueError(f"ref_mode must be 'keyframe' or 'previous', not {ref_mode!r}")
         p = ctx.params
@@ -260,6 +263,24 @@ class Engine:
         self._map_rows = np.zeros(0, MAP_POINT_DTYPE)   # rows of one ygz_vo_poll_map_updates call, grown on demand
         if map_updates:
             self.set_map_updates(True)
+        if cameras is not None:
+            if len(cameras) != self.n_streams:
+                raise ValueError(f"cameras: {len(cameras)} cameras for {self.n_streams} streams")
+            for s, cam in enumerate(cameras):
+                if cam is not None:
+                    self.set_camera(s, cam)
+
+    def set_camera(self, stream, K):
+        """K = (fx, fy, cx, cy) of `stream`'s next sequence (ygz_vo_set_camera): only before its first push or while a
+        restart is pending; frames pushed before the restart keep the old camera."""
+        K = np.ascontiguousarray(K, np.float64).reshape(4)
+        self.ctx.check(self.lib.ygz_vo_set_camera(self.h, int(stream), K.ctypes.data), "ygz_vo_set_camera")
+
+    def camera(self, stream):
+        """The camera (fx, fy, cx, cy) set_camera last gave `stream` (the engine's K until then)."""
+        K = np.zeros(4, np.float64)
+        self.ctx.check(self.lib.ygz_vo_get_camera(self.h, int(stream), K.ctypes.data), "ygz_vo_get_camera")
+        return K
 
     def set_observations(self, on):
         """Switch the observation rows of the results on or off (ygz_vo_set_observations): only while the engine is
