@@ -112,8 +112,7 @@ def _sentinel(buf):
 
 
 def _set_obs(tr, buf, capacity=None):
-    tr.lib.ygzb_tracker_set_observations.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
-    return tr.lib.ygzb_tracker_set_observations(tr.h, None if buf is None else buf.ctypes.data, len(buf) if capacity is None else capacity)
+    return tr.set_observations(buf, capacity)
 
 
 def _want_rows(dbg, mp0_of_local, cells):

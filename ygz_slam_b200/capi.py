@@ -912,20 +912,26 @@ class Tracker:
         except Exception:
             pass
 
+    def _set_output(self, name, buf, capacity):
+        fn = getattr(self.lib, name)
+        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+        return fn(self.h, None if buf is None else buf.ctypes.data, (0 if buf is None else len(buf)) if capacity is None else capacity)
+
+    def set_observations(self, buf, capacity=None):
+        """ygzb_tracker_set_observations: from the next track on, job j's observation rows go to buf[j * TRACK_RING * cells
+        ...] (a page-locked vo_native.OBS_DTYPE array, pinned_empty; None switches the rows off).  Returns the C status."""
+        return self._set_output("ygzb_tracker_set_observations", buf, capacity)
+
     def set_information(self, buf, capacity=None):
         """ygzb_tracker_set_information: from the next track on, job j's record goes to buf[j] (a page-locked INFO_DTYPE
         array, pinned_empty; None switches the records off).  Returns the C status."""
-        self.lib.ygzb_tracker_set_information.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
-        return self.lib.ygzb_tracker_set_information(self.h, None if buf is None else buf.ctypes.data,
-                                                     (0 if buf is None else len(buf)) if capacity is None else capacity)
+        return self._set_output("ygzb_tracker_set_information", buf, capacity)
 
     def set_map_updates(self, buf, capacity=None):
         """ygzb_tracker_set_map_updates: from the next make_keyframes on, key-frame job j's map rows (ba_points moved, then
         n_features new) go to buf[j * TRACK_RING * cells ...] (a page-locked MAP_POINT_DTYPE array, pinned_empty; None
         switches the rows off).  Returns the C status."""
-        self.lib.ygzb_tracker_set_map_updates.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
-        return self.lib.ygzb_tracker_set_map_updates(self.h, None if buf is None else buf.ctypes.data,
-                                                     (0 if buf is None else len(buf)) if capacity is None else capacity)
+        return self._set_output("ygzb_tracker_set_map_updates", buf, capacity)
 
     def export(self, stream: int, entries, images: bool = True, out: MapBuffers | None = None) -> MapBuffers:
         """Map record of ring entries `entries` of `stream`, complete (the call synchronises the context)."""

@@ -772,23 +772,39 @@ int tracker_xfer(ygzb_tracker* t, MapXfer& X) {
     return YGZB_OK;
 }
 
-// the observation rows of a whole batch (all its jobs have been through pose-only), when the caller asked for them
-int launch_track_obs(ygzb_tracker* t, const TrackBatch& b) {
-    if (!t->d_obs) return YGZB_OK;
-    ygzb_ctx* ctx = t->ctx;
-    ProfScope ps(ctx, kStageOther);
-    track_obs_kernel<<<(unsigned)b.J, 1024, kObsSmem, ctx->stream>>>(t->st, b, t->d_obs);
-    YGZB_LAUNCHED(ctx);
-    return YGZB_OK;
+// the batch arrays of a tracking batch of n_jobs jobs (the sparse alignment keeps its Hessians for the information records only)
+TrackBatch job_batch(ygzb_tracker* t, int n_jobs) {
+    TrackBatch b = t->b;
+    b.J = n_jobs;
+    if (!t->d_info) b.align_H = nullptr;
+    t->last_J = n_jobs;
+    return b;
 }
 
-// the information records of a whole batch (all its jobs have been through pose-only), when the caller asked for them
-int launch_track_info(ygzb_tracker* t, const TrackBatch& b) {
-    if (!t->d_info) return YGZB_OK;
+// the tail of a tracking batch whose jobs have all been through pose-only: the observation rows and information records
+// (when the caller asked for them), the results and their copy back, then e_main; before_copy() enqueues what has to come
+// between the results and their copy
+template <typename BeforeCopy>
+int finish_batch(ygzb_tracker* t, const TrackBatch& b, ygzb_track_result* results, BeforeCopy before_copy) {
     ygzb_ctx* ctx = t->ctx;
-    ProfScope ps(ctx, kStageOther);
-    track_info_kernel<<<(unsigned)b.J, 1024, 0, ctx->stream>>>(t->st, b, t->d_info);
-    YGZB_LAUNCHED(ctx);
+    if (t->d_obs) {
+        ProfScope ps(ctx, kStageOther);
+        track_obs_kernel<<<(unsigned)b.J, 1024, kObsSmem, ctx->stream>>>(t->st, b, t->d_obs);
+        YGZB_LAUNCHED(ctx);
+    }
+    if (t->d_info) {
+        ProfScope ps(ctx, kStageOther);
+        track_info_kernel<<<(unsigned)b.J, 1024, 0, ctx->stream>>>(t->st, b, t->d_info);
+        YGZB_LAUNCHED(ctx);
+    }
+    {
+        ProfScope ps(ctx, kStageOther);
+        track_finish_kernel<<<(b.J + 63) / 64, 64, 0, ctx->stream>>>(b);
+        YGZB_LAUNCHED(ctx);
+    }
+    TRY(before_copy());
+    YGZB_CUDA(ctx, cudaMemcpyAsync(results, b.results, sizeof(ygzb_track_result) * (size_t)b.J, cudaMemcpyDeviceToHost, ctx->stream));
+    YGZB_CUDA(ctx, cudaEventRecord(t->e_main, ctx->stream));
     return YGZB_OK;
 }
 
@@ -811,6 +827,27 @@ int mapped_view(ygzb_ctx* ctx, const void* host, size_t bytes, size_t align, con
         return set_error(ctx, YGZB_ERR_INVALID, "%s: the buffer spans more than one page-locked allocation", what);
     if (reinterpret_cast<uintptr_t>(dev[0]) % align) return set_error(ctx, YGZB_ERR_INVALID, "%s: buffer not %zu-byte aligned", what, align);
     *out = dev[0];
+    return YGZB_OK;
+}
+
+#define STRINGIFY_(x) #x
+#define STRINGIFY(x) STRINGIFY_(x)
+
+// one of the tracker's optional outputs: *dev becomes the device view of the caller's page-locked buffer `host` of `capacity`
+// elements, `need` of which the tracker writes (`rule` spells `need` out in the message), or NULL for a NULL host, which
+// switches the writes off.  A call that fails leaves *dev as it was
+template <typename T>
+int attach_output(ygzb_tracker* t, T* host, size_t capacity, size_t need, size_t align, const char* what, const char* rule, T** dev) {
+    if (!host) {
+        *dev = nullptr;
+        return YGZB_OK;
+    }
+    ygzb_ctx* ctx = t->ctx;
+    if (capacity < need) return set_error(ctx, YGZB_ERR_INVALID, "%s: capacity %zu %s = %zu", what, capacity, rule, need);
+    cudaSetDevice(ctx->device);
+    void* view = nullptr;
+    TRY(mapped_view(ctx, host, need * sizeof(T), align, what, &view));
+    *dev = static_cast<T*>(view);
     return YGZB_OK;
 }
 
@@ -887,15 +924,12 @@ int track_previous(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, ygzb
         h_ref_slot[p] = last[s] < 0 ? t->cur_ref[s] : jobs[last[s]].cur_slot;
         last[s] = j;
     }
-    TrackBatch b = t->b;
-    b.J = n_jobs;
-    if (!t->d_info) b.align_H = nullptr;
+    TrackBatch b = job_batch(t, n_jobs);
     b.prev = 1;
     b.job_ref_slot = t->d_aux;
     b.orig = t->d_aux + t->max_jobs;
     // the sparse alignment's per-feature scratch, for ref_cap features per problem (a wave has at most one job per stream)
     b.sa2_scratch = static_cast<uint8_t*>(t->d_ref) + ref_store_bytes(t->st);
-    t->last_J = n_jobs;
     const int cl = t->cluster;
     // uploads ran on the front stream; a key-frame insertion (and its BA) is on this stream already
     YGZB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, t->e_up, 0));
@@ -915,23 +949,15 @@ int track_previous(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, ygzb
         track_ref_write_kernel<<<(unsigned)wb.J, 256, 0, ctx->stream>>>(t->st, wb);
         YGZB_LAUNCHED(ctx);
     }
-    int rc = launch_track_obs(t, b);   // every wave's jobs keep their rows of the batch arrays
-    if (rc == YGZB_OK) rc = launch_track_info(t, b);
-    if (rc != YGZB_OK) return rc;
-    {
-        ProfScope ps(ctx, kStageOther);
-        track_finish_kernel<<<(n_jobs + 63) / 64, 64, 0, ctx->stream>>>(b);
-        YGZB_LAUNCHED(ctx);
-    }
-    for (int s = 0; s < S; ++s)
-        if (last[s] >= 0) {
-            const int rc = ygzb_frames_copy(t->f, jobs[last[s]].cur_slot, t->ref_slots[s]);
-            if (rc != YGZB_OK) return rc;
-            t->cur_ref[s] = t->ref_slots[s];
-        }
-    YGZB_CUDA(ctx, cudaMemcpyAsync(results, b.results, sizeof(ygzb_track_result) * (size_t)n_jobs, cudaMemcpyDeviceToHost, ctx->stream));
-    YGZB_CUDA(ctx, cudaEventRecord(t->e_main, ctx->stream));
-    return YGZB_OK;
+    // (every wave's jobs keep their rows of the batch arrays)
+    return finish_batch(t, b, results, [&] {
+        for (int s = 0; s < S; ++s)
+            if (last[s] >= 0) {
+                TRY(ygzb_frames_copy(t->f, jobs[last[s]].cur_slot, t->ref_slots[s]));
+                t->cur_ref[s] = t->ref_slots[s];
+            }
+        return YGZB_OK;
+    });
 }
 
 extern "C" {
@@ -1239,10 +1265,7 @@ int ygzb_tracker_track(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, 
     if (t->ref_mode == YGZB_TRACK_REF_PREVIOUS) return track_previous(t, n_jobs, jobs, results);
     YGZB_CUDA(ctx, cudaEventSynchronize(t->staged));   // the previous copy out of the staging buffer has finished
     memcpy(t->h_jobs, jobs, sizeof(ygzb_track_job) * (size_t)n_jobs);
-    TrackBatch b = t->b;
-    b.J = n_jobs;
-    if (!t->d_info) b.align_H = nullptr;
-    t->last_J = n_jobs;
+    const TrackBatch b = job_batch(t, n_jobs);
     t->pos_of.clear();
     const int cl = t->cluster;
     int rc;
@@ -1265,17 +1288,8 @@ int ygzb_tracker_track(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, 
     if (rc != YGZB_OK) return rc;
     rc = launch_pose_only_dev(ctx, n_jobs, b.c_off, b.c_cnt, b.c_pw, b.c_px, b.T_cur, b.inlier, b.c_depth, b.n_inl, b.enable, b.pose_ws, cl, b.cap,
                               b.cam);
-    if (rc == YGZB_OK) rc = launch_track_obs(t, b);
-    if (rc == YGZB_OK) rc = launch_track_info(t, b);
     if (rc != YGZB_OK) return rc;
-    {
-        ProfScope ps(ctx, kStageOther);
-        track_finish_kernel<<<(n_jobs + 63) / 64, 64, 0, ctx->stream>>>(b);
-        YGZB_LAUNCHED(ctx);
-    }
-    YGZB_CUDA(ctx, cudaMemcpyAsync(results, b.results, sizeof(ygzb_track_result) * (size_t)n_jobs, cudaMemcpyDeviceToHost, ctx->stream));
-    YGZB_CUDA(ctx, cudaEventRecord(t->e_main, ctx->stream));
-    return YGZB_OK;
+    return finish_batch(t, b, results, [] { return YGZB_OK; });
 }
 
 int ygzb_tracker_make_keyframes(ygzb_tracker* t, int n, const ygzb_keyframe_job* jobs, const ygzb_ba_params* ba,
@@ -1396,56 +1410,25 @@ int ygzb_tracker_make_keyframes(ygzb_tracker* t, int n, const ygzb_keyframe_job*
     return YGZB_OK;
 }
 
+// (the row buffers are 16-byte aligned: their kernels write the rows as 16-byte stores)
 int ygzb_tracker_set_observations(ygzb_tracker* t, ygzb_observation* host, size_t capacity) {
     if (!t) return YGZB_ERR_INVALID;
-    ygzb_ctx* ctx = t->ctx;
-    if (!host) {
-        t->d_obs = nullptr;
-        return YGZB_OK;
-    }
-    const size_t need = (size_t)t->max_jobs * t->b.cap;
-    if (capacity < need) return set_error(ctx, YGZB_ERR_INVALID, "set_observations: capacity %zu rows below max_jobs * %d * cells = %zu", capacity,
-                                          YGZB_TRACK_RING, need);
-    cudaSetDevice(ctx->device);
-    void* dev = nullptr;   // (16-byte aligned: the kernel writes the rows as 16-byte stores)
-    TRY(mapped_view(ctx, host, need * sizeof(ygzb_observation), 16, "set_observations", &dev));
-    YGZB_CUDA(ctx, cudaFuncSetAttribute(track_obs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kObsSmem));
-    t->d_obs = static_cast<ygzb_observation*>(dev);
+    TRY(attach_output(t, host, capacity, (size_t)t->max_jobs * t->b.cap, 16, "set_observations",
+                      "rows below max_jobs * " STRINGIFY(YGZB_TRACK_RING) " * cells", &t->d_obs));
+    if (host) YGZB_CUDA(t->ctx, cudaFuncSetAttribute(track_obs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kObsSmem));
     return YGZB_OK;
 }
 
 int ygzb_tracker_set_information(ygzb_tracker* t, ygzb_pose_information* host, size_t capacity) {
     if (!t) return YGZB_ERR_INVALID;
-    ygzb_ctx* ctx = t->ctx;
-    if (!host) {
-        t->d_info = nullptr;
-        return YGZB_OK;
-    }
-    const size_t need = (size_t)t->max_jobs;
-    if (capacity < need) return set_error(ctx, YGZB_ERR_INVALID, "set_information: capacity %zu records below max_jobs = %zu", capacity, need);
-    cudaSetDevice(ctx->device);
-    void* dev = nullptr;
-    TRY(mapped_view(ctx, host, need * sizeof(ygzb_pose_information), alignof(double), "set_information", &dev));
-    t->d_info = static_cast<ygzb_pose_information*>(dev);
-    return YGZB_OK;
+    return attach_output(t, host, capacity, (size_t)t->max_jobs, alignof(double), "set_information", "records below max_jobs", &t->d_info);
 }
 
 int ygzb_tracker_set_map_updates(ygzb_tracker* t, ygzb_map_point* host, size_t capacity) {
     if (!t) return YGZB_ERR_INVALID;
-    ygzb_ctx* ctx = t->ctx;
-    if (!host) {
-        t->d_map = nullptr;
-        return YGZB_OK;
-    }
-    const size_t need = (size_t)t->st.S * YGZB_TRACK_RING * t->st.cells;   // a key-frame batch has at most one job per stream
-    if (capacity < need)
-        return set_error(ctx, YGZB_ERR_INVALID, "set_map_updates: capacity %zu rows below n_streams * %d * cells = %zu", capacity,
-                         YGZB_TRACK_RING, need);
-    cudaSetDevice(ctx->device);
-    void* dev = nullptr;   // (16-byte aligned: the kernel writes the rows as 16-byte stores)
-    TRY(mapped_view(ctx, host, need * sizeof(ygzb_map_point), 16, "set_map_updates", &dev));
-    t->d_map = static_cast<ygzb_map_point*>(dev);
-    return YGZB_OK;
+    // a key-frame batch has at most one job per stream
+    return attach_output(t, host, capacity, (size_t)t->st.S * YGZB_TRACK_RING * t->st.cells, 16, "set_map_updates",
+                         "rows below n_streams * " STRINGIFY(YGZB_TRACK_RING) " * cells", &t->d_map);
 }
 
 int ygzb_tracker_export(ygzb_tracker* t, int stream, int n_entries, const int32_t* entries, ygzb_map_record* out) {

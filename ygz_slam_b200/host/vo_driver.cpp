@@ -584,14 +584,130 @@ struct EStream : Counters {
     long next_mp = 0;
 };
 
+// a page-locked buffer the tracker writes through its device mapping, `stride` elements per job, switched on and off
+// through one of the tracker's setters (ygzb_tracker_set_observations, _information, _map_updates)
+template <typename T>
+struct PinnedOutput {
+    T* h = nullptr;   // NULL: off
+    size_t stride = 0;
+    PinnedOutput() = default;
+    PinnedOutput(const PinnedOutput&) = delete;
+    PinnedOutput& operator=(const PinnedOutput&) = delete;
+    ~PinnedOutput() {
+        if (h) ygzb_host_free(h);
+    }
+    bool on() const { return h != nullptr; }
+    // job j's elements of the batch that has just come back, or NULL when off
+    const T* job(size_t j) const { return h ? h + j * stride : nullptr; }
+    // on: room for `jobs` jobs of `per_job` elements, allocated and handed to the tracker; off: the tracker stops writing
+    // and, once the device has caught up, the buffer is freed
+    int set(ygzb_ctx* ctx, ygzb_tracker* tr, int (*attach)(ygzb_tracker*, T*, size_t), bool on_, size_t jobs, size_t per_job) {
+        if (on_ == on()) return YGZB_OK;
+        if (!on_) {
+            CHK(attach(tr, nullptr, 0));
+            CHK(ygzb_synchronize(ctx));
+            ygzb_host_free(h);
+            h = nullptr;
+            return YGZB_OK;
+        }
+        void* p = nullptr;
+        CHK(ygzb_host_alloc(&p, jobs * per_job * sizeof(T)));
+        const int rc = attach(tr, static_cast<T*>(p), jobs * per_job);
+        if (rc != YGZB_OK) {
+            ygzb_host_free(p);
+            return rc;
+        }
+        h = static_cast<T*>(p);
+        stride = per_job;
+        return YGZB_OK;
+    }
+};
+
+// the part of a queue's buffer before `head` has been taken: clear the buffer when it is drained, erase that part once it
+// passes half of it
+template <typename T>
+void compact(std::vector<T>& v, size_t& head) {
+    if (head == v.size()) {
+        v.clear();
+        head = 0;
+    } else if (head > v.size() / 2) {
+        v.erase(v.begin(), v.begin() + (ptrdiff_t)head);
+        head = 0;
+    }
+}
+
+// records, oldest first, each with its run of rows: the records from `first` and the rows back to back from `head`, each
+// in one buffer that keeps its capacity across rounds, so that a round neither allocates nor touches fresh pages once the
+// buffers have grown
+template <typename Rec, typename Row>
+struct RowQueue {
+    struct Entry {
+        Rec rec;
+        size_t n_rows;
+    };
+    std::vector<Entry> recs;
+    std::vector<Row> rows;
+    size_t first = 0, head = 0;
+
+    size_t size() const { return recs.size() - first; }
+    bool empty() const { return size() == 0; }
+    const Entry& operator[](size_t i) const { return recs[first + i]; }
+    const Row* front_rows() const { return rows.data() + head; }
+    void push(const Rec& rec, const Row* r, size_t n_rows) {
+        recs.push_back({rec, n_rows});
+        rows.insert(rows.end(), r, r + n_rows);
+    }
+    void drop(size_t k) { take(k, nullptr, [](size_t, const Rec&) {}); }
+    // the k oldest records leave: each to put(i, record), their rows to `out` (NULL: dropped); returns their row count
+    template <typename Put>
+    size_t take(size_t k, Row* out, Put put) {
+        size_t n = 0;
+        for (size_t i = 0; i < k; ++i) {
+            put(i, (*this)[i].rec);
+            n += (*this)[i].n_rows;
+        }
+        if (out && n) std::memcpy(out, front_rows(), n * sizeof(Row));
+        first += k;
+        head += n;
+        compact(recs, first);
+        compact(rows, head);
+        return n;
+    }
+    // whole records, oldest first, while their rows fit: at most `capacity` records, their rows into out[row_capacity];
+    // YGZB_ERR_CAPACITY with *n = 0 and *n_rows = its row count when the first one's rows do not fit (never for capacity 0)
+    template <typename Put>
+    int take_whole(int capacity, int* n, Row* out, size_t row_capacity, size_t* n_rows, Put put) {
+        *n = 0;
+        *n_rows = 0;
+        if (capacity > 0 && !empty() && (*this)[0].n_rows > row_capacity) {
+            *n_rows = (*this)[0].n_rows;
+            return YGZB_ERR_CAPACITY;
+        }
+        for (size_t used = 0; *n < capacity && *n < (int)size() && used + (*this)[*n].n_rows <= row_capacity;) used += (*this)[(*n)++].n_rows;
+        *n_rows = take(*n, out, put);
+        return YGZB_OK;
+    }
+};
+
+// what a frame's result carries besides its pose: its observation rows (observations on) and its information record
+// (information on; NULL: zeros, as for a sequence's first key-frame and a LOST frame)
+struct Attachments {
+    const ygzb_observation* rows = nullptr;
+    size_t n_rows = 0;
+    const ygzb_pose_information* info = nullptr;
+};
+
 class Engine {
     struct Win { int stream, first, count, job0; };   // a window in flight: frames [first, first + count) of a stream (job0 < 0: first frame)
     struct KfFrame {   // the frame behind a pending key-frame job
         int frame, n_inliers;
         int64_t tag;
         const double* depth;
-        size_t obs0, n_obs;   // its tracking job's observation rows in kf_rows_ (observations on)
         ygzb_pose_information info;   // its tracking job's information record (information on; zeros for a first key-frame)
+    };
+    struct Result {   // a final result and its information record (zeros while information is off)
+        ygz_vo_result r;
+        ygzb_pose_information info;
     };
   public:
     Engine(ygzb_ctx* ctx, int n_streams, int window, const Params& p) : ctx_(ctx), S_(n_streams), F_(std::max(1, window)), prm_(p), st_(n_streams) {
@@ -608,9 +724,6 @@ class Engine {
         if (fr_) ygzb_frames_destroy(fr_);
         if (h_res_) ygzb_host_free(h_res_);
         if (h_kres_) ygzb_host_free(h_kres_);
-        if (h_obs_) ygzb_host_free(h_obs_);
-        if (h_info_) ygzb_host_free(h_info_);
-        if (h_map_) ygzb_host_free(h_map_);
     }
     // order[i] = the caller's index of tracker stream i (images, depth maps, trajectory rows); identity unless set
     void set_order(const std::vector<int>& order) { order_ = order; }
@@ -621,6 +734,9 @@ class Engine {
         CHK(ygzb_get_params(ctx_, &cp));
         W_ = cp.image_width;
         H_ = cp.image_height;
+        int rows = 0, cols = 0;
+        CHK(ygzb_grid_dims(ctx_, &rows, &cols));
+        ring_cells_ = (size_t)YGZB_TRACK_RING * rows * cols;
         // slots: S*F frame slots, S*RING key-frame slots, then (previous-frame reference) one reference slot per stream
         const bool prev = prm_.ref_mode == YGZB_TRACK_REF_PREVIOUS;
         CHK(ygzb_frames_create(ctx_, S_ * F_ + S_ * YGZB_TRACK_RING + (prev ? S_ : 0), &fr_));
@@ -689,14 +805,10 @@ class Engine {
         traj_frames_ = n_frames;
         collect_ = collect;
     }
+    // the oldest results, at most `capacity` of them (ygz_vo_poll: their rows and records are discarded)
     size_t pop_results(ygz_vo_result* out, size_t capacity) {
         const size_t n = std::min(capacity, results_.size());
-        for (size_t k = 0; k < n; ++k) {
-            out[k] = results_.front();
-            results_.pop_front();
-            if (observations()) drop_rows(1);   // (ygz_vo_poll: the rows go with their result)
-            if (information()) info_.pop_front();
-        }
+        results_.take(n, nullptr, [&](size_t k, const Result& r) { out[k] = r.r; });
         return n;
     }
     // whole results, oldest first, with their information records (info; NULL: discarded) and, with observations on,
@@ -704,31 +816,11 @@ class Engine {
     // one's rows do not.  n_obs is only touched with observations on
     int pop_results(ygz_vo_result* out, int capacity, int* n, ygzb_pose_information* info, ygzb_observation* obs, size_t obs_capacity,
                     size_t* n_obs) {
-        *n = 0;
-        const bool rows = observations();
-        size_t used = 0;
-        if (rows) {
-            *n_obs = 0;
-            if (capacity > 0 && !results_.empty() && row_count_.front() > obs_capacity) {
-                *n_obs = row_count_.front();
-                return YGZB_ERR_CAPACITY;
-            }
-            while (*n < capacity && *n < (int)results_.size() && used + row_count_[*n] <= obs_capacity) used += row_count_[(*n)++];
-            if (used) std::memcpy(obs, rows_.data() + rows_head_, used * sizeof(ygzb_observation));
-        } else {
-            *n = std::min(capacity, (int)results_.size());
-        }
-        std::copy(results_.begin(), results_.begin() + *n, out);
-        results_.erase(results_.begin(), results_.begin() + *n);
-        if (information()) {
-            if (info) std::copy(info_.begin(), info_.begin() + *n, info);
-            info_.erase(info_.begin(), info_.begin() + *n);
-        }
-        if (rows) {
-            drop_rows(*n);
-            *n_obs = used;
-        }
-        return YGZB_OK;
+        size_t no_rows;
+        return results_.take_whole(capacity, n, obs, obs_capacity, observations() ? n_obs : &no_rows, [&](size_t k, const Result& r) {
+            out[k] = r.r;
+            if (info) info[k] = r.info;
+        });
     }
     // nothing queued, no key-frame insertion pending, no result or map update waiting to be polled
     bool idle() const {
@@ -736,125 +828,23 @@ class Engine {
             if (!s.queue.empty()) return false;
         return kjobs_.empty() && results_.empty() && updates_.empty();
     }
-    bool observations() const { return h_obs_ != nullptr; }
-    bool information() const { return h_info_ != nullptr; }
-    bool map_updates() const { return h_map_ != nullptr; }
+    bool observations() const { return obs_.on(); }
+    bool information() const { return info_.on(); }
+    bool map_updates() const { return map_.on(); }
     // whole map updates with their rows, oldest first, while both fit; YGZB_ERR_CAPACITY with *n = 0 and *n_rows = its row
     // count when the first one's rows do not
     int pop_map_updates(ygz_vo_map_update* out, int capacity, int* n, ygzb_map_point* rows, size_t row_capacity, size_t* n_rows) {
-        *n = 0;
-        *n_rows = 0;
-        auto count = [](const ygz_vo_map_update& u) { return (size_t)u.n_moved + (size_t)u.n_new; };
-        if (capacity > 0 && !updates_.empty() && count(updates_.front()) > row_capacity) {
-            *n_rows = count(updates_.front());
-            return YGZB_ERR_CAPACITY;
-        }
-        size_t used = 0;
-        while (*n < capacity && *n < (int)updates_.size() && used + count(updates_[*n]) <= row_capacity) used += count(updates_[(*n)++]);
-        if (used) std::memcpy(rows, map_rows_.data() + map_head_, used * sizeof(ygzb_map_point));
-        std::copy(updates_.begin(), updates_.begin() + *n, out);
-        updates_.erase(updates_.begin(), updates_.begin() + *n);
-        map_head_ += used;
-        if (map_head_ == map_rows_.size()) {   // (one buffer keeps its capacity across rounds, as the observation rows')
-            map_rows_.clear();
-            map_head_ = 0;
-        } else if (map_head_ > map_rows_.size() / 2) {
-            map_rows_.erase(map_rows_.begin(), map_rows_.begin() + (ptrdiff_t)map_head_);
-            map_head_ = 0;
-        }
-        *n_rows = used;
-        return YGZB_OK;
+        return updates_.take_whole(capacity, n, rows, row_capacity, n_rows, [&](size_t k, const ygz_vo_map_update& u) { out[k] = u; });
     }
-    // the rows of the k oldest results have been polled: one buffer keeps its capacity across rounds, so a round neither
-    // allocates nor touches fresh pages once it has grown
-    void drop_rows(size_t k) {
-        for (size_t q = 0; q < k; ++q) {
-            rows_head_ += row_count_.front();
-            row_count_.pop_front();
-        }
-        if (rows_head_ == rows_.size()) {
-            rows_.clear();
-            rows_head_ = 0;
-        } else if (rows_head_ > rows_.size() / 2) {
-            rows_.erase(rows_.begin(), rows_.begin() + (ptrdiff_t)rows_head_);
-            rows_head_ = 0;
-        }
-    }
-    // on: every result from here on carries the observation rows of its frame (the tracker writes each job's rows into a
-    // page-locked buffer, allocated here: max_jobs * YGZB_TRACK_RING * cells rows); off: none, and the buffer is freed.
-    // Call only when idle()
-    int set_observations(bool on) {
-        if (on == observations()) return YGZB_OK;
-        if (!on) {
-            CHK(ygzb_tracker_set_observations(tr_, nullptr, 0));
-            CHK(ygzb_synchronize(ctx_));
-            ygzb_host_free(h_obs_);
-            h_obs_ = nullptr;
-            return YGZB_OK;
-        }
-        int rows = 0, cols = 0;
-        CHK(ygzb_grid_dims(ctx_, &rows, &cols));
-        obs_stride_ = (size_t)YGZB_TRACK_RING * rows * cols;
-        const size_t cap = (size_t)S_ * F_ * obs_stride_;
-        void* p = nullptr;
-        CHK(ygzb_host_alloc(&p, cap * sizeof(ygzb_observation)));
-        const int rc = ygzb_tracker_set_observations(tr_, static_cast<ygzb_observation*>(p), cap);
-        if (rc != YGZB_OK) {
-            ygzb_host_free(p);
-            return rc;
-        }
-        h_obs_ = static_cast<ygzb_observation*>(p);
-        return YGZB_OK;
-    }
-    // on: every result from here on carries the information record of its frame (the tracker writes each job's record
-    // into a page-locked buffer, allocated here: max_jobs records); off: none, and the buffer is freed.  Call only when
-    // idle()
-    int set_information(bool on) {
-        if (on == information()) return YGZB_OK;
-        if (!on) {
-            CHK(ygzb_tracker_set_information(tr_, nullptr, 0));
-            CHK(ygzb_synchronize(ctx_));
-            ygzb_host_free(h_info_);
-            h_info_ = nullptr;
-            return YGZB_OK;
-        }
-        const size_t cap = (size_t)S_ * F_;
-        void* p = nullptr;
-        CHK(ygzb_host_alloc(&p, cap * sizeof(ygzb_pose_information)));
-        const int rc = ygzb_tracker_set_information(tr_, static_cast<ygzb_pose_information*>(p), cap);
-        if (rc != YGZB_OK) {
-            ygzb_host_free(p);
-            return rc;
-        }
-        h_info_ = static_cast<ygzb_pose_information*>(p);
-        return YGZB_OK;
-    }
-    // on: every key-frame insertion from here on queues its map update (the tracker writes each key-frame job's rows into a
-    // page-locked buffer, allocated here: n_streams * YGZB_TRACK_RING * cells rows); off: none, and the buffer is freed.
-    // Call only when idle()
-    int set_map_updates(bool on) {
-        if (on == map_updates()) return YGZB_OK;
-        if (!on) {
-            CHK(ygzb_tracker_set_map_updates(tr_, nullptr, 0));
-            CHK(ygzb_synchronize(ctx_));
-            ygzb_host_free(h_map_);
-            h_map_ = nullptr;
-            return YGZB_OK;
-        }
-        int rows = 0, cols = 0;
-        CHK(ygzb_grid_dims(ctx_, &rows, &cols));
-        map_stride_ = (size_t)YGZB_TRACK_RING * rows * cols;
-        const size_t cap = (size_t)S_ * map_stride_;
-        void* p = nullptr;
-        CHK(ygzb_host_alloc(&p, cap * sizeof(ygzb_map_point)));
-        const int rc = ygzb_tracker_set_map_updates(tr_, static_cast<ygzb_map_point*>(p), cap);
-        if (rc != YGZB_OK) {
-            ygzb_host_free(p);
-            return rc;
-        }
-        h_map_ = static_cast<ygzb_map_point*>(p);
-        return YGZB_OK;
-    }
+    // on: every result from here on carries the observation rows of its frame (max_jobs * YGZB_TRACK_RING * cells rows
+    // for the tracker); off: none.  Call only when idle()
+    int set_observations(bool on) { return obs_.set(ctx_, tr_, ygzb_tracker_set_observations, on, (size_t)S_ * F_, ring_cells_); }
+    // on: every result from here on carries the information record of its frame (max_jobs records for the tracker); off:
+    // none.  Call only when idle()
+    int set_information(bool on) { return info_.set(ctx_, tr_, ygzb_tracker_set_information, on, (size_t)S_ * F_, 1); }
+    // on: every key-frame insertion from here on queues its map update (n_streams * YGZB_TRACK_RING * cells rows for the
+    // tracker); off: none.  Call only when idle()
+    int set_map_updates(bool on) { return map_.set(ctx_, tr_, ygzb_tracker_set_map_updates, on, (size_t)S_, ring_cells_); }
 
     // Batch feed: queues frames [queued, limit) of every stream from the stacked sequences images[caller stream] (with the
     // depth map of init) and runs until they all have their result and nothing is in flight.
@@ -887,9 +877,10 @@ class Engine {
             StageTimer tm(kTLocalBA);
             for (size_t q = 0; q < kjobs_.size(); ++q) {   // bookkeeping that does not need the device's answer
                 EStream& s = st_[kjobs_[q].stream];
+                const KfFrame& f = kframes_[q].rec;
                 KfInfo kf;
                 kf.entry = kjobs_[q].entry;
-                kf.frame_id = kframes_[q].frame;
+                kf.frame_id = f.frame;
                 kf.mp0 = kjobs_[q].mp0;
                 kf.T = s.T;
                 s.kfs.push_back(kf);
@@ -897,8 +888,8 @@ class Engine {
                 s.frames_since_kf = 0;
                 s.n_keyframes += 1;
                 // the key-frame's own depth map: on the context stream like the insertion, so it lands just before it
-                if (kframes_[q].depth) {
-                    CHK(ygzb_tracker_set_depth(tr_, kjobs_[q].stream, kframes_[q].depth));
+                if (f.depth) {
+                    CHK(ygzb_tracker_set_depth(tr_, kjobs_[q].stream, f.depth));
                     h2d_other_bytes += (long long)W_ * H_ * (long long)sizeof(double);
                 }
                 // a sequence's first key-frame starts at the pose its frame was pushed with
@@ -974,13 +965,12 @@ class Engine {
                 const double kbar = r.ba_points ? (double)r.ba_observations / r.ba_points : 0.0, dim = 6.0 * (kj.n_local - 1);
                 s.ba_flops += r.ba_trials * (300.0 * r.ba_observations + r.ba_points * (216.0 * kbar * kbar + 108.0 * kbar + 50.0) + dim * dim * dim / 3.0);
             }
-            emit(kj.stream, kframes_[q].frame, kframes_[q].tag, YGZ_VO_KEYFRAME, kframes_[q].n_inliers, kf_rows_.data() + kframes_[q].obs0,
-                 kframes_[q].n_obs, &kframes_[q].info);
-            if (map_updates()) queue_map_update(kj, r, h_map_ + q * map_stride_);
+            const auto& kf = kframes_[0];
+            emit(kj.stream, kf.rec.frame, kf.rec.tag, YGZ_VO_KEYFRAME, kf.rec.n_inliers, {kframes_.front_rows(), kf.n_rows, &kf.rec.info});
+            kframes_.drop(1);
+            if (map_updates()) queue_map_update(kj, r, map_.job(q));
         }
         kjobs_.clear();
-        kframes_.clear();
-        kf_rows_.clear();
         // ---- 4. results of the tracking batch
         for (const Win& b : wins_) {
             EStream& s = st_[b.stream];
@@ -1001,8 +991,9 @@ class Engine {
                 continue;
             }
             for (int t = 0; t < b.count; ++t) {
-                const ygzb_track_result& r = h_res_[b.job0 + t];
-                const ygzb_observation* rows = job_rows(b.job0 + t);   // (exactly r.n_inliers of them)
+                const int j = b.job0 + t;
+                const ygzb_track_result& r = h_res_[j];
+                const Attachments a{obs_.job(j), obs_.on() ? (size_t)r.n_inliers : 0, info_.job(j)};   // (the tracker wrote r.n_inliers rows)
                 if (!r.aligned) {   // Matcher::SparseImageAlignment returned false (Matcher.cpp:482-488)
                     s.lost = true;
                     emit_front(b.stream, YGZ_VO_LOST, 0);
@@ -1012,17 +1003,17 @@ class Engine {
                 s.n_projected += r.n_projected;
                 if (r.n_inliers < prm_.min_inliers) {
                     s.lost = true;
-                    emit_front(b.stream, YGZ_VO_LOST, r.n_inliers, rows);
+                    emit_front(b.stream, YGZ_VO_LOST, r.n_inliers, {a.rows, a.n_rows});
                     break;
                 }
                 std::memcpy(s.T.m, r.T_cw, sizeof(s.T.m));
                 s.frames_since_kf += 1;
                 s.n_inliers += r.n_inliers;
                 if (need_keyframe(prm_, s.frames_since_kf, s.T, s.kfs.back().T)) {
-                    pend_keyframe(b.stream, b.stream * F_ + t, b.job0 + t, r.n_inliers, rows, job_info(b.job0 + t));
+                    pend_keyframe(b.stream, b.stream * F_ + t, j, r.n_inliers, a);
                     break;   // frames of the window behind the key-frame (speculative ones) stay queued: tracked again next round
                 }
-                emit_front(b.stream, YGZ_VO_TRACKED, r.n_inliers, rows, job_info(b.job0 + t));
+                emit_front(b.stream, YGZ_VO_TRACKED, r.n_inliers, a);
             }
         }
         wins_.clear();
@@ -1110,56 +1101,42 @@ class Engine {
         for (int k = 0; k < kj.n_local; ++k) std::memcpy(u.T_cw[k], r.T_cw[k], sizeof(u.T_cw[k]));
         u.n_moved = r.ba_points;
         u.n_new = r.n_features;
-        map_rows_.insert(map_rows_.end(), rows, rows + (size_t)u.n_moved + (size_t)u.n_new);
-        updates_.push_back(u);
+        updates_.push(u, rows, (size_t)u.n_moved + (size_t)u.n_new);
     }
-    // observation rows of job j of the tracking batch that has just come back (observations on), else NULL
-    const ygzb_observation* job_rows(int j) const { return h_obs_ ? h_obs_ + (size_t)j * obs_stride_ : nullptr; }
-    // information record of job j of the tracking batch that has just come back (information on), else NULL
-    const ygzb_pose_information* job_info(int j) const { return h_info_ ? h_info_ + j : nullptr; }
     // the stream's oldest queued frame becomes a key-frame: its insertion is enqueued at the start of the next round, its
-    // result is emitted once the insertion's local BA has come back; its n_inliers observation rows (rows: its tracking
-    // job's, or NULL) and its tracking job's information record (info, or NULL: zeros) are held with it until then, since
-    // the next round's batch reuses the buffers
-    void pend_keyframe(int stream, int frame_slot, int track_job, int n_inliers, const ygzb_observation* rows = nullptr,
-                       const ygzb_pose_information* info = nullptr) {
+    // result is emitted once the insertion's local BA has come back; its tracking job's attachments are held with it until
+    // then, since the next round's batch reuses the buffers
+    void pend_keyframe(int stream, int frame_slot, int track_job, int n_inliers, const Attachments& a = {}) {
         EStream& s = st_[stream];
         const QFrame f = s.queue.front();
         s.queue.pop_front();
         kjobs_.push_back(make_kf_job(stream, frame_slot, track_job));
-        const size_t n_rows = rows ? (size_t)n_inliers : 0;
-        kframes_.push_back({s.next_frame++, n_inliers, f.tag, f.depth, kf_rows_.size(), n_rows, info ? *info : ygzb_pose_information{}});
-        if (n_rows) kf_rows_.insert(kf_rows_.end(), rows, rows + n_rows);
+        kframes_.push({s.next_frame++, n_inliers, f.tag, f.depth, a.info ? *a.info : ygzb_pose_information{}}, a.rows, a.n_rows);
     }
-    // the stream's oldest queued frame is final with the stream's current pose; rows: its n_inliers observation rows, or NULL;
-    // info: its information record, or NULL (zeros)
-    void emit_front(int stream, int status, int n_inliers, const ygzb_observation* rows = nullptr, const ygzb_pose_information* info = nullptr) {
+    // the stream's oldest queued frame is final with the stream's current pose
+    void emit_front(int stream, int status, int n_inliers, const Attachments& a = {}) {
         EStream& s = st_[stream];
         const int64_t tag = s.queue.front().tag;
         s.queue.pop_front();
-        emit(stream, s.next_frame++, tag, status, n_inliers, rows, rows ? (size_t)n_inliers : 0, info);
+        emit(stream, s.next_frame++, tag, status, n_inliers, a);
     }
-    void emit(int stream, int frame, int64_t tag, int status, int n_inliers, const ygzb_observation* rows = nullptr, size_t n_rows = 0,
-              const ygzb_pose_information* info = nullptr) {
+    void emit(int stream, int frame, int64_t tag, int status, int n_inliers, const Attachments& a) {
         const EStream& s = st_[stream];
         if (traj_) {
             double* out = traj_ + ((size_t)order_[stream] * traj_frames_ + frame) * 12;
             for (int c = 0; c < 12; ++c) out[c] = s.has_pose ? s.T.m[c] : NAN;
         }
         if (collect_) {
-            ygz_vo_result r{};
+            Result res{};
+            ygz_vo_result& r = res.r;
             r.stream = order_[stream];
             r.frame = frame;
             r.tag = tag;
             r.status = status;
             r.n_inliers = n_inliers;
             std::memcpy(r.T_cw, s.T.m, sizeof(r.T_cw));
-            results_.push_back(r);
-            if (observations()) {
-                if (n_rows) rows_.insert(rows_.end(), rows, rows + n_rows);
-                row_count_.push_back(n_rows);
-            }
-            if (information()) info_.push_back(info ? *info : ygzb_pose_information{});
+            if (a.info) res.info = *a.info;
+            results_.push(res, a.rows, a.n_rows);
         }
     }
     ygzb_keyframe_job make_kf_job(int stream, int frame_slot, int track_job) const {
@@ -1199,30 +1176,20 @@ class Engine {
     ygzb_ba_params ba_;
     std::vector<Win> wins_;
     std::vector<ygzb_keyframe_job> kjobs_;   // key-frame insertions for the next round ...
-    std::vector<KfFrame> kframes_;           // ... and their frames
+    RowQueue<KfFrame, ygzb_observation> kframes_;   // ... and their frames, with their observation rows
     std::vector<int> order_;
     std::vector<Camera> tr_cam_;   // the tracker's camera of every stream (ygzb_tracker_set_camera), as last set
     double* traj_ = nullptr;
     int traj_frames_ = 0;
     bool collect_ = false;
-    std::deque<ygz_vo_result> results_;
-    // observations (set_observations): the tracker's page-locked rows, obs_stride_ rows per job; the rows of the results
-    // in results_, back to back from rows_head_ (row_count_: how many each); the rows of the pending key-frames
-    ygzb_observation* h_obs_ = nullptr;
-    size_t obs_stride_ = 0;
-    std::vector<ygzb_observation> rows_, kf_rows_;
-    size_t rows_head_ = 0;
-    std::deque<size_t> row_count_;
-    // information (set_information): the tracker's page-locked records, one per job; the records of the results in results_
-    ygzb_pose_information* h_info_ = nullptr;
-    std::deque<ygzb_pose_information> info_;
-    // map updates (set_map_updates): the tracker's page-locked rows, map_stride_ rows per key-frame job; the updates waiting
-    // to be polled, their rows back to back from map_head_
-    ygzb_map_point* h_map_ = nullptr;
-    size_t map_stride_ = 0;
-    std::deque<ygz_vo_map_update> updates_;
-    std::vector<ygzb_map_point> map_rows_;
-    size_t map_head_ = 0;
+    RowQueue<Result, ygzb_observation> results_;   // final results waiting to be polled, with their observation rows
+    RowQueue<ygz_vo_map_update, ygzb_map_point> updates_;   // map updates waiting to be polled, with their rows
+    // the tracker's page-locked outputs: observation rows (set_observations), information records (set_information) and
+    // map rows (set_map_updates)
+    size_t ring_cells_ = 0;   // YGZB_TRACK_RING * cells: the rows of a tracking job or a key-frame job
+    PinnedOutput<ygzb_observation> obs_;
+    PinnedOutput<ygzb_pose_information> info_;
+    PinnedOutput<ygzb_map_point> map_;
     bool blocking_sync_ = false;
 };
 

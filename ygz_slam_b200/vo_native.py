@@ -3,6 +3,7 @@ vo.VisualOdometry with the GPU backend, used by bench.py for BASELINE config C5 
 from __future__ import annotations
 
 import ctypes as C
+from operator import itemgetter
 from pathlib import Path
 
 import numpy as np
@@ -252,15 +253,14 @@ class Engine:
         ctx.check(self.lib.ygz_vo_create(ctx.h, C.byref(self.cfg), C.byref(self.h)), "ygz_vo_create")
         self._pushed = [0] * self.n_streams
         self._alive = {}   # (stream, frame) -> the arrays its result still needs
+        self._rows = {}   # row dtype -> the row buffer of one poll call, grown on demand
         self.observations = False
-        self._obs = np.zeros(0, OBS_DTYPE)   # rows of one ygz_vo_poll_observations call, grown on demand
         if observations:
             self.set_observations(True)
         self.information = False
         if information:
             self.set_information(True)
         self.map_updates = False
-        self._map_rows = np.zeros(0, MAP_POINT_DTYPE)   # rows of one ygz_vo_poll_map_updates call, grown on demand
         if map_updates:
             self.set_map_updates(True)
         if cameras is not None:
@@ -300,30 +300,47 @@ class Engine:
         self.ctx.check(self.lib.ygz_vo_set_map_updates(self.h, int(bool(on))), "ygz_vo_set_map_updates")
         self.map_updates = bool(on)
 
+    def _drain(self, call, name, capacity, dtypes, row_dtype=None, row_count=None):
+        """Polls until nothing is left: call(records, n, rows, row_capacity, n_rows) gets one array of `capacity` records per
+        dtype in `dtypes` and the row buffer (None and 0 without a row dtype), and returns the C status; YGZB_ERR_CAPACITY
+        (the next record's rows do not fit) grows the row buffer and asks again.  Returns the records, one array per dtype,
+        and with a row dtype the rows, one array per record of row_count(records[0]) rows."""
+        recs, rows = [[] for _ in dtypes], []
+        while True:
+            bufs = [np.zeros(capacity, dt) for dt in dtypes]
+            n, n_rows = C.c_int(0), C.c_size_t(0)
+            if row_dtype is None:
+                rc = call(bufs, C.byref(n), None, 0, C.byref(n_rows))
+            else:
+                buf = self._rows.get(row_dtype)
+                if buf is None:
+                    buf = self._rows[row_dtype] = np.zeros(4 * 4096, row_dtype)
+                rc = call(bufs, C.byref(n), buf.ctypes.data, len(buf), C.byref(n_rows))
+                if rc == _ERR_CAPACITY:
+                    self._rows[row_dtype] = np.zeros(max(2 * len(buf), n_rows.value), row_dtype)
+                    continue
+            self.ctx.check(rc, name)
+            if n.value == 0:
+                break
+            for r, b in zip(recs, bufs):
+                r.append(b[:n.value])
+            if row_dtype is None and n.value < capacity:   # (without rows, a short answer has drained the queue)
+                break
+            if row_dtype is not None:
+                ends = np.cumsum(row_count(bufs[0][:n.value]))
+                assert ends[-1] == n_rows.value
+                rows.extend(np.split(buf[:n_rows.value].copy(), ends[:-1]))
+        return [np.concatenate(r) if r else np.zeros(0, dt) for r, dt in zip(recs, dtypes)], rows
+
     def poll_map_updates(self, capacity=256):
         """Map updates since the last call, oldest first: (updates, rows) -- a MAP_UPDATE_DTYPE array and, per update, a
         MAP_POINT_DTYPE array of its n_moved rows (the local BA's points) followed by its n_new rows (the new key-frame's
         points).  Independent of poll: results and updates have queues of their own."""
-        out, rows = [], []
-        if len(self._map_rows) == 0:
-            self._map_rows = np.zeros(4 * 4096, MAP_POINT_DTYPE)
-        while True:
-            buf = np.zeros(capacity, MAP_UPDATE_DTYPE)
-            n, n_rows = C.c_int(0), C.c_size_t(0)
-            rc = self.lib.ygz_vo_poll_map_updates(self.h, buf.ctypes.data, capacity, C.byref(n), self._map_rows.ctypes.data,
-                                                  len(self._map_rows), C.byref(n_rows))
-            if rc == _ERR_CAPACITY:   # the next update's rows do not fit: grow the row buffer and ask again
-                self._map_rows = np.zeros(max(2 * len(self._map_rows), n_rows.value), MAP_POINT_DTYPE)
-                continue
-            self.ctx.check(rc, "ygz_vo_poll_map_updates")
-            if n.value == 0:
-                break
-            upd = buf[:n.value]
-            ends = np.cumsum(upd["n_moved"].astype(np.int64) + upd["n_new"])
-            assert ends[-1] == n_rows.value
-            out.append(upd)
-            rows.extend(np.split(self._map_rows[:n_rows.value].copy(), ends[:-1]))
-        return (np.concatenate(out) if out else np.zeros(0, MAP_UPDATE_DTYPE)), rows
+        lib, h = self.lib, self.h
+        (upd,), rows = self._drain(lambda out, n, *r: lib.ygz_vo_poll_map_updates(h, out[0].ctypes.data, capacity, n, *r),
+                                   "ygz_vo_poll_map_updates", capacity, (MAP_UPDATE_DTYPE,), MAP_POINT_DTYPE,
+                                   lambda u: u["n_moved"].astype(np.int64) + u["n_new"])
+        return upd, rows
 
     def push(self, stream, image, depth=None, tag=None):
         """Queue grey `image` (H, W) uint8 of `stream` with its depth map (H, W) float64, or None to keep the stream's current
@@ -362,75 +379,26 @@ class Engine:
         observations on, (results, rows): rows[k] is an OBS_DTYPE array of result k's n_inliers observations.  With
         information on, (results, info) or (results, rows, info): info[k] = [alignment Fisher, pose information] of
         result k, [n, 2, 6, 6] (zeros for a sequence's first key-frame and for LOST results)."""
+        lib, h, obs = self.lib, self.h, self.observations
+        row_dtype, n_inliers = (OBS_DTYPE if obs else None), itemgetter("n_inliers")
         if self.information:
-            return self._poll_ex(capacity)
-        if self.observations:
-            return self._poll_observations(capacity)
-        out = []
-        while True:
-            buf = np.zeros(capacity, RESULT_DTYPE)
-            n = C.c_int(0)
-            self.ctx.check(self.lib.ygz_vo_poll(self.h, buf.ctypes.data, capacity, C.byref(n)), "ygz_vo_poll")
-            out.append(buf[:n.value])
-            if n.value < capacity:
-                break
-        return self._release(np.concatenate(out))
+            (res, info), rows = self._drain(
+                lambda out, n, *r: lib.ygz_vo_poll_ex(h, out[0].ctypes.data, capacity, n, out[1].ctypes.data, *r), "ygz_vo_poll_ex",
+                capacity, (RESULT_DTYPE, INFO_DTYPE), row_dtype, n_inliers)
+            full = np.stack([unpack_sym6(info["align_fisher"]), unpack_sym6(info["pose_info"])], axis=1)
+            return (self._release(res), rows, full) if obs else (self._release(res), full)
+        if obs:
+            (res,), rows = self._drain(lambda out, n, *r: lib.ygz_vo_poll_observations(h, out[0].ctypes.data, capacity, n, *r),
+                                       "ygz_vo_poll_observations", capacity, (RESULT_DTYPE,), row_dtype, n_inliers)
+            return self._release(res), rows
+        (res,), _ = self._drain(lambda out, n, *r: lib.ygz_vo_poll(h, out[0].ctypes.data, capacity, n), "ygz_vo_poll", capacity,
+                                (RESULT_DTYPE,))
+        return self._release(res)
 
     def _release(self, res):
         for s_, f in zip(res["stream"].tolist(), res["frame"].tolist()):
             self._alive.pop((s_, f), None)
         return res
-
-    def _poll_observations(self, capacity):
-        out, rows = [], []
-        if len(self._obs) == 0:
-            self._obs = np.zeros(4 * 4096, OBS_DTYPE)
-        while True:
-            buf = np.zeros(capacity, RESULT_DTYPE)
-            n, n_obs = C.c_int(0), C.c_size_t(0)
-            rc = self.lib.ygz_vo_poll_observations(self.h, buf.ctypes.data, capacity, C.byref(n), self._obs.ctypes.data, len(self._obs),
-                                                   C.byref(n_obs))
-            if rc == _ERR_CAPACITY:   # the next result's rows do not fit: grow the row buffer and ask again
-                self._obs = np.zeros(max(2 * len(self._obs), n_obs.value), OBS_DTYPE)
-                continue
-            self.ctx.check(rc, "ygz_vo_poll_observations")
-            if n.value == 0:
-                break
-            res = buf[:n.value]
-            ends = np.cumsum(res["n_inliers"])
-            assert ends[-1] == n_obs.value
-            out.append(res)
-            rows.extend(np.split(self._obs[:n_obs.value].copy(), ends[:-1]))
-        res = np.concatenate(out) if out else np.zeros(0, RESULT_DTYPE)
-        return self._release(res), rows
-
-    def _poll_ex(self, capacity):
-        out, rows, infos = [], [], []
-        if self.observations and len(self._obs) == 0:
-            self._obs = np.zeros(4 * 4096, OBS_DTYPE)
-        while True:
-            buf = np.zeros(capacity, RESULT_DTYPE)
-            info = np.zeros(capacity, INFO_DTYPE)
-            n, n_obs = C.c_int(0), C.c_size_t(0)
-            obs, obs_cap = (self._obs.ctypes.data, len(self._obs)) if self.observations else (None, 0)
-            rc = self.lib.ygz_vo_poll_ex(self.h, buf.ctypes.data, capacity, C.byref(n), info.ctypes.data, obs, obs_cap, C.byref(n_obs))
-            if rc == _ERR_CAPACITY:   # the next result's rows do not fit: grow the row buffer and ask again
-                self._obs = np.zeros(max(2 * len(self._obs), n_obs.value), OBS_DTYPE)
-                continue
-            self.ctx.check(rc, "ygz_vo_poll_ex")
-            if n.value == 0:
-                break
-            res = buf[:n.value]
-            out.append(res)
-            infos.append(info[:n.value])
-            if self.observations:
-                ends = np.cumsum(res["n_inliers"])
-                assert ends[-1] == n_obs.value
-                rows.extend(np.split(self._obs[:n_obs.value].copy(), ends[:-1]))
-        res = self._release(np.concatenate(out) if out else np.zeros(0, RESULT_DTYPE))
-        info = np.concatenate(infos) if infos else np.zeros(0, INFO_DTYPE)
-        full = np.stack([unpack_sym6(info["align_fisher"]), unpack_sym6(info["pose_info"])], axis=1)
-        return (res, rows, full) if self.observations else (res, full)
 
     def _stat_row(self, stream):
         row = np.zeros(16, np.int64)
