@@ -491,6 +491,21 @@ int ygzb_tracker_set_camera(ygzb_tracker* t, int stream, const double K[4]);
  * but on the tracker's second CUDA stream: behind the last key-frame insertion and tracking chain (which still read the
  * slots), concurrent with a local BA in flight.  ygzb_tracker_track orders itself behind these uploads.              */
 int ygzb_tracker_upload(ygzb_tracker* t, int first, int count, const uint8_t* host, size_t frame_stride);
+/* undistortion maps of `stream` (the format of ygzb_frames_set_undistort: image_width x image_height entries, host or
+ * device memory), so that the streams of one tracker may come from different lenses; map_xy == map_a == NULL clears
+ * them.  They apply to the frames ygzb_tracker_upload_stream uploads for `stream`: level 0 becomes the remap of the raw
+ * grey frame, bit for bit as with the pool's maps, and the stream's camera (ygzb_tracker_set_camera) and depth maps are
+ * the undistorted camera's.  Ordered like an upload, on the tracker's second CUDA stream: the uploads enqueued before the
+ * call read the old maps, those enqueued after it the new ones; it waits for no key-frame insertion or local BA.  The
+ * call returns once the maps have been read (a device buffer of 6 bytes per pixel per stream, allocated on the stream's
+ * first maps and kept until ygzb_tracker_destroy).  YGZB_ERR_INVALID, with the stream's maps unchanged, for a NULL
+ * tracker, a stream out of range, only one of the two pointers, an entry map_a >= 1024, or maps on the frame pool
+ * (ygzb_frames_set_undistort): a pool's maps and a stream's are never combined.                                       */
+int ygzb_tracker_set_undistort(ygzb_tracker* t, int stream, const int16_t* map_xy, const uint16_t* map_a);
+/* ygzb_tracker_upload of frames of `stream`: with maps set for the stream (ygzb_tracker_set_undistort), level 0 is
+ * remapped through them; without, it is exactly ygzb_tracker_upload.  YGZB_ERR_INVALID for a NULL tracker, a stream out
+ * of range, the arguments ygzb_tracker_upload refuses, or a stream with maps on a frame pool that has maps too.       */
+int ygzb_tracker_upload_stream(ygzb_tracker* t, int stream, int first, int count, const uint8_t* host, size_t frame_stride);
 /* asynchronous: enqueues the chain on the context's stream and a copy of the n_jobs result records into `results`
  * (host memory, page-locked for a truly asynchronous copy); valid after ygzb_synchronize(ctx).                    */
 int ygzb_tracker_track(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, ygzb_track_result* results);

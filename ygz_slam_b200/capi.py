@@ -47,6 +47,7 @@ EXPORTS = [
     "ygzb_tracker_export_reference", "ygzb_tracker_import_reference", "ygzb_undistort_map", "ygzb_frames_set_undistort",
     "ygzb_tracker_set_start_pose", "ygzb_tracker_get_depth", "ygzb_tracker_set_observations",
     "ygzb_sparse_align_fisher", "ygzb_tracker_set_information", "ygzb_tracker_set_map_updates", "ygzb_tracker_set_camera",
+    "ygzb_tracker_set_undistort", "ygzb_tracker_upload_stream",
 ]
 
 
@@ -888,6 +889,8 @@ class Tracker:
         self.lib.ygzb_tracker_set_start_pose.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         self.lib.ygzb_tracker_set_camera.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         self.lib.ygzb_tracker_upload.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
+        self.lib.ygzb_tracker_set_undistort.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+        self.lib.ygzb_tracker_upload_stream.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
         self.lib.ygzb_tracker_track.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         self.lib.ygzb_tracker_make_keyframes.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         self.lib.ygzb_tracker_debug_job.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
@@ -986,6 +989,30 @@ class Tracker:
         """K = (fx, fy, cx, cy) of `stream` for every later job and key-frame insertion (ygzb_tracker_set_camera)."""
         K = np.ascontiguousarray(K, np.float64).reshape(4)
         self.ctx.check(self.lib.ygzb_tracker_set_camera(self.h, int(stream), _p(K)), "ygzb_tracker_set_camera")
+
+    def set_undistort(self, stream: int, map_xy=None, map_a=None):
+        """Undistortion maps of `stream` (ygzb_tracker_set_undistort), the format of Frames.set_undistort; no maps clear
+        them.  They apply to upload_stream of that stream."""
+        if map_xy is None and map_a is None:
+            self.ctx.check(self.lib.ygzb_tracker_set_undistort(self.h, int(stream), None, None), "ygzb_tracker_set_undistort")
+            return
+        f = self.frames
+        H, W = f.lh[0], f.lw[0]
+        map_xy = np.ascontiguousarray(map_xy, np.int16)
+        map_a = np.ascontiguousarray(map_a, np.uint16)
+        if map_xy.shape != (H, W, 2) or map_a.shape != (H, W):
+            raise ValueError(f"maps must be ({H}, {W}, 2) int16 and ({H}, {W}) uint16, not {map_xy.shape} and {map_a.shape}")
+        self.ctx.check(self.lib.ygzb_tracker_set_undistort(self.h, int(stream), _p(map_xy), _p(map_a)), "ygzb_tracker_set_undistort")
+
+    def upload_stream(self, stream: int, first: int, images):
+        """Raw grey frames (n, H, W) of `stream` into slots [first, first + n), remapped through the stream's maps if it
+        has any (ygzb_tracker_upload_stream)."""
+        images = np.ascontiguousarray(images, np.uint8)
+        if images.ndim == 2:
+            images = images[None]
+        self.ctx.check(self.lib.ygzb_tracker_upload_stream(self.h, int(stream), int(first), len(images), _p(images),
+                                                           C.c_size_t(images[0].size)), "ygzb_tracker_upload_stream")
+        self.ctx.synchronize()
 
     def upload(self, first: int, images):
         """Grey frames (n, H, W) into slots [first, first + n)."""

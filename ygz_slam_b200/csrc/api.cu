@@ -422,7 +422,7 @@ void* ygzb_frames_device_ptr(ygzb_frames* f) { return f ? f->d_pyr : nullptr; }
 int ygzb_frames_build_pyramid(ygzb_frames* f, int first, int count) {
     if (!f || first < 0 || count < 0 || first + count > f->capacity) return YGZB_ERR_INVALID;
     cudaSetDevice(f->ctx->device);
-    return launch_pyramid(f, first, count, nullptr, 1, false);
+    return launch_pyramid(f, first, count, nullptr, 1, nullptr, nullptr);
 }
 
 int ygzb_frames_copy(ygzb_frames* f, int src_slot, int dst_slot) {
@@ -454,11 +454,13 @@ int stage_frames(ygzb_ctx* ctx, uint8_t* dst, const uint8_t* src, int count, siz
     return YGZB_OK;
 }
 
-// undistorting upload: the raw frames go to the pool's staging buffer, remap_gray_kernel writes level 0.  The buffer is the
+// undistorting upload: the raw frames go to the pool's staging buffer, remap_gray_kernel writes level 0 through the maps
+// (the pool's, or a tracker stream's: ygzb_tracker_set_undistort).  The buffer is the
 // pool's own, not a context scratch buffer, because a tracker uploads on its front stream while the context's stream runs a
 // local BA; e_stage, recorded behind every remap on whichever stream ran it, orders each reuse of the buffer behind the
 // last read of it.
-int upload_undistorted(ygzb_frames* f, int first, int count, const uint8_t* src, int channels, size_t frame_stride) {
+int upload_undistorted(ygzb_frames* f, int first, int count, const uint8_t* src, int channels, size_t frame_stride, const short2* map_xy,
+                       const uint16_t* map_a) {
     ygzb_ctx* ctx = f->ctx;
     const Geometry& g = ctx->geo;
     const size_t frame = (size_t)g.lv[0].w * g.lv[0].h * channels, bytes = frame * count;
@@ -472,7 +474,7 @@ int upload_undistorted(ygzb_frames* f, int first, int count, const uint8_t* src,
     }
     YGZB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, f->e_stage, 0));
     int rc = stage_frames(ctx, f->d_stage, src, count, frame, frame_stride);
-    if (rc == YGZB_OK) rc = launch_pyramid(f, first, count, f->d_stage, channels, true);
+    if (rc == YGZB_OK) rc = launch_pyramid(f, first, count, f->d_stage, channels, map_xy, map_a);
     // recorded even after a failed launch: a copy into the buffer may be in flight
     const int rc_ev = check_cuda(ctx, cudaEventRecord(f->e_stage, ctx->stream), "cudaEventRecord");
     return rc != YGZB_OK ? rc : rc_ev;
@@ -480,7 +482,8 @@ int upload_undistorted(ygzb_frames* f, int first, int count, const uint8_t* src,
 
 }  // namespace
 
-int ygzb::frames_upload(ygzb_frames* f, int first, int count, const uint8_t* host, int channels, size_t frame_stride, bool undistort) {
+int ygzb::frames_upload(ygzb_frames* f, int first, int count, const uint8_t* host, int channels, size_t frame_stride, const short2* map_xy,
+                        const uint16_t* map_a) {
     if (!f || !host || first < 0 || count < 0 || first + count > f->capacity) return YGZB_ERR_INVALID;
     ygzb_ctx* ctx = f->ctx;
     const Geometry& g = ctx->geo;
@@ -489,7 +492,7 @@ int ygzb::frames_upload(ygzb_frames* f, int first, int count, const uint8_t* hos
     if (channels != 1 && channels != 3) return set_error(ctx, YGZB_ERR_INVALID, "channels must be 1 or 3");
     if (frame_stride < row * g.lv[0].h) return set_error(ctx, YGZB_ERR_INVALID, "frame_stride smaller than one image");
     if (count == 0) return YGZB_OK;
-    if (undistort && f->undistort) return upload_undistorted(f, first, count, host, channels, frame_stride);
+    if (map_xy) return upload_undistorted(f, first, count, host, channels, frame_stride, map_xy, map_a);
     // cudaMemcpyDefault: `host` may also be a device pointer (frames already resident in HBM, unified addressing).
     // A strided batch copy treats one image as a "row", so its pitch is limited (cudaDeviceProp::memPitch, 2^31 - 1):
     // longer strides (a stacked [stream][frame] array of thousands of frames) fall back to one copy per image.
@@ -505,7 +508,7 @@ int ygzb::frames_upload(ygzb_frames* f, int first, int count, const uint8_t* hos
                 YGZB_CUDA(ctx, cudaMemcpy2DAsync(dst + (size_t)i * ctx->slot_stride, g.lv[0].pitch, host + (size_t)i * frame_stride,
                                                  row, row, g.lv[0].h, cudaMemcpyDefault, ctx->stream));
         }
-        return launch_pyramid(f, first, count, nullptr, 1, false);
+        return launch_pyramid(f, first, count, nullptr, 1, nullptr, nullptr);
     }
     uint8_t* d_bgr = (uint8_t*)dev_scratch(ctx, 0, (size_t)count * row * g.lv[0].h);
     if (!d_bgr) return YGZB_ERR_CUDA;
@@ -517,13 +520,13 @@ int ygzb::frames_upload(ygzb_frames* f, int first, int count, const uint8_t* hos
             YGZB_CUDA(ctx, cudaMemcpyAsync(d_bgr + (size_t)i * row * g.lv[0].h, host + (size_t)i * frame_stride, row * g.lv[0].h,
                                            cudaMemcpyDefault, ctx->stream));
     }
-    return launch_pyramid(f, first, count, d_bgr, 3, false);
+    return launch_pyramid(f, first, count, d_bgr, 3, nullptr, nullptr);
 }
 
 extern "C" {
 
 int ygzb_frames_upload(ygzb_frames* f, int first, int count, const uint8_t* host, int channels, size_t frame_stride) {
-    return frames_upload(f, first, count, host, channels, frame_stride, true);
+    return f ? frames_upload(f, first, count, host, channels, frame_stride, f->undistort ? f->d_map_xy : nullptr, f->d_map_a) : YGZB_ERR_INVALID;
 }
 
 int ygzb_frames_set_undistort(ygzb_frames* f, const int16_t* map_xy, const uint16_t* map_a) {

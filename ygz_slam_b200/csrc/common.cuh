@@ -172,12 +172,14 @@ struct ProfScope {
 };
 
 // ---- stage launchers (one .cu each) -----------------------------------------------------------
-// d_src = raw frames staged on the device (`channels` 1 or 3) or null (level 0 already in the slots); remap: level 0 =
-// remap_gray_kernel of d_src through the pool's undistortion maps, otherwise d_src must be BGR (bgr2gray_kernel)
-int launch_pyramid(ygzb_frames* f, int first, int count, const uint8_t* d_src, int channels, bool remap);
-// ygzb_frames_upload; undistort = false skips the pool's undistortion maps (images that are undistorted already, e.g. the
-// key-frame and reference images of the tracker's records)
-int frames_upload(ygzb_frames* f, int first, int count, const uint8_t* host, int channels, size_t frame_stride, bool undistort);
+// d_src = raw frames staged on the device (`channels` 1 or 3) or null (level 0 already in the slots); map_xy != NULL: level
+// 0 = remap_gray_kernel of d_src through the undistortion maps map_xy / map_a, otherwise d_src must be BGR (bgr2gray_kernel)
+int launch_pyramid(ygzb_frames* f, int first, int count, const uint8_t* d_src, int channels, const short2* map_xy, const uint16_t* map_a);
+// ygzb_frames_upload through the undistortion maps map_xy / map_a (device memory, [H][W] each: the pool's or a tracker
+// stream's), or with none (map_xy == NULL: images that are undistorted already, e.g. the key-frame and reference images of
+// the tracker's records, or frames without a lens); a remap stages the raw frames in the pool's d_stage behind e_stage
+int frames_upload(ygzb_frames* f, int first, int count, const uint8_t* host, int channels, size_t frame_stride, const short2* map_xy,
+                  const uint16_t* map_a);
 int launch_pyrdown_ptrs(ygzb_ctx* ctx, const uint8_t* const* d_src_ptr, uint8_t* const* d_dst_ptr, int sw, int sh, int spitch,
                         int dw, int dh, int dpitch, int count);
 int launch_detect(ygzb_frames* f, int n, bool have_occupied);

@@ -312,20 +312,21 @@ __global__ void __launch_bounds__(256) remap_gray_kernel(const uint8_t* __restri
 
 }  // namespace
 
-int launch_pyramid(ygzb_frames* f, int first, int count, const uint8_t* d_src, int channels, bool remap) {
+int launch_pyramid(ygzb_frames* f, int first, int count, const uint8_t* d_src, int channels, const short2* map_xy, const uint16_t* map_a) {
     ygzb_ctx* ctx = f->ctx;
     const Geometry& g = ctx->geo;
     if (count <= 0) return YGZB_OK;
-    if (d_src && remap) {
-        // undistortion (ygzb_frames_set_undistort): level 0 = remap of the staged raw frames, in place of bgr2gray_kernel
+    if (d_src && map_xy) {
+        // undistortion (ygzb_frames_set_undistort, ygzb_tracker_set_undistort): level 0 = remap of the staged raw frames, in
+        // place of bgr2gray_kernel
         const int quads = ((g.lv[0].w + 3) / 4) * g.lv[0].h;
         const size_t frame = (size_t)g.lv[0].w * g.lv[0].h * channels;
         dim3 grid((quads + 255) / 256, count);
         ProfScope ps(ctx, kStageBgr2Gray);
         if (channels == 3)
-            remap_gray_kernel<3><<<grid, 256, 0, ctx->stream>>>(d_src, frame, f->d_map_xy, f->d_map_a, f->d_pyr, ctx->slot_stride, first, g.lv[0]);
+            remap_gray_kernel<3><<<grid, 256, 0, ctx->stream>>>(d_src, frame, map_xy, map_a, f->d_pyr, ctx->slot_stride, first, g.lv[0]);
         else
-            remap_gray_kernel<1><<<grid, 256, 0, ctx->stream>>>(d_src, frame, f->d_map_xy, f->d_map_a, f->d_pyr, ctx->slot_stride, first, g.lv[0]);
+            remap_gray_kernel<1><<<grid, 256, 0, ctx->stream>>>(d_src, frame, map_xy, map_a, f->d_pyr, ctx->slot_stride, first, g.lv[0]);
         YGZB_LAUNCHED(ctx);
     } else if (d_src) {
         const uint8_t* d_bgr = d_src;

@@ -72,6 +72,12 @@ struct ygzb_tracker {
     void* d_cam;
     std::vector<double> cam_K;     // [S][4]
     std::vector<float> cam_F;      // [S][4]
+    // per-stream undistortion maps (ygzb_tracker_set_undistort), allocated on a stream's first maps and kept until destroy:
+    // map_xy then map_a on the device, read only by that stream's uploads on the front stream, and their page-locked
+    // staging with an event behind its last copy
+    std::vector<uint8_t*> d_lens, h_lens;
+    std::vector<cudaEvent_t> e_lens;
+    std::vector<char> has_lens;    // maps set: ygzb_tracker_upload_stream remaps level 0
 };
 
 namespace {
@@ -79,6 +85,9 @@ namespace {
 static_assert(sizeof(ygzb_observation) == 48, "an observation row is 48 bytes");
 static_assert(sizeof(ygzb_pose_information) == 336, "an information record is 336 bytes");
 static_assert(sizeof(ygzb_map_point) == 32 && offsetof(ygzb_map_point, pw) == 8, "a map point row is 32 bytes: id, pw[3]");
+// a stream's maps: map_xy (short2 per pixel), then map_a (uint16 per pixel) from a 256-byte boundary
+size_t lens_a_offset(size_t pixels) { return (pixels * sizeof(short2) + 255) & ~(size_t)255; }
+size_t lens_bytes(size_t pixels) { return lens_a_offset(pixels) + pixels * sizeof(uint16_t); }
 constexpr size_t kf_stage_bytes = sizeof(ygzb_keyframe_job) + 12 * sizeof(double);   // a key-frame job and its start pose
 static_assert(sizeof(ygzb_keyframe_job) % sizeof(double) == 0, "the start poses behind the key-frame jobs are 8-byte aligned");
 
@@ -1048,6 +1057,10 @@ int ygzb_tracker_create(ygzb_frames* f, int n_streams, int max_jobs, const doubl
     if (rc == YGZB_OK) {
         t->start_T.assign(12 * S, 0.0);
         for (size_t s = 0; s < S; ++s) t->start_T[12 * s] = t->start_T[12 * s + 5] = t->start_T[12 * s + 10] = 1.0;
+        t->d_lens.assign(S, nullptr);
+        t->h_lens.assign(S, nullptr);
+        t->e_lens.assign(S, nullptr);
+        t->has_lens.assign(S, 0);
     }
     if (rc == YGZB_OK) rc = dalloc(ctx, &t->d_kfres, S);
     // (a result record carries YGZB_TRACK_RING pose slots and only the first n_local are written by a job: the whole record is
@@ -1105,6 +1118,11 @@ void ygzb_tracker_destroy(ygzb_tracker* t) {
     }
     for (cudaEvent_t e : {t->e_fill, t->e_front, t->e_main, t->e_up})
         if (e) cudaEventDestroy(e);
+    for (size_t s = 0; s < t->d_lens.size(); ++s) {
+        if (t->e_lens[s]) cudaEventDestroy(t->e_lens[s]);
+        if (t->d_lens[s]) cudaFree(t->d_lens[s]);
+        if (t->h_lens[s]) cudaFreeHost(t->h_lens[s]);
+    }
     delete t;
 }
 
@@ -1233,20 +1251,76 @@ int ygzb_tracker_set_camera(ygzb_tracker* t, int stream, const double K[4]) {
     return YGZB_OK;
 }
 
-int ygzb_tracker_upload(ygzb_tracker* t, int first, int count, const uint8_t* host, size_t frame_stride) {
+int ygzb_tracker_set_undistort(ygzb_tracker* t, int stream, const int16_t* map_xy, const uint16_t* map_a) {
     if (!t) return YGZB_ERR_INVALID;
     ygzb_ctx* ctx = t->ctx;
+    if (stream < 0 || stream >= t->st.S) return set_error(ctx, YGZB_ERR_INVALID, "set_undistort: stream %d out of range", stream);
+    if (!map_xy != !map_a) return set_error(ctx, YGZB_ERR_INVALID, "set_undistort: map_xy and map_a must both be given, or both be NULL");
+    if (!map_xy) {   // uploads enqueued before keep reading the maps, which stay allocated until the tracker is destroyed
+        t->has_lens[stream] = 0;
+        return YGZB_OK;
+    }
+    ygzb_frames* f = t->f;
+    if (f->undistort) return set_error(ctx, YGZB_ERR_INVALID, "set_undistort: the frame pool has undistortion maps of its own");
     cudaSetDevice(ctx->device);
-    // on the front stream, behind the last key-frame insertion (which still reads the frame slots of the previous window) and
-    // behind the last tracking chain (ditto); NOT behind a local BA in flight
+    const size_t n = (size_t)t->st.W * t->st.H, a_off = lens_a_offset(n);
+    if (!t->h_lens[stream]) {
+        YGZB_CUDA(ctx, cudaMallocHost((void**)&t->h_lens[stream], lens_bytes(n)));
+        YGZB_CUDA(ctx, cudaMalloc((void**)&t->d_lens[stream], lens_bytes(n)));
+        YGZB_CUDA(ctx, cudaEventCreateWithFlags(&t->e_lens[stream], cudaEventDisableTiming));
+    } else {   // the staging's last copy to the device has run (it waited for nothing but earlier front-stream work)
+        YGZB_CUDA(ctx, cudaEventSynchronize(t->e_lens[stream]));
+    }
+    if (!f->e_stage) YGZB_CUDA(ctx, cudaEventCreateWithFlags(&f->e_stage, cudaEventDisableTiming));
+    // the maps (host or device memory) are read into the staging and checked before anything an upload reads changes
+    uint8_t* h = t->h_lens[stream];
+    const uint16_t* a = reinterpret_cast<const uint16_t*>(h + a_off);
+    YGZB_CUDA(ctx, cudaMemcpy(h, map_xy, n * sizeof(short2), cudaMemcpyDefault));
+    YGZB_CUDA(ctx, cudaMemcpy(h + a_off, map_a, n * sizeof(uint16_t), cudaMemcpyDefault));
+    for (size_t i = 0; i < n; ++i)
+        if (a[i] >= 1024)
+            return set_error(ctx, YGZB_ERR_INVALID, "set_undistort: map_a[%zu] = %d is not a 5 + 5-bit fraction (< 1024)", i, (int)a[i]);
+    // in order on the front stream, which runs every upload: the ones enqueued before read the old maps, the ones enqueued
+    // after the new; nothing waits for the key-frame insertion or a local BA in flight
+    YGZB_CUDA(ctx, cudaMemcpyAsync(t->d_lens[stream], h, lens_bytes(n), cudaMemcpyHostToDevice, t->front));
+    YGZB_CUDA(ctx, cudaEventRecord(t->e_lens[stream], t->front));
+    t->has_lens[stream] = 1;
+    return YGZB_OK;
+}
+
+// on the front stream, behind the last key-frame insertion (which still reads the frame slots of the previous window) and
+// behind the last tracking chain (ditto); NOT behind a local BA in flight.  map_xy / map_a: the undistortion maps of level
+// 0, or NULL
+static int upload_front(ygzb_tracker* t, int first, int count, const uint8_t* host, size_t frame_stride, const short2* map_xy, const uint16_t* map_a) {
+    ygzb_ctx* ctx = t->ctx;
+    cudaSetDevice(ctx->device);
     YGZB_CUDA(ctx, cudaStreamWaitEvent(t->front, t->e_fill, 0));
     YGZB_CUDA(ctx, cudaStreamWaitEvent(t->front, t->e_main, 0));
     cudaStream_t main = ctx->stream;
     ctx->stream = t->front;
-    int rc = ygzb_frames_upload(t->f, first, count, host, 1, frame_stride);
+    int rc = frames_upload(t->f, first, count, host, 1, frame_stride, map_xy, map_a);
     if (rc == YGZB_OK) rc = check_cuda(ctx, cudaEventRecord(t->e_up, ctx->stream), "cudaEventRecord");
     ctx->stream = main;
     return rc;
+}
+
+int ygzb_tracker_upload(ygzb_tracker* t, int first, int count, const uint8_t* host, size_t frame_stride) {
+    if (!t) return YGZB_ERR_INVALID;
+    ygzb_frames* f = t->f;
+    return upload_front(t, first, count, host, frame_stride, f->undistort ? f->d_map_xy : nullptr, f->d_map_a);
+}
+
+int ygzb_tracker_upload_stream(ygzb_tracker* t, int stream, int first, int count, const uint8_t* host, size_t frame_stride) {
+    if (!t) return YGZB_ERR_INVALID;
+    ygzb_ctx* ctx = t->ctx;
+    if (stream < 0 || stream >= t->st.S) return set_error(ctx, YGZB_ERR_INVALID, "upload_stream: stream %d out of range", stream);
+    if (!t->has_lens[stream]) return ygzb_tracker_upload(t, first, count, host, frame_stride);
+    if (t->f->undistort)
+        return set_error(ctx, YGZB_ERR_INVALID, "upload_stream: stream %d and the frame pool both have undistortion maps", stream);
+    const uint8_t* d = t->d_lens[stream];
+    const size_t n = (size_t)t->st.W * t->st.H;
+    return upload_front(t, first, count, host, frame_stride, reinterpret_cast<const short2*>(d),
+                        reinterpret_cast<const uint16_t*>(d + lens_a_offset(n)));
 }
 
 int ygzb_tracker_track(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, ygzb_track_result* results) {
@@ -1553,7 +1627,7 @@ int ygzb_tracker_import(ygzb_tracker* t, int stream, const int32_t* entries, con
     }
     const size_t WH = (size_t)st.W * st.H;
     // the record's images are level 0 of key-frames, undistorted already: the pool's undistortion maps must not warp them again
-    for (int k = 0; k < n && rc == YGZB_OK; ++k) rc = frames_upload(t->f, kf_slots[k], 1, in->image + k * WH, 1, WH, false);
+    for (int k = 0; k < n && rc == YGZB_OK; ++k) rc = frames_upload(t->f, kf_slots[k], 1, in->image + k * WH, 1, WH, nullptr, nullptr);
     if (rc == YGZB_OK) rc = check_cuda(ctx, cudaEventRecord(t->e_fill, ctx->stream), "cudaEventRecord");
     return rc;
 }
@@ -1633,7 +1707,7 @@ int ygzb_tracker_import_reference(ygzb_tracker* t, int stream, const ygzb_refere
         YGZB_LAUNCHED(ctx);
     }
     const size_t WH = (size_t)st.W * st.H;
-    rc = frames_upload(t->f, t->ref_slots[stream], 1, in->image, 1, WH, false);   // undistorted already, like a map record's images
+    rc = frames_upload(t->f, t->ref_slots[stream], 1, in->image, 1, WH, nullptr, nullptr);   // undistorted already, like a map record's images
     if (rc == YGZB_OK) rc = check_cuda(ctx, cudaEventRecord(t->e_fill, ctx->stream), "cudaEventRecord");
     if (rc != YGZB_OK) return rc;
     t->cur_ref[stream] = t->ref_slots[stream];

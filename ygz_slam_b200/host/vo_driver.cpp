@@ -567,9 +567,20 @@ struct QFrame {
     bool restart = false;  // first frame of a new sequence (ygz_vo_restart): it becomes a first key-frame
 };
 using Camera = std::array<double, 4>;   // fx, fy, cx, cy
+// a lens (ygz_vo_set_lens): the raw camera K and its distortion dist = {k1, k2, p1, p2, k3}; on = false: none
+struct Lens {
+    bool on = false;
+    std::array<double, 4> K{};
+    std::array<double, 5> dist{};
+    // bit for bit, as records compare cameras
+    bool same(const Lens& o) const {
+        return on == o.on && (!on || (std::memcmp(K.data(), o.K.data(), sizeof K) == 0 && std::memcmp(dist.data(), o.dist.data(), sizeof dist) == 0));
+    }
+};
 struct SeqStart {
     Mat34 T;                  // pose of the sequence's first key-frame
     Camera K;                 // camera of the sequence
+    Lens lens;                // lens of the sequence
 };
 struct EStream : Counters {
     std::deque<KfInfo> kfs;   // at most YGZB_TRACK_RING, the newest is the reference key-frame; the last kLocalKeyframes are local
@@ -577,6 +588,7 @@ struct EStream : Counters {
     Mat34 T = identity();
     Mat34 start = identity(); // pose of the next sequence's first key-frame (ygz_vo_restart)
     Camera cam{};             // camera of the current sequence, or of the next one while a restart is pending (ygz_vo_set_camera)
+    Lens lens;                // lens of the current sequence, or of the next one while a restart is pending (ygz_vo_set_lens)
     std::deque<SeqStart> starts;   // the queued frames that start a sequence (the stream's first, restarts), in order
     bool has_pose = false, lost = false, has_depth = false;
     bool restart_pending = false;   // the next push starts a new sequence at `start`
@@ -714,6 +726,7 @@ class Engine {
         for (int i = 0; i < S_; ++i) order_.push_back(i);
         for (EStream& s : st_) std::copy_n(prm_.K, 4, s.cam.begin());
         tr_cam_.assign(S_, st_[0].cam);
+        tr_lens_.assign(S_, TrLens{});
         // YGZ_VO_BLOCKING_SYNC=1: sleep instead of spinning in the one synchronisation per round (hosts with fewer CPUs than
         // engine threads; bench.py sets it when the threads of all ranks outnumber the CPUs it may use)
         const char* e = std::getenv("YGZ_VO_BLOCKING_SYNC");
@@ -771,7 +784,7 @@ class Engine {
         QFrame f{image, depth, tag, stacked};
         if (pushed(i) == 0 || s.restart_pending) {
             f.restart = s.restart_pending;
-            s.starts.push_back({s.start, s.cam});
+            s.starts.push_back({s.start, s.cam, s.lens});
             s.restart_pending = false;
         }
         s.queue.push_back(f);
@@ -797,6 +810,20 @@ class Engine {
         if (pushed(i) > 0 && !s.restart_pending) return YGZB_ERR_INVALID;
         s.cam = K;
         return YGZB_OK;
+    }
+    // the lens of stream i's next sequence, at the times set_camera accepts (the caller has checked it); its maps, built for
+    // the camera that sequence ends up with, reach the tracker when the sequence's first frame is uploaded (use_lens)
+    int set_lens(int i, const Lens& L) {
+        EStream& s = st_[i];
+        if (pushed(i) > 0 && !s.restart_pending) return YGZB_ERR_INVALID;
+        s.lens = L;
+        return YGZB_OK;
+    }
+    // some stream has a lens, now or for its next sequence: its records carry a lens block
+    bool any_lens() const {
+        for (const EStream& s : st_)
+            if (s.lens.on) return true;
+        return false;
     }
     // final results go to `traj` (this group's [S][n_frames][12], rows in the caller's stream order; NULL: none) and, with
     // collect, to the result queue that pop_results drains
@@ -920,6 +947,9 @@ class Engine {
                     if (s.queue[t].restart) w = t;
             }
             w = std::min(w, (int)s.queue.size());
+            // a sequence's lens reaches the tracker with its first frame's upload: every frame of the old sequence has been
+            // uploaded before (a window never crosses a restart), and the tracker orders the maps behind those uploads
+            if (first) CHK(use_lens(i, s.starts.front().lens, s.starts.front().K));
             CHK(upload(i, w));
             if (first) {
                 wins_.push_back({i, s.next_frame, 1, -1});
@@ -1044,6 +1074,7 @@ class Engine {
         }
         if (rec->n_keyframes != (int)entries.size()) return YGZB_ERR_INVALID;
         CHK(use_camera(i, s.cam));
+        CHK(use_lens(i, s.lens, s.cam));
         CHK(ygzb_tracker_import(tr_, i, entries.data(), slots.data(), rec));
         if (ref) CHK(ygzb_tracker_import_reference(tr_, i, ref));
         st_[i] = s;
@@ -1071,6 +1102,28 @@ class Engine {
         tr_cam_[i] = K;
         return YGZB_OK;
     }
+    // the tracker's undistortion maps of stream i become those of lens L seen through camera K (none without a lens) for
+    // every upload enqueued from here on; nothing is enqueued when they are already
+    int use_lens(int i, const Lens& L, const Camera& K) {
+        TrLens& cur = tr_lens_[i];
+        if (cur.lens.same(L) && (!L.on || cur.K == K)) return YGZB_OK;
+        if (L.on) {
+            const size_t n = (size_t)W_ * H_;
+            if (!(maps_for_.lens.same(L) && maps_for_.K == K)) {   // (streams of one lens and camera share the host maps)
+                map_xy_.resize(2 * n);
+                map_a_.resize(n);
+                maps_for_ = {};
+                CHK(ygzb_undistort_map(W_, H_, L.K.data(), L.dist.data(), K.data(), map_xy_.data(), map_a_.data()));
+                maps_for_ = {L, K};
+            }
+            CHK(ygzb_tracker_set_undistort(tr_, i, map_xy_.data(), map_a_.data()));
+            h2d_other_bytes += (long long)(n * 6);
+        } else {
+            CHK(ygzb_tracker_set_undistort(tr_, i, nullptr, nullptr));
+        }
+        cur = {L, K};
+        return YGZB_OK;
+    }
     // the first w queued frames of stream i into its frame slots: one strided copy when they are equally spaced in one
     // stacked sequence, one copy per frame otherwise (frames pushed one by one may sit in separate allocations, which one
     // strided copy cannot span even when their addresses happen to be equally spaced)
@@ -1081,8 +1134,13 @@ class Engine {
         bool strided = stride >= (ptrdiff_t)fb;
         for (int t = 0; t < w && strided; ++t) strided = q[t].stacked && (t < 2 || q[t].image - q[t - 1].image == stride);
         h2d_image_bytes += (long long)w * (long long)fb;
-        if (strided) return ygzb_tracker_upload(tr_, i * F_, w, q[0].image, (size_t)stride);
-        for (int t = 0; t < w; ++t) CHK(ygzb_tracker_upload(tr_, i * F_ + t, 1, q[t].image, fb));
+        // a stream without a lens uploads exactly as before lenses existed
+        auto up = [&](int first, int count, const uint8_t* src, size_t frame_stride) {
+            return tr_lens_[i].lens.on ? ygzb_tracker_upload_stream(tr_, i, first, count, src, frame_stride)
+                                       : ygzb_tracker_upload(tr_, first, count, src, frame_stride);
+        };
+        if (strided) return up(i * F_, w, q[0].image, (size_t)stride);
+        for (int t = 0; t < w; ++t) CHK(up(i * F_ + t, 1, q[t].image, fb));
         return YGZB_OK;
     }
     // the map update of key-frame job kj, whose result r and rows (r.ba_points moved, then r.n_features new) have just come
@@ -1179,6 +1237,14 @@ class Engine {
     RowQueue<KfFrame, ygzb_observation> kframes_;   // ... and their frames, with their observation rows
     std::vector<int> order_;
     std::vector<Camera> tr_cam_;   // the tracker's camera of every stream (ygzb_tracker_set_camera), as last set
+    struct TrLens {
+        Lens lens;
+        Camera K;
+    };
+    std::vector<TrLens> tr_lens_;  // the lens and camera the tracker's maps of every stream were built for (ygzb_tracker_set_undistort)
+    std::vector<int16_t> map_xy_;  // host maps of use_lens, built for the lens and camera maps_for_ (lens off: none)
+    std::vector<uint16_t> map_a_;
+    TrLens maps_for_;
     double* traj_ = nullptr;
     int traj_frames_ = 0;
     bool collect_ = false;
@@ -1227,19 +1293,24 @@ struct RefBuf {
 static_assert(std::endian::native == std::endian::little, "stream records are little-endian and copied field by field");
 constexpr uint8_t kRecordMagic[4] = {'Y', 'G', 'Z', 'S'};
 
-// what a record is made under and must be loaded under: the engine's image size, grid, pyramid, camera and reference mode
+// what a record is made under and must be loaded under: the engine's image size, grid, pyramid, camera and reference mode,
+// and the stream's lens
 struct RecordGeom {
     int32_t width, height, cells, n_levels;
     double K[4];
     int32_t ref_mode;
+    Lens lens{};
     size_t wh() const { return (size_t)width * height; }
 };
+constexpr size_t kRecordLensBytes = 9 * sizeof(double);   // version 2's lens block: K[4], dist[5]
 
-// the largest record of an engine: a full ring at capacity, a full reference, a depth map (the sections of write_record)
-size_t record_bound(const RecordGeom& g) {
+// the largest record of an engine: a full ring at capacity, a full reference, a depth map (the sections of write_record),
+// and with lens, a lens block
+size_t record_bound(const RecordGeom& g, bool lens) {
     const size_t R = YGZB_TRACK_RING, F = R * g.cells, O = R * YGZB_MAP_OBS_PER_CELL * g.cells;
     const size_t C = (size_t)YGZB_TRACK_REF_FEATURES_PER_CELL * g.cells, WH = g.wh();
-    return 68 + (4 + R * 116 + 2 * 96 + 4 + 16 + 12 * 8)        // header, host state
+    return 68 + (lens ? kRecordLensBytes : 0)                   // header, lens
+           + (4 + R * 116 + 2 * 96 + 4 + 16 + 12 * 8)           // host state
            + (4 + R * (116 + WH) + F * 49 + O * 24)             // map
            + (4 + 96 + C * 24 + WH)                             // reference
            + WH * sizeof(double);                               // depth map
@@ -1283,12 +1354,16 @@ void write_record(RecordWriter& w, const RecordGeom& g, const EStream& s, const 
     const size_t WH = g.wh();
     // 1. header (the size is written last)
     w.bytes(kRecordMagic, 4);
-    w.put<uint32_t>(YGZ_VO_STREAM_RECORD_VERSION);
+    w.put<uint32_t>(g.lens.on ? YGZ_VO_STREAM_RECORD_VERSION_LENS : YGZ_VO_STREAM_RECORD_VERSION);
     const size_t size_at = w.n;
     w.put<uint64_t>(0);
     w.put<int32_t>(g.width); w.put<int32_t>(g.height); w.put<int32_t>(g.cells); w.put<int32_t>(g.n_levels);
     w.bytes(g.K, sizeof g.K);
     w.put<int32_t>(g.ref_mode);
+    if (g.lens.on) {   // version 2
+        w.bytes(g.lens.K.data(), sizeof g.lens.K);
+        w.bytes(g.lens.dist.data(), sizeof g.lens.dist);
+    }
     // 2. host state
     w.put<int32_t>((int32_t)s.kfs.size());
     for (const KfInfo& kf : s.kfs) {
@@ -1353,9 +1428,15 @@ int read_record(const uint8_t* in, size_t size, const RecordGeom& g, StreamRecor
     rg.width = r.get<int32_t>(); rg.height = r.get<int32_t>(); rg.cells = r.get<int32_t>(); rg.n_levels = r.get<int32_t>();
     r.bytes(rg.K, sizeof rg.K);
     rg.ref_mode = r.get<int32_t>();
-    if (!r.ok || std::memcmp(magic, kRecordMagic, 4) != 0 || version != YGZ_VO_STREAM_RECORD_VERSION || total != size) return YGZB_ERR_INVALID;
-    if (rg.width != g.width || rg.height != g.height || rg.cells != g.cells || rg.n_levels != g.n_levels || rg.ref_mode != g.ref_mode ||
-        std::memcmp(rg.K, g.K, sizeof g.K) != 0)   // K bit for bit
+    if (!r.ok || std::memcmp(magic, kRecordMagic, 4) != 0 || total != size) return YGZB_ERR_INVALID;
+    if (version != YGZ_VO_STREAM_RECORD_VERSION && version != YGZ_VO_STREAM_RECORD_VERSION_LENS) return YGZB_ERR_INVALID;
+    rg.lens.on = version == YGZ_VO_STREAM_RECORD_VERSION_LENS;
+    if (rg.lens.on) {
+        r.bytes(rg.lens.K.data(), sizeof rg.lens.K);
+        r.bytes(rg.lens.dist.data(), sizeof rg.lens.dist);
+    }
+    if (!r.ok || rg.width != g.width || rg.height != g.height || rg.cells != g.cells || rg.n_levels != g.n_levels || rg.ref_mode != g.ref_mode ||
+        std::memcmp(rg.K, g.K, sizeof g.K) != 0 || !rg.lens.same(g.lens))   // K and the lens bit for bit
         return YGZB_ERR_INVALID;
     // 2. host state
     EStream& s = out.s;
@@ -1797,6 +1878,31 @@ int ygz_vo_set_camera(ygz_vo* vo, int stream, const double K[4]) {
     return vo->eng->set_camera(stream, Camera{K[0], K[1], K[2], K[3]});
 }
 
+int ygz_vo_set_lens(ygz_vo* vo, int stream, const double K[4], const double dist[5]) {
+    if (!vo || stream < 0 || stream >= vo->n_streams || !K != !dist) return YGZB_ERR_INVALID;
+    Lens L;
+    if (K) {
+        for (int c = 0; c < 4; ++c)
+            if (!std::isfinite(K[c])) return YGZB_ERR_INVALID;
+        for (int c = 0; c < 5; ++c)
+            if (!std::isfinite(dist[c])) return YGZB_ERR_INVALID;
+        if (!(K[0] > 0 && K[1] > 0)) return YGZB_ERR_INVALID;
+        L.on = true;
+        std::copy_n(K, 4, L.K.begin());
+        std::copy_n(dist, 5, L.dist.begin());
+    }
+    return vo->eng->set_lens(stream, L);
+}
+
+int ygz_vo_get_lens(const ygz_vo* vo, int stream, int* has_lens, double K[4], double dist[5]) {
+    if (!vo || !has_lens || !K || !dist || stream < 0 || stream >= vo->n_streams) return YGZB_ERR_INVALID;
+    const Lens& L = vo->eng->streams()[stream].lens;
+    *has_lens = L.on ? 1 : 0;
+    std::copy(L.K.begin(), L.K.end(), K);   // (zeros without a lens)
+    std::copy(L.dist.begin(), L.dist.end(), dist);
+    return YGZB_OK;
+}
+
 int ygz_vo_get_camera(const ygz_vo* vo, int stream, double K[4]) {
     if (!vo || !K || stream < 0 || stream >= vo->n_streams) return YGZB_ERR_INVALID;
     const Camera& c = vo->eng->streams()[stream].cam;
@@ -1872,7 +1978,7 @@ int ygz_vo_export_map(ygz_vo* vo, int stream, ygzb_map_record* out) {
 
 int ygz_vo_stream_record_bound(const ygz_vo* vo, size_t* bytes) {
     if (!vo || !bytes) return YGZB_ERR_INVALID;
-    *bytes = record_bound(vo->geom);
+    *bytes = record_bound(vo->geom, vo->eng->any_lens());
     return YGZB_OK;
 }
 
@@ -1884,8 +1990,9 @@ int ygz_vo_save_stream(ygz_vo* vo, int stream, void* buf, size_t capacity, size_
     if (!e.settled(stream)) return YGZB_ERR_INVALID;
     if (!vo->stage.mem) CHK(vo->stage.init(vo->geom));
     const EStream& s = e.streams()[stream];
-    RecordGeom g = vo->geom;   // with the stream's own camera
+    RecordGeom g = vo->geom;   // with the stream's own camera and lens
     std::copy(s.cam.begin(), s.cam.end(), g.K);
+    g.lens = s.lens;
     SaveStage& st = vo->stage;
     CHK(e.export_map(stream, &st.map));
     const bool ref = e.has_reference(stream);
@@ -1907,12 +2014,15 @@ int ygz_vo_load_stream(ygz_vo* vo, int stream, const void* buf, size_t size) {
     if (!vo || !buf || stream < 0 || stream >= vo->n_streams) return YGZB_ERR_INVALID;
     Engine& e = *vo->eng;
     if (!e.settled(stream)) return YGZB_ERR_INVALID;
-    const Camera cam = e.streams()[stream].cam;   // the record's K must be the destination stream's camera
+    const Camera cam = e.streams()[stream].cam;   // the record's K and lens must be the destination stream's
+    const Lens lens = e.streams()[stream].lens;
     RecordGeom g = vo->geom;
     std::copy(cam.begin(), cam.end(), g.K);
+    g.lens = lens;
     StreamRecord rec(g);
     CHK(read_record(static_cast<const uint8_t*>(buf), size, g, rec));
     rec.s.cam = cam;
+    rec.s.lens = lens;
     CHK(e.check_start_pose(stream, rec.s.start));
     CHK(e.adopt(stream, rec.s, &rec.map.rec, rec.has_ref ? &rec.ref.rec : nullptr));
     if (rec.s.has_depth) CHK(e.set_depth(stream, rec.depth.data()));

@@ -41,6 +41,8 @@ def _lib():
         _LIB.ygz_vo_restart.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         _LIB.ygz_vo_set_camera.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         _LIB.ygz_vo_get_camera.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        _LIB.ygz_vo_set_lens.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+        _LIB.ygz_vo_get_lens.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         _LIB.ygz_vo_step.argtypes = [C.c_void_p]
         _LIB.ygz_vo_flush.argtypes = [C.c_void_p]
         _LIB.ygz_vo_poll.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
@@ -166,11 +168,15 @@ _COUNTERS = ("n_keyframes", "n_ba", "n_candidates", "n_projected", "n_inliers", 
              "n_restarts")
 
 
+_LENS_VERSION = 2   # YGZ_VO_STREAM_RECORD_VERSION_LENS: a 72-byte lens block (K[4], dist[5]) follows the header
+
+
 def stream_record_next_frame(rec):
-    """next_frame of a stream record (uint8 array) from its fixed offset: the 68-byte header, n_kf, n_kf key-frames of 116
-    bytes, the two poses, the four flags and frames_since_kf come before it."""
-    n_kf = int(rec[68:72].view("<i4")[0])
-    off = 72 + 116 * n_kf + 2 * 96 + 4 + 4
+    """next_frame of a stream record (uint8 array) from its fixed offset: the 68-byte header, in version 2 the 72-byte lens
+    block, n_kf, n_kf key-frames of 116 bytes, the two poses, the four flags and frames_since_kf come before it."""
+    head = 68 + (72 if int(rec[4:8].view("<u4")[0]) == _LENS_VERSION else 0)
+    n_kf = int(rec[head:head + 4].view("<i4")[0])
+    off = head + 4 + 116 * n_kf + 2 * 96 + 4 + 4
     return int(rec[off:off + 4].view("<i4")[0])
 
 
@@ -193,10 +199,13 @@ def parse_stream_record(data):
         return out[name][1]
 
     take("magic", "u1", 4)
-    take("version", "u4"); take("size", "u8")
+    version = take("version", "u4")
+    take("size", "u8")
     W, H = take("width", "i4"), take("height", "i4")
     take("cells", "i4"); take("n_levels", "i4"); take("K", "f8", 4)
     mode = take("ref_mode", "i4")
+    if version == _LENS_VERSION:
+        take("lens.K", "f8", 4); take("lens.dist", "f8", 5)
     n_kf = take("n_kf", "i4")
     for k in range(n_kf):
         take(f"kf[{k}].entry", "i4"); take(f"kf[{k}].n", "i4"); take(f"kf[{k}].frame_id", "i4"); take(f"kf[{k}].mp0", "i8")
@@ -236,10 +245,12 @@ class Engine:
     poll also returns an [n, 2, 6, 6] array, the sparse alignment's Fisher information and pose-only's information
     matrix of each result as full symmetric matrices.  map_updates=True: every key-frame insertion queues what it changed
     in the local map (ygz_vo_set_map_updates), which poll_map_updates returns.  cameras: None, or one (fx, fy, cx, cy)
-    per stream (None: K), set before any push (ygz_vo_set_camera)."""
+    per stream (None: K), set before any push (ygz_vo_set_camera).  lenses: None, or one (K, dist) or None per stream:
+    the stream's raw frames are those of camera K = (fx, fy, cx, cy) with distortion dist = (k1, k2, p1, p2, k3), and the
+    engine undistorts them on the device to the stream's camera (ygz_vo_set_lens)."""
 
     def __init__(self, ctx, n_streams, window=8, ref_mode="keyframe", kf_min_frames=10, kf_min_rot=0.1, kf_min_trans=0.1,
-                 min_inliers=30, K=None, observations=False, information=False, map_updates=False, cameras=None):
+                 min_inliers=30, K=None, observations=False, information=False, map_updates=False, cameras=None, lenses=None):
         if ref_mode not in _REF_MODES:
             raise ValueError(f"ref_mode must be 'keyframe' or 'previous', not {ref_mode!r}")
         p = ctx.params
@@ -269,6 +280,12 @@ class Engine:
             for s, cam in enumerate(cameras):
                 if cam is not None:
                     self.set_camera(s, cam)
+        if lenses is not None:
+            if len(lenses) != self.n_streams:
+                raise ValueError(f"lenses: {len(lenses)} lenses for {self.n_streams} streams")
+            for s, lens in enumerate(lenses):
+                if lens is not None:
+                    self.set_lens(s, *lens)
 
     def set_camera(self, stream, K):
         """K = (fx, fy, cx, cy) of `stream`'s next sequence (ygz_vo_set_camera): only before its first push or while a
@@ -281,6 +298,24 @@ class Engine:
         K = np.zeros(4, np.float64)
         self.ctx.check(self.lib.ygz_vo_get_camera(self.h, int(stream), K.ctypes.data), "ygz_vo_get_camera")
         return K
+
+    def set_lens(self, stream, K=None, dist=None):
+        """The lens of `stream`'s next sequence (ygz_vo_set_lens): raw camera K = (fx, fy, cx, cy) and dist = (k1, k2, p1,
+        p2[, k3]); no arguments: none.  At the times set_camera is accepted; frames pushed before the restart keep the old
+        lens."""
+        if K is None and dist is None:
+            self.ctx.check(self.lib.ygz_vo_set_lens(self.h, int(stream), None, None), "ygz_vo_set_lens")
+            return
+        K = np.ascontiguousarray(K, np.float64).reshape(4)
+        d = np.zeros(5)
+        d[:len(dist)] = dist
+        self.ctx.check(self.lib.ygz_vo_set_lens(self.h, int(stream), K.ctypes.data, d.ctypes.data), "ygz_vo_set_lens")
+
+    def lens(self, stream):
+        """The lens set_lens last gave `stream`: (K, dist) arrays, or None for none."""
+        has, K, d = C.c_int(0), np.zeros(4, np.float64), np.zeros(5, np.float64)
+        self.ctx.check(self.lib.ygz_vo_get_lens(self.h, int(stream), C.byref(has), K.ctypes.data, d.ctypes.data), "ygz_vo_get_lens")
+        return (K, d) if has.value else None
 
     def set_observations(self, on):
         """Switch the observation rows of the results on or off (ygz_vo_set_observations): only while the engine is
@@ -430,8 +465,9 @@ class Engine:
     def save_stream(self, stream):
         """The whole state of `stream` as a stream record (bytes, the layout of include/ygz_vo.h); flush first.  The stream
         is unchanged and may go on tracking."""
-        if not hasattr(self, "_record_buf"):
-            self._record_buf = np.empty(self.stream_record_bound(), np.uint8)
+        bound = self.stream_record_bound()   # (grows by the lens block once a stream has a lens)
+        if getattr(self, "_record_buf", None) is None or self._record_buf.size < bound:
+            self._record_buf = np.empty(bound, np.uint8)
         buf, n = self._record_buf, C.c_size_t(0)
         self.ctx.check(self.lib.ygz_vo_save_stream(self.h, int(stream), buf.ctypes.data, buf.size, C.byref(n)), "ygz_vo_save_stream")
         return buf[:n.value].tobytes()
