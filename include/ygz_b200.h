@@ -494,7 +494,7 @@ int ygzb_tracker_upload(ygzb_tracker* t, int first, int count, const uint8_t* ho
 /* undistortion maps of `stream` (the format of ygzb_frames_set_undistort: image_width x image_height entries, host or
  * device memory), so that the streams of one tracker may come from different lenses; map_xy == map_a == NULL clears
  * them.  They apply to the frames ygzb_tracker_upload_stream uploads for `stream`: level 0 becomes the remap of the raw
- * grey frame, bit for bit as with the pool's maps, and the stream's camera (ygzb_tracker_set_camera) and depth maps are
+ * frame (of the stream's format, ygzb_tracker_set_source), bit for bit as with the pool's maps, and the stream's camera (ygzb_tracker_set_camera) and depth maps are
  * the undistorted camera's.  Ordered like an upload, on the tracker's second CUDA stream: the uploads enqueued before the
  * call read the old maps, those enqueued after it the new ones; it waits for no key-frame insertion or local BA.  The
  * call returns once the maps have been read (a device buffer of 6 bytes per pixel per stream, allocated on the stream's
@@ -502,9 +502,23 @@ int ygzb_tracker_upload(ygzb_tracker* t, int first, int count, const uint8_t* ho
  * tracker, a stream out of range, only one of the two pointers, an entry map_a >= 1024, or maps on the frame pool
  * (ygzb_frames_set_undistort): a pool's maps and a stream's are never combined.                                       */
 int ygzb_tracker_set_undistort(ygzb_tracker* t, int stream, const int16_t* map_xy, const uint16_t* map_a);
-/* ygzb_tracker_upload of frames of `stream`: with maps set for the stream (ygzb_tracker_set_undistort), level 0 is
- * remapped through them; without, it is exactly ygzb_tracker_upload.  YGZB_ERR_INVALID for a NULL tracker, a stream out
- * of range, the arguments ygzb_tracker_upload refuses, or a stream with maps on a frame pool that has maps too.       */
+/* the frames ygzb_tracker_upload_stream reads for `stream`: width x height pixels of `channels` bytes (1: grey, 3: BGR,
+ * converted as cv::cvtColor(COLOR_BGR2GRAY)), rows packed, so that the streams of one tracker may come from sensors of
+ * their own size and colour.  The default is image_width x image_height, grey.  A size other than the context's is
+ * resampled through the stream's maps (ygzb_tracker_set_undistort, built for that raw size, e.g. by ygzb_undistort_map
+ * with the raw camera's K and the stream's camera as newK): level 0 is cv::remap(cvtColor(raw)) bit for bit, taps outside
+ * the raw frame reading 0.  INTER_LINEAR samples, so a downscale of 2x or more aliases, exactly as cv::remap does.  Read
+ * when an upload is enqueued: the uploads enqueued before the call read the old format, those after it the new one.
+ * YGZB_ERR_INVALID, with the stream's format unchanged, for a NULL tracker, a stream out of range, a width or height < 1
+ * or > 32767 (the maps' int16 range) or channels other than 1 and 3.                                                  */
+int ygzb_tracker_set_source(ygzb_tracker* t, int stream, int width, int height, int channels);
+/* ygzb_tracker_upload of frames of `stream`, in the stream's format (ygzb_tracker_set_source; frame_stride >= width *
+ * height * channels): with maps set for the stream (ygzb_tracker_set_undistort), level 0 is remapped through them;
+ * without, a BGR frame is converted (through the frame pool's maps, if it has any), and a grey frame of the context's size
+ * is exactly ygzb_tracker_upload.  Raw frames that a kernel reads are staged in the frame pool's own buffer, whose every
+ * reuse waits for the last kernel that read it.  YGZB_ERR_INVALID for a NULL tracker, a stream out of range, the arguments
+ * ygzb_tracker_upload refuses, a frame_stride below one raw frame, a raw size other than the context's without maps for
+ * the stream, or a stream with maps on a frame pool that has maps too.                                               */
 int ygzb_tracker_upload_stream(ygzb_tracker* t, int stream, int first, int count, const uint8_t* host, size_t frame_stride);
 /* asynchronous: enqueues the chain on the context's stream and a copy of the n_jobs result records into `results`
  * (host memory, page-locked for a truly asynchronous copy); valid after ygzb_synchronize(ctx).                    */

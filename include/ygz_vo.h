@@ -68,10 +68,13 @@ typedef struct {
 /* A tracker on `ctx` for cfg->n_streams streams; the image size is the context's (ygzb_params image_width/height).
  * YGZB_ERR_INVALID for a NULL argument or a config that does not match the context.                                 */
 int ygz_vo_create(ygzb_ctx* ctx, const ygz_vo_config* cfg, ygz_vo** out);
-/* queues a grey image (image_width * image_height bytes, host or device memory) of `stream`: the raw, distorted frame
- * when the stream's sequence has a lens (ygz_vo_set_lens), which the engine undistorts on the device as it uploads it.  Nothing runs until
- * ygz_vo_step or ygz_vo_flush.  YGZB_ERR_INVALID, with nothing queued, for a stream out of range, a NULL image, or a NULL
- * depth on a stream that has no depth map yet or whose next frame starts a new sequence (ygz_vo_restart).          */
+/* queues an image of `stream` (host or device memory) in the format of its sequence (ygz_vo_set_frame_format; by default
+ * grey, image_width * image_height bytes): width * height * channels bytes, rows packed.  It is the raw, distorted frame
+ * when the stream's sequence has a lens (ygz_vo_set_lens), which the engine resamples on the device as it uploads it; a
+ * BGR frame is converted there.  Nothing runs until ygz_vo_step or ygz_vo_flush.  YGZB_ERR_INVALID, with nothing queued,
+ * for a stream out of range, a NULL image, a NULL depth on a stream that has no depth map yet or whose next frame starts
+ * a new sequence (ygz_vo_restart), or a sequence's first frame whose format has another size than the context's while the
+ * sequence has no lens.                                                                                              */
 int ygz_vo_push(ygz_vo* vo, int stream, const uint8_t* image, const double* depth, int64_t tag);
 /* starts a new sequence of `stream` whose first key-frame takes pose T_cw (3x4 row-major; NULL: identity), to place a
  * sequence in the caller's world frame or to resume a lost stream, e.g. at the pose of its last YGZ_VO_LOST result.
@@ -118,7 +121,9 @@ int ygz_vo_get_camera(const ygz_vo* vo, int stream, double K[4]);
  * the raw camera and dist = {k1, k2, p1, p2, k3} (the model of ygzb_undistort_map); K = dist = NULL: no lens.
  *  - The sequence's frames are undistorted on the device as they are uploaded, level 0 being
  *    cv::remap(image, ygzb_undistort_map(width, height, K, dist, newK)) bit for bit, with newK the stream's camera for
- *    that sequence (ygz_vo_set_camera, or the config's K).  Everything else is in that undistorted camera: the depth maps
+ *    that sequence (ygz_vo_set_camera, or the config's K), and `image` the pushed frame, converted to grey first if it is
+ *    BGR.  The raw frame may have its own size (ygz_vo_set_frame_format): K is then that raw camera's, the maps keep the
+ *    context's width x height and taps outside the raw frame read 0.  With dist = 0 that is a pure crop or scale.  Everything else is in that undistorted camera: the depth maps
  *    pushed with the frames, the results, observation rows, information records, map updates and ygz_vo_export_map;
  *    the key-frame images of map and reference records are undistorted level 0 and are never remapped again.
  *  - A stream with a lens gives what a stream without one gives when it is pushed the undistorted frames.  A stream
@@ -129,6 +134,7 @@ int ygz_vo_get_camera(const ygz_vo* vo, int stream, double K[4]);
  *  - Barrier: frames pushed before ygz_vo_restart are remapped with the old lens (or none) even when they are uploaded
  *    after the call; the new maps reach the device behind the last of them, without waiting for a local BA in flight.
  *  - The tracker holds 6 bytes of maps per pixel for each stream that has had a lens (1.8 MB at 640x480).
+ *  - Clearing the lens of a sequence whose frame format has another size than the context's makes its first push fail.
  *  - Stream records of a stream with a lens are version 2 (a lens block behind the header), and ygz_vo_load_stream
  *    accepts a record only if its lens, or the absence of one, equals the destination stream's bit for bit (as for K).
  *    To hand a stream over into a stream that has tracked: ygz_vo_flush, ygz_vo_restart(stream), ygz_vo_set_camera,
@@ -139,6 +145,27 @@ int ygz_vo_set_lens(ygz_vo* vo, int stream, const double K[4], const double dist
 /* the lens ygz_vo_set_lens last gave `stream`: that of its current sequence, or of the next one while a restart is
  * pending.  *has_lens = 0 (K and dist zeros) for none.  YGZB_ERR_INVALID for a NULL argument or a stream out of range. */
 int ygz_vo_get_lens(const ygz_vo* vo, int stream, int* has_lens, double K[4], double dist[5]);
+/* the format of the frames `stream`'s next sequence pushes, so that each stream may come from a sensor of its own size and
+ * colour: width x height pixels of `channels` bytes, 1 (grey) or 3 (BGR, converted as cv::cvtColor(COLOR_BGR2GRAY)), rows
+ * packed.  The default, image_width x image_height x 1, is the frames as they have always been pushed.
+ *  - A width x height other than the context's needs a lens (ygz_vo_set_lens) whose K is the raw camera's: level 0 is
+ *    cv::remap(cvtColor(raw), ygzb_undistort_map(image_width, image_height, K, dist, newK)) bit for bit, newK the stream's
+ *    camera.  The resampling is INTER_LINEAR, so a downscale of 2x or more aliases, exactly as cv::remap does.
+ *  - Everything downstream keeps the context's size and the stream's camera: pyramid, grid, the depth maps pushed with
+ *    the frames (image_width x image_height doubles), results, observation rows, information records, map updates and
+ *    ygz_vo_export_map.  A stream with a format gives, byte for byte, what a default-format stream gives when it is
+ *    pushed the frames resampled beforehand.  A stream of the default format without a lens uploads exactly as before.
+ *  - Accepted at the times ygz_vo_set_camera is; of two calls with no push in between, the last one counts.
+ *  - Barrier: frames pushed before ygz_vo_restart are uploaded with the old format even when they are uploaded after the
+ *    call.
+ *  - Stream records of a stream with a format other than the default are version 3 (a format block behind the header),
+ *    and ygz_vo_load_stream accepts a record only if its format equals the destination stream's.
+ * YGZB_ERR_INVALID, changing nothing, for a NULL vo, a stream out of range, a width or height < 1 or > 32767, channels
+ * other than 1 and 3, or a call at any other time.                                                                 */
+int ygz_vo_set_frame_format(ygz_vo* vo, int stream, int width, int height, int channels);
+/* the format ygz_vo_set_frame_format last gave `stream` (the default until then): that of its current sequence, or of
+ * the next one while a restart is pending.  YGZB_ERR_INVALID for a NULL argument or a stream out of range.           */
+int ygz_vo_get_frame_format(const ygz_vo* vo, int stream, int* width, int* height, int* channels);
 /* one round over what is queued, with one host synchronisation: the results of the windows it tracks are final on
  * return, except a frame that triggers a key-frame, whose insertion is enqueued by the next round.                 */
 int ygz_vo_step(ygz_vo* vo);
@@ -243,9 +270,13 @@ int ygz_vo_export_map(ygz_vo* vo, int stream, ygzb_map_record* out);
  * depth = NULL would use (ygzb_tracker_get_depth).  A stream loaded from it continues exactly as the saved one would have.
  *
  * Layout: little-endian, packed (no padding; fields are not aligned), every count before the rows it describes.
- *   1. header      u8 magic[4] = "YGZS", u32 version = 1 (no lens) or 2 (a lens), u64 size (of the whole record),
+ *   1. header      u8 magic[4] = "YGZS", u32 version = 1 (no lens, default format), 2 (a lens, default format) or 3
+ *                  (a format other than the default), u64 size (of the whole record),
  *                  i32 width, height, cells, n_levels, f64 K[4] (the stream's camera), i32 ref_mode           (68 bytes)
- *      lens        (version 2 only) f64 K[4], f64 dist[5]: the stream's lens (ygz_vo_get_lens)                   (72 bytes)
+ *      format      (version 3 only) i32 width, height, channels: the stream's frame format
+ *                  (ygz_vo_get_frame_format), i32 has_lens (0 or 1)                                             (16 bytes)
+ *      lens        (version 2, and version 3 with has_lens) f64 K[4], f64 dist[5]: the stream's lens
+ *                  (ygz_vo_get_lens)                                                                            (72 bytes)
  *   2. host state  i32 n_kf, then per key-frame of the stream's ring, oldest first:
  *                      i32 entry, i32 n, i32 frame_id, i64 mp0, f64 T_cw[12]                               (116 bytes)
  *                  f64 T_cw[12] (current pose), f64 start[12] (pose of the next sequence's first key-frame),
@@ -263,8 +294,10 @@ int ygz_vo_export_map(ygz_vo* vo, int stream, ygzb_map_record* out);
  * and an empty map.                                                                                                 */
 #define YGZ_VO_STREAM_RECORD_VERSION 1
 #define YGZ_VO_STREAM_RECORD_VERSION_LENS 2
-/* *bytes = an upper bound of the size of any stream record of `vo`: a full ring, a full reference, a depth map, and
- * while a stream of `vo` has a lens (ygz_vo_get_lens), the lens block.                                                */
+#define YGZ_VO_STREAM_RECORD_VERSION_FORMAT 3
+/* *bytes = an upper bound of the size of any stream record of `vo`: a full ring, a full reference, a depth map, while a
+ * stream of `vo` has a lens (ygz_vo_get_lens) the lens block, and while one has a format other than the default
+ * (ygz_vo_get_frame_format) the format block.                                                                         */
 int ygz_vo_stream_record_bound(const ygz_vo* vo, size_t* bytes);
 /* the whole state of `stream` as a record in buf[0 .. *size).  Synchronous: it synchronises the context.
  *  - The stream must have no queued frame and no pending key-frame insertion (ygz_vo_flush first), so that every frame
@@ -281,11 +314,12 @@ int ygz_vo_save_stream(ygz_vo* vo, int stream, void* buf, size_t capacity, size_
  *  - The engine may differ from the saved one in n_streams, window, key-frame policy and min_inliers (the destination's
  *    apply from here on), in the stream index and in its context and device.  It must match it in image size, grid
  *    cells, pyramid levels and ref_mode, and the destination stream's camera (ygz_vo_get_camera) must equal the
- *    record's K bit for bit, and its lens (ygz_vo_get_lens) the record's lens, or have none for a version-1 record.
+ *    record's K bit for bit, its lens (ygz_vo_get_lens) the record's lens, or have none for a version-1 record, and its
+ *    frame format (ygz_vo_get_frame_format) the record's, or be the default for a version-1 or -2 record.
  *  - The record is checked whole on the host before anything is enqueued.
  * Asynchronous like ygzb_tracker_import; `buf` may be released when the call returns.  YGZB_ERR_INVALID, with the
  * stream exactly as before, for a NULL vo or buf, a stream out of range or with queued frames or a pending insertion,
- * a wrong magic or version, a size that is not the record's, a different geometry, K, lens or ref_mode, a count, entry,
+ * a wrong magic or version, a size that is not the record's, a different geometry, K, lens, format or ref_mode, a count, entry,
  * level or pose out of range, or a host state no saved stream can have (e.g. frames pushed but no key-frame, key-frames
  * but no frame pushed, map sections that disagree with the host state).                                            */
 int ygz_vo_load_stream(ygz_vo* vo, int stream, const void* buf, size_t size);

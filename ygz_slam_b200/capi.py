@@ -47,7 +47,7 @@ EXPORTS = [
     "ygzb_tracker_export_reference", "ygzb_tracker_import_reference", "ygzb_undistort_map", "ygzb_frames_set_undistort",
     "ygzb_tracker_set_start_pose", "ygzb_tracker_get_depth", "ygzb_tracker_set_observations",
     "ygzb_sparse_align_fisher", "ygzb_tracker_set_information", "ygzb_tracker_set_map_updates", "ygzb_tracker_set_camera",
-    "ygzb_tracker_set_undistort", "ygzb_tracker_upload_stream",
+    "ygzb_tracker_set_undistort", "ygzb_tracker_upload_stream", "ygzb_tracker_set_source",
 ]
 
 
@@ -891,6 +891,7 @@ class Tracker:
         self.lib.ygzb_tracker_upload.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
         self.lib.ygzb_tracker_set_undistort.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         self.lib.ygzb_tracker_upload_stream.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
+        self.lib.ygzb_tracker_set_source.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]
         self.lib.ygzb_tracker_track.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         self.lib.ygzb_tracker_make_keyframes.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         self.lib.ygzb_tracker_debug_job.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
@@ -1004,9 +1005,15 @@ class Tracker:
             raise ValueError(f"maps must be ({H}, {W}, 2) int16 and ({H}, {W}) uint16, not {map_xy.shape} and {map_a.shape}")
         self.ctx.check(self.lib.ygzb_tracker_set_undistort(self.h, int(stream), _p(map_xy), _p(map_a)), "ygzb_tracker_set_undistort")
 
+    def set_source(self, stream: int, width: int, height: int, channels: int = 1):
+        """The raw frames upload_stream takes for `stream` (ygzb_tracker_set_source): width x height, grey (channels 1) or
+        BGR (3); a size other than the context's needs the stream's maps (set_undistort)."""
+        self.ctx.check(self.lib.ygzb_tracker_set_source(self.h, int(stream), int(width), int(height), int(channels)),
+                       "ygzb_tracker_set_source")
+
     def upload_stream(self, stream: int, first: int, images):
-        """Raw grey frames (n, H, W) of `stream` into slots [first, first + n), remapped through the stream's maps if it
-        has any (ygzb_tracker_upload_stream)."""
+        """Raw frames of `stream` in its format (set_source; by default grey (n, H, W), BGR (n, h, w, 3)) into slots
+        [first, first + n), remapped through the stream's maps if it has any (ygzb_tracker_upload_stream)."""
         images = np.ascontiguousarray(images, np.uint8)
         if images.ndim == 2:
             images = images[None]

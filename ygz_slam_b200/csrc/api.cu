@@ -422,7 +422,8 @@ void* ygzb_frames_device_ptr(ygzb_frames* f) { return f ? f->d_pyr : nullptr; }
 int ygzb_frames_build_pyramid(ygzb_frames* f, int first, int count) {
     if (!f || first < 0 || count < 0 || first + count > f->capacity) return YGZB_ERR_INVALID;
     cudaSetDevice(f->ctx->device);
-    return launch_pyramid(f, first, count, nullptr, 1, nullptr, nullptr);
+    const RawFormat l0{f->ctx->geo.lv[0].w, f->ctx->geo.lv[0].h, 1};
+    return launch_pyramid(f, first, count, nullptr, l0, nullptr, nullptr);
 }
 
 int ygzb_frames_copy(ygzb_frames* f, int src_slot, int dst_slot) {
@@ -454,16 +455,16 @@ int stage_frames(ygzb_ctx* ctx, uint8_t* dst, const uint8_t* src, int count, siz
     return YGZB_OK;
 }
 
-// undistorting upload: the raw frames go to the pool's staging buffer, remap_gray_kernel writes level 0 through the maps
-// (the pool's, or a tracker stream's: ygzb_tracker_set_undistort).  The buffer is the
-// pool's own, not a context scratch buffer, because a tracker uploads on its front stream while the context's stream runs a
-// local BA; e_stage, recorded behind every remap on whichever stream ran it, orders each reuse of the buffer behind the
-// last read of it.
-int upload_undistorted(ygzb_frames* f, int first, int count, const uint8_t* src, int channels, size_t frame_stride, const short2* map_xy,
-                       const uint16_t* map_a) {
+// staged upload: the raw frames go to the pool's staging buffer, and remap_gray_kernel (through the maps: the pool's, or a
+// tracker stream's, ygzb_tracker_set_undistort) or bgr2gray_kernel writes level 0.  The buffer is the pool's own, not a
+// context scratch buffer, because a tracker uploads on its front stream while the context's stream runs a local BA; e_stage,
+// recorded behind every kernel that reads the buffer on whichever stream ran it, orders each reuse of the buffer (a copy
+// into it, or its reallocation) behind the last read of it, so a frame in flight is never overwritten.
+int upload_staged(ygzb_frames* f, int first, int count, const uint8_t* src, RawFormat fmt, size_t frame_stride, const short2* map_xy,
+                  const uint16_t* map_a) {
     ygzb_ctx* ctx = f->ctx;
-    const Geometry& g = ctx->geo;
-    const size_t frame = (size_t)g.lv[0].w * g.lv[0].h * channels, bytes = frame * count;
+    const size_t frame = fmt.bytes(), bytes = frame * count;
+    if (!f->e_stage) YGZB_CUDA(ctx, cudaEventCreateWithFlags(&f->e_stage, cudaEventDisableTiming));
     if (f->stage_bytes < bytes) {
         YGZB_CUDA(ctx, cudaEventSynchronize(f->e_stage));
         if (f->d_stage) cudaFree(f->d_stage);
@@ -474,7 +475,7 @@ int upload_undistorted(ygzb_frames* f, int first, int count, const uint8_t* src,
     }
     YGZB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, f->e_stage, 0));
     int rc = stage_frames(ctx, f->d_stage, src, count, frame, frame_stride);
-    if (rc == YGZB_OK) rc = launch_pyramid(f, first, count, f->d_stage, channels, map_xy, map_a);
+    if (rc == YGZB_OK) rc = launch_pyramid(f, first, count, f->d_stage, fmt, map_xy, map_a);
     // recorded even after a failed launch: a copy into the buffer may be in flight
     const int rc_ev = check_cuda(ctx, cudaEventRecord(f->e_stage, ctx->stream), "cudaEventRecord");
     return rc != YGZB_OK ? rc : rc_ev;
@@ -482,51 +483,44 @@ int upload_undistorted(ygzb_frames* f, int first, int count, const uint8_t* src,
 
 }  // namespace
 
-int ygzb::frames_upload(ygzb_frames* f, int first, int count, const uint8_t* host, int channels, size_t frame_stride, const short2* map_xy,
+int ygzb::frames_upload(ygzb_frames* f, int first, int count, const uint8_t* host, RawFormat src, size_t frame_stride, const short2* map_xy,
                         const uint16_t* map_a) {
     if (!f || !host || first < 0 || count < 0 || first + count > f->capacity) return YGZB_ERR_INVALID;
     ygzb_ctx* ctx = f->ctx;
     const Geometry& g = ctx->geo;
     cudaSetDevice(ctx->device);
-    const size_t row = (size_t)g.lv[0].w * channels;
-    if (channels != 1 && channels != 3) return set_error(ctx, YGZB_ERR_INVALID, "channels must be 1 or 3");
-    if (frame_stride < row * g.lv[0].h) return set_error(ctx, YGZB_ERR_INVALID, "frame_stride smaller than one image");
+    if (src.channels != 1 && src.channels != 3) return set_error(ctx, YGZB_ERR_INVALID, "channels must be 1 or 3");
+    if (src.w < 1 || src.h < 1) return set_error(ctx, YGZB_ERR_INVALID, "raw frame size %d x %d", src.w, src.h);
+    if ((src.w != g.lv[0].w || src.h != g.lv[0].h) && !map_xy)
+        return set_error(ctx, YGZB_ERR_INVALID, "a raw frame of %d x %d needs undistortion maps to become level 0 (%d x %d)", src.w, src.h,
+                         g.lv[0].w, g.lv[0].h);
+    if (frame_stride < src.bytes()) return set_error(ctx, YGZB_ERR_INVALID, "frame_stride smaller than one image");
     if (count == 0) return YGZB_OK;
-    if (map_xy) return upload_undistorted(f, first, count, host, channels, frame_stride, map_xy, map_a);
+    if (map_xy || src.channels == 3) return upload_staged(f, first, count, host, src, frame_stride, map_xy, map_a);
+    // a grey frame of level 0's size, straight into the slots.
     // cudaMemcpyDefault: `host` may also be a device pointer (frames already resident in HBM, unified addressing).
     // A strided batch copy treats one image as a "row", so its pitch is limited (cudaDeviceProp::memPitch, 2^31 - 1):
     // longer strides (a stacked [stream][frame] array of thousands of frames) fall back to one copy per image.
-    const bool one_copy = frame_stride <= (size_t)0x7FFFFFFF;
-    if (channels == 1) {
-        uint8_t* dst = f->d_pyr + (size_t)first * ctx->slot_stride + g.lv[0].off;
-        if (g.lv[0].pitch == g.lv[0].w && one_copy) {
-            // level 0 of a slot is one contiguous run: a single strided copy moves the whole batch
-            YGZB_CUDA(ctx, cudaMemcpy2DAsync(dst, ctx->slot_stride, host, frame_stride, row * g.lv[0].h, count, cudaMemcpyDefault,
-                                             ctx->stream));
-        } else {
-            for (int i = 0; i < count; ++i)
-                YGZB_CUDA(ctx, cudaMemcpy2DAsync(dst + (size_t)i * ctx->slot_stride, g.lv[0].pitch, host + (size_t)i * frame_stride,
-                                                 row, row, g.lv[0].h, cudaMemcpyDefault, ctx->stream));
-        }
-        return launch_pyramid(f, first, count, nullptr, 1, nullptr, nullptr);
-    }
-    uint8_t* d_bgr = (uint8_t*)dev_scratch(ctx, 0, (size_t)count * row * g.lv[0].h);
-    if (!d_bgr) return YGZB_ERR_CUDA;
-    if (one_copy) {
-        YGZB_CUDA(ctx, cudaMemcpy2DAsync(d_bgr, row * g.lv[0].h, host, frame_stride, row * g.lv[0].h, count, cudaMemcpyDefault,
+    const size_t row = (size_t)g.lv[0].w;
+    uint8_t* dst = f->d_pyr + (size_t)first * ctx->slot_stride + g.lv[0].off;
+    if (g.lv[0].pitch == g.lv[0].w && frame_stride <= (size_t)0x7FFFFFFF) {
+        // level 0 of a slot is one contiguous run: a single strided copy moves the whole batch
+        YGZB_CUDA(ctx, cudaMemcpy2DAsync(dst, ctx->slot_stride, host, frame_stride, row * g.lv[0].h, count, cudaMemcpyDefault,
                                          ctx->stream));
     } else {
         for (int i = 0; i < count; ++i)
-            YGZB_CUDA(ctx, cudaMemcpyAsync(d_bgr + (size_t)i * row * g.lv[0].h, host + (size_t)i * frame_stride, row * g.lv[0].h,
-                                           cudaMemcpyDefault, ctx->stream));
+            YGZB_CUDA(ctx, cudaMemcpy2DAsync(dst + (size_t)i * ctx->slot_stride, g.lv[0].pitch, host + (size_t)i * frame_stride,
+                                             row, row, g.lv[0].h, cudaMemcpyDefault, ctx->stream));
     }
-    return launch_pyramid(f, first, count, d_bgr, 3, nullptr, nullptr);
+    return launch_pyramid(f, first, count, nullptr, src, nullptr, nullptr);
 }
 
 extern "C" {
 
 int ygzb_frames_upload(ygzb_frames* f, int first, int count, const uint8_t* host, int channels, size_t frame_stride) {
-    return f ? frames_upload(f, first, count, host, channels, frame_stride, f->undistort ? f->d_map_xy : nullptr, f->d_map_a) : YGZB_ERR_INVALID;
+    if (!f) return YGZB_ERR_INVALID;
+    const RawFormat src{f->ctx->geo.lv[0].w, f->ctx->geo.lv[0].h, channels};
+    return frames_upload(f, first, count, host, src, frame_stride, f->undistort ? f->d_map_xy : nullptr, f->d_map_a);
 }
 
 int ygzb_frames_set_undistort(ygzb_frames* f, const int16_t* map_xy, const uint16_t* map_a) {

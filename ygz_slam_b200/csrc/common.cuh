@@ -96,13 +96,14 @@ struct ygzb_frames {
     int32_t* d_offsets;               // [capacity+1]
     int last_n;
     // lens undistortion (ygzb_frames_set_undistort): OpenCV fixed-point maps, [H][W] each, and the pool's own staging of the
-    // raw frames a remap reads (uploads run on the context's stream and on a tracker's front stream: no shared scratch)
+    // raw frames a remap or a BGR conversion reads (uploads run on the context's stream and on a tracker's front stream: no
+    // shared scratch)
     bool undistort;                   // maps set: uploads remap level 0
     short2* d_map_xy;
     uint16_t* d_map_a;
     uint8_t* d_stage;
     size_t stage_bytes;
-    cudaEvent_t e_stage;              // recorded behind the last remap, on whichever stream ran it: reuse of d_stage waits for it
+    cudaEvent_t e_stage;              // recorded behind the last read of d_stage, on whichever stream ran it: reuse waits for it
 };
 
 namespace ygzb {
@@ -172,13 +173,21 @@ struct ProfScope {
 };
 
 // ---- stage launchers (one .cu each) -----------------------------------------------------------
-// d_src = raw frames staged on the device (`channels` 1 or 3) or null (level 0 already in the slots); map_xy != NULL: level
-// 0 = remap_gray_kernel of d_src through the undistortion maps map_xy / map_a, otherwise d_src must be BGR (bgr2gray_kernel)
-int launch_pyramid(ygzb_frames* f, int first, int count, const uint8_t* d_src, int channels, const short2* map_xy, const uint16_t* map_a);
-// ygzb_frames_upload through the undistortion maps map_xy / map_a (device memory, [H][W] each: the pool's or a tracker
-// stream's), or with none (map_xy == NULL: images that are undistorted already, e.g. the key-frame and reference images of
-// the tracker's records, or frames without a lens); a remap stages the raw frames in the pool's d_stage behind e_stage
-int frames_upload(ygzb_frames* f, int first, int count, const uint8_t* host, int channels, size_t frame_stride, const short2* map_xy,
+// the raw frames an upload reads: w x h pixels of `channels` bytes (1 grey, 3 BGR), rows packed
+struct RawFormat {
+    int w, h, channels;
+    size_t bytes() const { return (size_t)w * h * channels; }
+};
+// d_src = raw frames of format `src` staged on the device, packed, or null (level 0 already in the slots); map_xy != NULL:
+// level 0 = remap_gray_kernel of d_src through the undistortion maps map_xy / map_a (level 0's size, whatever src's),
+// otherwise d_src must be BGR of level 0's size (bgr2gray_kernel)
+int launch_pyramid(ygzb_frames* f, int first, int count, const uint8_t* d_src, RawFormat src, const short2* map_xy, const uint16_t* map_a);
+// ygzb_frames_upload of frames of format `src` through the undistortion maps map_xy / map_a (device memory, [H][W] each:
+// the pool's or a tracker stream's), or with none (map_xy == NULL: images that are undistorted already, e.g. the key-frame
+// and reference images of the tracker's records, or frames without a lens).  A remap and a BGR conversion stage the raw
+// frames in the pool's d_stage behind e_stage; a grey frame without maps is copied into level 0.  A size other than level
+// 0's needs maps
+int frames_upload(ygzb_frames* f, int first, int count, const uint8_t* host, RawFormat src, size_t frame_stride, const short2* map_xy,
                   const uint16_t* map_a);
 int launch_pyrdown_ptrs(ygzb_ctx* ctx, const uint8_t* const* d_src_ptr, uint8_t* const* d_dst_ptr, int sw, int sh, int spitch,
                         int dw, int dh, int dpitch, int count);

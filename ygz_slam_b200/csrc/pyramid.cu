@@ -9,7 +9,9 @@
 //
 // With undistortion maps on the pool (ygzb_frames_set_undistort), level 0 is instead
 //     cv::remap(gray, map_xy, map_a, INTER_LINEAR, BORDER_CONSTANT, 0)      (remap_gray_kernel, the BGR conversion per tap)
-// of the raw frames staged in the pool's own buffer; the pyramid kernels are the same.
+// of the raw frames staged in the pool's own buffer; the pyramid kernels are the same.  A tracker stream's maps
+// (ygzb_tracker_set_undistort) may read raw frames of another size than level 0 (ygzb_tracker_set_source): the maps have
+// level 0's size and the taps are bounded by the raw frame's.
 //
 // Layout: every frame slot holds all levels back to back, each level pitch-linear with a 16-byte
 // multiple pitch (so level rows can be moved with 16-byte vectors / TMA boxes).
@@ -253,12 +255,12 @@ __global__ void __launch_bounds__(256) bgr2gray_kernel(const uint8_t* __restrict
     }
 }
 
-// one tap of the remap: the grey value of source pixel (x, y), 0 outside the image (BORDER_CONSTANT, value 0); a BGR tap is
+// one tap of the remap: the grey value of source pixel (x, y) of a w x h frame, 0 outside it (BORDER_CONSTANT, value 0); a BGR tap is
 // converted with bgr2gray_kernel's formula, so that the result is cv::remap(cv::cvtColor(image))
 template <int C>
 __device__ __forceinline__ int remap_tap(const uint8_t* __restrict__ img, int x, int y, int w, int h) {
     if ((unsigned)x >= (unsigned)w || (unsigned)y >= (unsigned)h) return 0;
-    const uint8_t* p = img + ((size_t)y * w + x) * C;
+    const uint8_t* p = img + ((size_t)y * w + x) * C;   // rows packed: w * C bytes
     if (C == 1) return p[0];
     return (p[0] * 3735 + p[1] * 19235 + p[2] * 9798 + (1 << 14)) >> 15;
 }
@@ -274,13 +276,14 @@ __device__ __forceinline__ uint8_t remap_pixel(const uint8_t* __restrict__ img, 
 }
 
 // cv::remap(src, map_xy, map_a, INTER_LINEAR, BORDER_CONSTANT, 0) with OpenCV's fixed-point maps (CV_16SC2 + CV_16UC1), of a grey
-// (C = 1) or BGR (C = 3) frame, 4 adjacent output pixels per thread.  OpenCV's weight table entry (fy, fx) is
+// (C = 1) or BGR (C = 3) frame of sw x sh pixels (rows packed, sw * C bytes; any size: the maps have the output's size, l0,
+// and only the taps read the source), 4 adjacent output pixels per thread.  OpenCV's weight table entry (fy, fx) is
 //   32 * {(32 - fx)(32 - fy), fx (32 - fy), (32 - fx) fy, fx fy}        (the float products (1 - x)(1 - y) .. scaled by 2^15)
 // and the result (sum w p + 2^14) >> 15.  The products are exact, so the table is this formula, except entry 0, whose 32768
 // saturates to 32767 in OpenCV's int16 table before the rounding correction moves the missing unit to another tap; with 8-bit
 // taps that cannot change a result (32768 p0 + d + 2^14 with |d| <= 255 has the same quotient), so no table is read.
 template <int C>
-__global__ void __launch_bounds__(256) remap_gray_kernel(const uint8_t* __restrict__ src, size_t src_frame_stride,
+__global__ void __launch_bounds__(256) remap_gray_kernel(const uint8_t* __restrict__ src, size_t src_frame_stride, int sw, int sh,
                                                          const short2* __restrict__ map_xy, const uint16_t* __restrict__ map_a,
                                                          uint8_t* __restrict__ pyr, size_t slot_stride, int first_slot, LevelGeom l0) {
     const int quads_per_row = (l0.w + 3) / 4;
@@ -300,19 +303,19 @@ __global__ void __launch_bounds__(256) remap_gray_kernel(const uint8_t* __restri
         uint32_t packed = 0;
 #pragma unroll
         for (int j = 0; j < 4; ++j)
-            packed |= (uint32_t)remap_pixel<C>(img, (short)(xy[j] & 0xFFFF), (short)(xy[j] >> 16), (int)a[j], l0.w, l0.h) << (8 * j);
+            packed |= (uint32_t)remap_pixel<C>(img, (short)(xy[j] & 0xFFFF), (short)(xy[j] >> 16), (int)a[j], sw, sh) << (8 * j);
         *reinterpret_cast<uint32_t*>(out) = packed;
         return;
     }
     for (int j = 0; j < 4 && x + j < l0.w; ++j) {
         const short2 s = map_xy[m + j];
-        out[j] = remap_pixel<C>(img, s.x, s.y, map_a[m + j], l0.w, l0.h);
+        out[j] = remap_pixel<C>(img, s.x, s.y, map_a[m + j], sw, sh);
     }
 }
 
 }  // namespace
 
-int launch_pyramid(ygzb_frames* f, int first, int count, const uint8_t* d_src, int channels, const short2* map_xy, const uint16_t* map_a) {
+int launch_pyramid(ygzb_frames* f, int first, int count, const uint8_t* d_src, RawFormat src, const short2* map_xy, const uint16_t* map_a) {
     ygzb_ctx* ctx = f->ctx;
     const Geometry& g = ctx->geo;
     if (count <= 0) return YGZB_OK;
@@ -320,13 +323,13 @@ int launch_pyramid(ygzb_frames* f, int first, int count, const uint8_t* d_src, i
         // undistortion (ygzb_frames_set_undistort, ygzb_tracker_set_undistort): level 0 = remap of the staged raw frames, in
         // place of bgr2gray_kernel
         const int quads = ((g.lv[0].w + 3) / 4) * g.lv[0].h;
-        const size_t frame = (size_t)g.lv[0].w * g.lv[0].h * channels;
+        const size_t frame = src.bytes();
         dim3 grid((quads + 255) / 256, count);
         ProfScope ps(ctx, kStageBgr2Gray);
-        if (channels == 3)
-            remap_gray_kernel<3><<<grid, 256, 0, ctx->stream>>>(d_src, frame, map_xy, map_a, f->d_pyr, ctx->slot_stride, first, g.lv[0]);
+        if (src.channels == 3)
+            remap_gray_kernel<3><<<grid, 256, 0, ctx->stream>>>(d_src, frame, src.w, src.h, map_xy, map_a, f->d_pyr, ctx->slot_stride, first, g.lv[0]);
         else
-            remap_gray_kernel<1><<<grid, 256, 0, ctx->stream>>>(d_src, frame, map_xy, map_a, f->d_pyr, ctx->slot_stride, first, g.lv[0]);
+            remap_gray_kernel<1><<<grid, 256, 0, ctx->stream>>>(d_src, frame, src.w, src.h, map_xy, map_a, f->d_pyr, ctx->slot_stride, first, g.lv[0]);
         YGZB_LAUNCHED(ctx);
     } else if (d_src) {
         const uint8_t* d_bgr = d_src;

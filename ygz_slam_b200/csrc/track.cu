@@ -78,6 +78,7 @@ struct ygzb_tracker {
     std::vector<uint8_t*> d_lens, h_lens;
     std::vector<cudaEvent_t> e_lens;
     std::vector<char> has_lens;    // maps set: ygzb_tracker_upload_stream remaps level 0
+    std::vector<RawFormat> src;    // per stream: the raw frames ygzb_tracker_upload_stream reads (ygzb_tracker_set_source)
 };
 
 namespace {
@@ -1061,6 +1062,7 @@ int ygzb_tracker_create(ygzb_frames* f, int n_streams, int max_jobs, const doubl
         t->h_lens.assign(S, nullptr);
         t->e_lens.assign(S, nullptr);
         t->has_lens.assign(S, 0);
+        t->src.assign(S, RawFormat{st.W, st.H, 1});
     }
     if (rc == YGZB_OK) rc = dalloc(ctx, &t->d_kfres, S);
     // (a result record carries YGZB_TRACK_RING pose slots and only the first n_local are written by a job: the whole record is
@@ -1288,17 +1290,32 @@ int ygzb_tracker_set_undistort(ygzb_tracker* t, int stream, const int16_t* map_x
     return YGZB_OK;
 }
 
+int ygzb_tracker_set_source(ygzb_tracker* t, int stream, int width, int height, int channels) {
+    if (!t) return YGZB_ERR_INVALID;
+    ygzb_ctx* ctx = t->ctx;
+    if (stream < 0 || stream >= t->st.S) return set_error(ctx, YGZB_ERR_INVALID, "set_source: stream %d out of range", stream);
+    // (the maps' int16 source coordinates reach 32767)
+    if (width < 1 || height < 1 || width > 32767 || height > 32767)
+        return set_error(ctx, YGZB_ERR_INVALID, "set_source: a raw frame of %d x %d is not within 1 .. 32767 each way", width, height);
+    if (channels != 1 && channels != 3) return set_error(ctx, YGZB_ERR_INVALID, "set_source: channels must be 1 or 3, not %d", channels);
+    // read when an upload is enqueued, so the uploads enqueued before the call read the old format and those after it the new
+    // one, in order on the front stream like the maps (ygzb_tracker_set_undistort)
+    t->src[stream] = RawFormat{width, height, channels};
+    return YGZB_OK;
+}
+
 // on the front stream, behind the last key-frame insertion (which still reads the frame slots of the previous window) and
-// behind the last tracking chain (ditto); NOT behind a local BA in flight.  map_xy / map_a: the undistortion maps of level
-// 0, or NULL
-static int upload_front(ygzb_tracker* t, int first, int count, const uint8_t* host, size_t frame_stride, const short2* map_xy, const uint16_t* map_a) {
+// behind the last tracking chain (ditto); NOT behind a local BA in flight.  Frames of format `src`; map_xy / map_a: the
+// undistortion maps of level 0, or NULL
+static int upload_front(ygzb_tracker* t, int first, int count, const uint8_t* host, RawFormat src, size_t frame_stride, const short2* map_xy,
+                        const uint16_t* map_a) {
     ygzb_ctx* ctx = t->ctx;
     cudaSetDevice(ctx->device);
     YGZB_CUDA(ctx, cudaStreamWaitEvent(t->front, t->e_fill, 0));
     YGZB_CUDA(ctx, cudaStreamWaitEvent(t->front, t->e_main, 0));
     cudaStream_t main = ctx->stream;
     ctx->stream = t->front;
-    int rc = frames_upload(t->f, first, count, host, 1, frame_stride, map_xy, map_a);
+    int rc = frames_upload(t->f, first, count, host, src, frame_stride, map_xy, map_a);
     if (rc == YGZB_OK) rc = check_cuda(ctx, cudaEventRecord(t->e_up, ctx->stream), "cudaEventRecord");
     ctx->stream = main;
     return rc;
@@ -1307,19 +1324,24 @@ static int upload_front(ygzb_tracker* t, int first, int count, const uint8_t* ho
 int ygzb_tracker_upload(ygzb_tracker* t, int first, int count, const uint8_t* host, size_t frame_stride) {
     if (!t) return YGZB_ERR_INVALID;
     ygzb_frames* f = t->f;
-    return upload_front(t, first, count, host, frame_stride, f->undistort ? f->d_map_xy : nullptr, f->d_map_a);
+    return upload_front(t, first, count, host, RawFormat{t->st.W, t->st.H, 1}, frame_stride, f->undistort ? f->d_map_xy : nullptr, f->d_map_a);
 }
 
 int ygzb_tracker_upload_stream(ygzb_tracker* t, int stream, int first, int count, const uint8_t* host, size_t frame_stride) {
     if (!t) return YGZB_ERR_INVALID;
     ygzb_ctx* ctx = t->ctx;
     if (stream < 0 || stream >= t->st.S) return set_error(ctx, YGZB_ERR_INVALID, "upload_stream: stream %d out of range", stream);
-    if (!t->has_lens[stream]) return ygzb_tracker_upload(t, first, count, host, frame_stride);
-    if (t->f->undistort)
+    const RawFormat src = t->src[stream];
+    const bool grey_l0 = src.w == t->st.W && src.h == t->st.H && src.channels == 1;
+    if (!t->has_lens[stream] && grey_l0) return ygzb_tracker_upload(t, first, count, host, frame_stride);
+    ygzb_frames* f = t->f;
+    if (!t->has_lens[stream])   // a BGR frame of level 0's size: converted, or remapped through the pool's maps
+        return upload_front(t, first, count, host, src, frame_stride, f->undistort ? f->d_map_xy : nullptr, f->d_map_a);
+    if (f->undistort)
         return set_error(ctx, YGZB_ERR_INVALID, "upload_stream: stream %d and the frame pool both have undistortion maps", stream);
     const uint8_t* d = t->d_lens[stream];
     const size_t n = (size_t)t->st.W * t->st.H;
-    return upload_front(t, first, count, host, frame_stride, reinterpret_cast<const short2*>(d),
+    return upload_front(t, first, count, host, src, frame_stride, reinterpret_cast<const short2*>(d),
                         reinterpret_cast<const uint16_t*>(d + lens_a_offset(n)));
 }
 
@@ -1627,7 +1649,7 @@ int ygzb_tracker_import(ygzb_tracker* t, int stream, const int32_t* entries, con
     }
     const size_t WH = (size_t)st.W * st.H;
     // the record's images are level 0 of key-frames, undistorted already: the pool's undistortion maps must not warp them again
-    for (int k = 0; k < n && rc == YGZB_OK; ++k) rc = frames_upload(t->f, kf_slots[k], 1, in->image + k * WH, 1, WH, nullptr, nullptr);
+    for (int k = 0; k < n && rc == YGZB_OK; ++k) rc = frames_upload(t->f, kf_slots[k], 1, in->image + k * WH, RawFormat{st.W, st.H, 1}, WH, nullptr, nullptr);
     if (rc == YGZB_OK) rc = check_cuda(ctx, cudaEventRecord(t->e_fill, ctx->stream), "cudaEventRecord");
     return rc;
 }
@@ -1707,7 +1729,7 @@ int ygzb_tracker_import_reference(ygzb_tracker* t, int stream, const ygzb_refere
         YGZB_LAUNCHED(ctx);
     }
     const size_t WH = (size_t)st.W * st.H;
-    rc = frames_upload(t->f, t->ref_slots[stream], 1, in->image, 1, WH, nullptr, nullptr);   // undistorted already, like a map record's images
+    rc = frames_upload(t->f, t->ref_slots[stream], 1, in->image, RawFormat{st.W, st.H, 1}, WH, nullptr, nullptr);   // undistorted already, like a map record's images
     if (rc == YGZB_OK) rc = check_cuda(ctx, cudaEventRecord(t->e_fill, ctx->stream), "cudaEventRecord");
     if (rc != YGZB_OK) return rc;
     t->cur_ref[stream] = t->ref_slots[stream];

@@ -577,10 +577,17 @@ struct Lens {
         return on == o.on && (!on || (std::memcmp(K.data(), o.K.data(), sizeof K) == 0 && std::memcmp(dist.data(), o.dist.data(), sizeof dist) == 0));
     }
 };
+// the frames a stream pushes (ygz_vo_set_frame_format): w x h pixels of `channels` bytes (1 grey, 3 BGR), rows packed
+struct Format {
+    int w = 0, h = 0, channels = 1;
+    size_t bytes() const { return (size_t)w * h * channels; }
+    bool operator==(const Format&) const = default;
+};
 struct SeqStart {
     Mat34 T;                  // pose of the sequence's first key-frame
     Camera K;                 // camera of the sequence
     Lens lens;                // lens of the sequence
+    Format fmt;               // frame format of the sequence
 };
 struct EStream : Counters {
     std::deque<KfInfo> kfs;   // at most YGZB_TRACK_RING, the newest is the reference key-frame; the last kLocalKeyframes are local
@@ -589,6 +596,7 @@ struct EStream : Counters {
     Mat34 start = identity(); // pose of the next sequence's first key-frame (ygz_vo_restart)
     Camera cam{};             // camera of the current sequence, or of the next one while a restart is pending (ygz_vo_set_camera)
     Lens lens;                // lens of the current sequence, or of the next one while a restart is pending (ygz_vo_set_lens)
+    Format fmt;               // frame format of the current sequence, or of the next one ... (ygz_vo_set_frame_format)
     std::deque<SeqStart> starts;   // the queued frames that start a sequence (the stream's first, restarts), in order
     bool has_pose = false, lost = false, has_depth = false;
     bool restart_pending = false;   // the next push starts a new sequence at `start`
@@ -747,6 +755,8 @@ class Engine {
         CHK(ygzb_get_params(ctx_, &cp));
         W_ = cp.image_width;
         H_ = cp.image_height;
+        for (EStream& s : st_) s.fmt = default_format();
+        tr_fmt_.assign(S_, default_format());
         int rows = 0, cols = 0;
         CHK(ygzb_grid_dims(ctx_, &rows, &cols));
         ring_cells_ = (size_t)YGZB_TRACK_RING * rows * cols;
@@ -784,7 +794,7 @@ class Engine {
         QFrame f{image, depth, tag, stacked};
         if (pushed(i) == 0 || s.restart_pending) {
             f.restart = s.restart_pending;
-            s.starts.push_back({s.start, s.cam, s.lens});
+            s.starts.push_back({s.start, s.cam, s.lens, s.fmt});
             s.restart_pending = false;
         }
         s.queue.push_back(f);
@@ -823,6 +833,22 @@ class Engine {
     bool any_lens() const {
         for (const EStream& s : st_)
             if (s.lens.on) return true;
+        return false;
+    }
+    // the frame format of stream i's next sequence, at the times set_camera accepts (the caller has checked it); it reaches
+    // the tracker when the sequence's first frame is uploaded (use_format)
+    int set_frame_format(int i, const Format& F) {
+        EStream& s = st_[i];
+        if (pushed(i) > 0 && !s.restart_pending) return YGZB_ERR_INVALID;
+        s.fmt = F;
+        return YGZB_OK;
+    }
+    // the format of a stream that was never given one: grey frames of the context's size
+    Format default_format() const { return {W_, H_, 1}; }
+    // some stream has a format other than the default, now or for its next sequence: its records carry a format block
+    bool any_format() const {
+        for (const EStream& s : st_)
+            if (s.fmt != default_format()) return true;
         return false;
     }
     // final results go to `traj` (this group's [S][n_frames][12], rows in the caller's stream order; NULL: none) and, with
@@ -949,7 +975,10 @@ class Engine {
             w = std::min(w, (int)s.queue.size());
             // a sequence's lens reaches the tracker with its first frame's upload: every frame of the old sequence has been
             // uploaded before (a window never crosses a restart), and the tracker orders the maps behind those uploads
-            if (first) CHK(use_lens(i, s.starts.front().lens, s.starts.front().K));
+            if (first) {   // (the format likewise)
+                CHK(use_lens(i, s.starts.front().lens, s.starts.front().K));
+                CHK(use_format(i, s.starts.front().fmt));
+            }
             CHK(upload(i, w));
             if (first) {
                 wins_.push_back({i, s.next_frame, 1, -1});
@@ -1075,6 +1104,7 @@ class Engine {
         if (rec->n_keyframes != (int)entries.size()) return YGZB_ERR_INVALID;
         CHK(use_camera(i, s.cam));
         CHK(use_lens(i, s.lens, s.cam));
+        CHK(use_format(i, s.fmt));
         CHK(ygzb_tracker_import(tr_, i, entries.data(), slots.data(), rec));
         if (ref) CHK(ygzb_tracker_import_reference(tr_, i, ref));
         st_[i] = s;
@@ -1124,20 +1154,30 @@ class Engine {
         cur = {L, K};
         return YGZB_OK;
     }
+    // the tracker reads the raw frames of stream i in format F for every upload enqueued from here on; nothing is enqueued
+    // when it does already
+    int use_format(int i, const Format& F) {
+        if (tr_fmt_[i] == F) return YGZB_OK;
+        CHK(ygzb_tracker_set_source(tr_, i, F.w, F.h, F.channels));
+        tr_fmt_[i] = F;
+        return YGZB_OK;
+    }
     // the first w queued frames of stream i into its frame slots: one strided copy when they are equally spaced in one
     // stacked sequence, one copy per frame otherwise (frames pushed one by one may sit in separate allocations, which one
-    // strided copy cannot span even when their addresses happen to be equally spaced)
+    // strided copy cannot span even when their addresses happen to be equally spaced).  The frames are in the tracker's
+    // format of the stream (use_format), that of their sequence
     int upload(int i, int w) {
         const std::deque<QFrame>& q = st_[i].queue;
-        const size_t fb = (size_t)W_ * H_;
+        const size_t fb = tr_fmt_[i].bytes();
         const ptrdiff_t stride = w > 1 ? q[1].image - q[0].image : (ptrdiff_t)fb;
         bool strided = stride >= (ptrdiff_t)fb;
         for (int t = 0; t < w && strided; ++t) strided = q[t].stacked && (t < 2 || q[t].image - q[t - 1].image == stride);
         h2d_image_bytes += (long long)w * (long long)fb;
-        // a stream without a lens uploads exactly as before lenses existed
+        // a stream without a lens, of the default format, uploads exactly as before lenses and formats existed
+        const bool own = tr_lens_[i].lens.on || tr_fmt_[i] != default_format();
         auto up = [&](int first, int count, const uint8_t* src, size_t frame_stride) {
-            return tr_lens_[i].lens.on ? ygzb_tracker_upload_stream(tr_, i, first, count, src, frame_stride)
-                                       : ygzb_tracker_upload(tr_, first, count, src, frame_stride);
+            return own ? ygzb_tracker_upload_stream(tr_, i, first, count, src, frame_stride)
+                       : ygzb_tracker_upload(tr_, first, count, src, frame_stride);
         };
         if (strided) return up(i * F_, w, q[0].image, (size_t)stride);
         for (int t = 0; t < w; ++t) CHK(up(i * F_ + t, 1, q[t].image, fb));
@@ -1242,6 +1282,7 @@ class Engine {
         Camera K;
     };
     std::vector<TrLens> tr_lens_;  // the lens and camera the tracker's maps of every stream were built for (ygzb_tracker_set_undistort)
+    std::vector<Format> tr_fmt_;   // the tracker's raw frame format of every stream (ygzb_tracker_set_source), as last set
     std::vector<int16_t> map_xy_;  // host maps of use_lens, built for the lens and camera maps_for_ (lens off: none)
     std::vector<uint16_t> map_a_;
     TrLens maps_for_;
@@ -1294,22 +1335,25 @@ static_assert(std::endian::native == std::endian::little, "stream records are li
 constexpr uint8_t kRecordMagic[4] = {'Y', 'G', 'Z', 'S'};
 
 // what a record is made under and must be loaded under: the engine's image size, grid, pyramid, camera and reference mode,
-// and the stream's lens
+// and the stream's lens and frame format
 struct RecordGeom {
     int32_t width, height, cells, n_levels;
     double K[4];
     int32_t ref_mode;
     Lens lens{};
+    Format fmt{};   // (save and load set it; read_record's is the record's)
     size_t wh() const { return (size_t)width * height; }
+    bool default_fmt() const { return fmt == Format{width, height, 1}; }
 };
 constexpr size_t kRecordLensBytes = 9 * sizeof(double);   // version 2's lens block: K[4], dist[5]
+constexpr size_t kRecordFormatBytes = 4 * sizeof(int32_t);   // version 3's format block: width, height, channels, has_lens
 
 // the largest record of an engine: a full ring at capacity, a full reference, a depth map (the sections of write_record),
-// and with lens, a lens block
-size_t record_bound(const RecordGeom& g, bool lens) {
+// with lens, a lens block, and with fmt, a format block
+size_t record_bound(const RecordGeom& g, bool lens, bool fmt) {
     const size_t R = YGZB_TRACK_RING, F = R * g.cells, O = R * YGZB_MAP_OBS_PER_CELL * g.cells;
     const size_t C = (size_t)YGZB_TRACK_REF_FEATURES_PER_CELL * g.cells, WH = g.wh();
-    return 68 + (lens ? kRecordLensBytes : 0)                   // header, lens
+    return 68 + (fmt ? kRecordFormatBytes : 0) + (lens ? kRecordLensBytes : 0)   // header, format, lens
            + (4 + R * 116 + 2 * 96 + 4 + 16 + 12 * 8)           // host state
            + (4 + R * (116 + WH) + F * 49 + O * 24)             // map
            + (4 + 96 + C * 24 + WH)                             // reference
@@ -1354,13 +1398,17 @@ void write_record(RecordWriter& w, const RecordGeom& g, const EStream& s, const 
     const size_t WH = g.wh();
     // 1. header (the size is written last)
     w.bytes(kRecordMagic, 4);
-    w.put<uint32_t>(g.lens.on ? YGZ_VO_STREAM_RECORD_VERSION_LENS : YGZ_VO_STREAM_RECORD_VERSION);
+    const bool v3 = !g.default_fmt();
+    w.put<uint32_t>(v3 ? YGZ_VO_STREAM_RECORD_VERSION_FORMAT : g.lens.on ? YGZ_VO_STREAM_RECORD_VERSION_LENS : YGZ_VO_STREAM_RECORD_VERSION);
     const size_t size_at = w.n;
     w.put<uint64_t>(0);
     w.put<int32_t>(g.width); w.put<int32_t>(g.height); w.put<int32_t>(g.cells); w.put<int32_t>(g.n_levels);
     w.bytes(g.K, sizeof g.K);
     w.put<int32_t>(g.ref_mode);
-    if (g.lens.on) {   // version 2
+    if (v3) {
+        w.put<int32_t>(g.fmt.w); w.put<int32_t>(g.fmt.h); w.put<int32_t>(g.fmt.channels); w.put<int32_t>(g.lens.on);
+    }
+    if (g.lens.on) {   // version 2, or 3 with has_lens
         w.bytes(g.lens.K.data(), sizeof g.lens.K);
         w.bytes(g.lens.dist.data(), sizeof g.lens.dist);
     }
@@ -1429,14 +1477,24 @@ int read_record(const uint8_t* in, size_t size, const RecordGeom& g, StreamRecor
     r.bytes(rg.K, sizeof rg.K);
     rg.ref_mode = r.get<int32_t>();
     if (!r.ok || std::memcmp(magic, kRecordMagic, 4) != 0 || total != size) return YGZB_ERR_INVALID;
-    if (version != YGZ_VO_STREAM_RECORD_VERSION && version != YGZ_VO_STREAM_RECORD_VERSION_LENS) return YGZB_ERR_INVALID;
+    if (version != YGZ_VO_STREAM_RECORD_VERSION && version != YGZ_VO_STREAM_RECORD_VERSION_LENS &&
+        version != YGZ_VO_STREAM_RECORD_VERSION_FORMAT)
+        return YGZB_ERR_INVALID;
     rg.lens.on = version == YGZ_VO_STREAM_RECORD_VERSION_LENS;
+    rg.fmt = {rg.width, rg.height, 1};
+    if (version == YGZ_VO_STREAM_RECORD_VERSION_FORMAT) {
+        rg.fmt.w = r.get<int32_t>(); rg.fmt.h = r.get<int32_t>(); rg.fmt.channels = r.get<int32_t>();
+        const int32_t has_lens = r.get<int32_t>();
+        // (a default format is always written as version 1 or 2)
+        if (!r.ok || (has_lens != 0 && has_lens != 1) || rg.default_fmt()) return YGZB_ERR_INVALID;
+        rg.lens.on = has_lens;
+    }
     if (rg.lens.on) {
         r.bytes(rg.lens.K.data(), sizeof rg.lens.K);
         r.bytes(rg.lens.dist.data(), sizeof rg.lens.dist);
     }
     if (!r.ok || rg.width != g.width || rg.height != g.height || rg.cells != g.cells || rg.n_levels != g.n_levels || rg.ref_mode != g.ref_mode ||
-        std::memcmp(rg.K, g.K, sizeof g.K) != 0 || !rg.lens.same(g.lens))   // K and the lens bit for bit
+        std::memcmp(rg.K, g.K, sizeof g.K) != 0 || !rg.lens.same(g.lens) || rg.fmt != g.fmt)   // K and the lens bit for bit
         return YGZB_ERR_INVALID;
     // 2. host state
     EStream& s = out.s;
@@ -1859,6 +1917,9 @@ int ygz_vo_push(ygz_vo* vo, int stream, const uint8_t* image, const double* dept
     if (!vo || stream < 0 || stream >= vo->n_streams || !image) return YGZB_ERR_INVALID;
     const EStream& s = vo->eng->streams()[stream];
     if (!depth && (!s.has_depth || s.restart_pending)) return YGZB_ERR_INVALID;
+    // a sequence's first frame fixes its format and lens: a raw size other than the context's is only resampled by a lens
+    const bool starts = vo->eng->pushed(stream) == 0 || s.restart_pending;
+    if (starts && (s.fmt.w != vo->eng->width() || s.fmt.h != vo->eng->height()) && !s.lens.on) return YGZB_ERR_INVALID;
     vo->eng->push(stream, image, depth, tag);
     return YGZB_OK;
 }
@@ -1900,6 +1961,21 @@ int ygz_vo_get_lens(const ygz_vo* vo, int stream, int* has_lens, double K[4], do
     *has_lens = L.on ? 1 : 0;
     std::copy(L.K.begin(), L.K.end(), K);   // (zeros without a lens)
     std::copy(L.dist.begin(), L.dist.end(), dist);
+    return YGZB_OK;
+}
+
+int ygz_vo_set_frame_format(ygz_vo* vo, int stream, int width, int height, int channels) {
+    if (!vo || stream < 0 || stream >= vo->n_streams) return YGZB_ERR_INVALID;
+    if (width < 1 || height < 1 || width > 32767 || height > 32767 || (channels != 1 && channels != 3)) return YGZB_ERR_INVALID;
+    return vo->eng->set_frame_format(stream, Format{width, height, channels});
+}
+
+int ygz_vo_get_frame_format(const ygz_vo* vo, int stream, int* width, int* height, int* channels) {
+    if (!vo || !width || !height || !channels || stream < 0 || stream >= vo->n_streams) return YGZB_ERR_INVALID;
+    const Format& F = vo->eng->streams()[stream].fmt;
+    *width = F.w;
+    *height = F.h;
+    *channels = F.channels;
     return YGZB_OK;
 }
 
@@ -1978,7 +2054,7 @@ int ygz_vo_export_map(ygz_vo* vo, int stream, ygzb_map_record* out) {
 
 int ygz_vo_stream_record_bound(const ygz_vo* vo, size_t* bytes) {
     if (!vo || !bytes) return YGZB_ERR_INVALID;
-    *bytes = record_bound(vo->geom, vo->eng->any_lens());
+    *bytes = record_bound(vo->geom, vo->eng->any_lens(), vo->eng->any_format());
     return YGZB_OK;
 }
 
@@ -1990,9 +2066,10 @@ int ygz_vo_save_stream(ygz_vo* vo, int stream, void* buf, size_t capacity, size_
     if (!e.settled(stream)) return YGZB_ERR_INVALID;
     if (!vo->stage.mem) CHK(vo->stage.init(vo->geom));
     const EStream& s = e.streams()[stream];
-    RecordGeom g = vo->geom;   // with the stream's own camera and lens
+    RecordGeom g = vo->geom;   // with the stream's own camera, lens and frame format
     std::copy(s.cam.begin(), s.cam.end(), g.K);
     g.lens = s.lens;
+    g.fmt = s.fmt;
     SaveStage& st = vo->stage;
     CHK(e.export_map(stream, &st.map));
     const bool ref = e.has_reference(stream);
@@ -2014,15 +2091,18 @@ int ygz_vo_load_stream(ygz_vo* vo, int stream, const void* buf, size_t size) {
     if (!vo || !buf || stream < 0 || stream >= vo->n_streams) return YGZB_ERR_INVALID;
     Engine& e = *vo->eng;
     if (!e.settled(stream)) return YGZB_ERR_INVALID;
-    const Camera cam = e.streams()[stream].cam;   // the record's K and lens must be the destination stream's
+    const Camera cam = e.streams()[stream].cam;   // the record's K, lens and format must be the destination stream's
     const Lens lens = e.streams()[stream].lens;
+    const Format fmt = e.streams()[stream].fmt;
     RecordGeom g = vo->geom;
     std::copy(cam.begin(), cam.end(), g.K);
     g.lens = lens;
+    g.fmt = fmt;
     StreamRecord rec(g);
     CHK(read_record(static_cast<const uint8_t*>(buf), size, g, rec));
     rec.s.cam = cam;
     rec.s.lens = lens;
+    rec.s.fmt = fmt;
     CHK(e.check_start_pose(stream, rec.s.start));
     CHK(e.adopt(stream, rec.s, &rec.map.rec, rec.has_ref ? &rec.ref.rec : nullptr));
     if (rec.s.has_depth) CHK(e.set_depth(stream, rec.depth.data()));

@@ -122,14 +122,16 @@ def undistort_rays(u, v, dist, fx: float = FX, fy: float = FY, cx: float = CX, c
 
 
 def render_plane_lens(tex: np.ndarray, T_cw: np.ndarray, dist, plane_z: float = 2.0, metres_per_texel: float = 0.0025,
-                      noise_sigma: float = 0.0, seed: int = 1):
+                      noise_sigma: float = 0.0, seed: int = 1, raw=None):
     """render_plane through a lens: the camera K = (FX, FY, CX, CY) with radial-tangential distortion dist = (k1, k2, p1, p2[,
     k3]).  Every distorted pixel is undistorted iteratively to its ray, the ray is intersected with the plane z = plane_z and
-    the texture is sampled there.  Returns (raw distorted gray uint8 HxW, depth HxW of the UNDISTORTED pinhole camera with
-    the same K -- the depth map a tracker wants once its frame pool undistorts with newK = K)."""
+    the texture is sampled there.  raw = (width, height, (fx, fy, cx, cy)): a raw camera of its own size and K in place of
+    W x H and (FX, FY, CX, CY).  Returns (raw distorted gray uint8 of the raw camera's size, depth HxW of the UNDISTORTED
+    pinhole camera (FX, FY, CX, CY) at W x H -- the depth map a tracker wants once it resamples with newK = that camera)."""
     R, t = T_cw[:, :3], T_cw[:, 3]
-    u, v = np.meshgrid(np.arange(W, dtype=np.float64), np.arange(H, dtype=np.float64))
-    x, y = undistort_rays(u, v, dist)
+    rw_, rh_, rK = (W, H, (FX, FY, CX, CY)) if raw is None else raw
+    u, v = np.meshgrid(np.arange(rw_, dtype=np.float64), np.arange(rh_, dtype=np.float64))
+    x, y = undistort_rays(u, v, dist, *rK)
     cw = -R.T @ t
 
     def hit(rx, ry):
@@ -148,6 +150,8 @@ def render_plane_lens(tex: np.ndarray, T_cw: np.ndarray, dist, plane_z: float = 
     if noise_sigma > 0:
         val = val + np.random.default_rng(seed).normal(0, noise_sigma, val.shape)
     gray = np.clip(np.rint(val), 0, 255).astype(np.uint8)
+    if raw is not None:
+        u, v = np.meshgrid(np.arange(W, dtype=np.float64), np.arange(H, dtype=np.float64))
     _, depth = hit((u - CX) / FX, (v - CY) / FY)
     return gray, depth
 
@@ -156,14 +160,15 @@ def render_plane_lens(tex: np.ndarray, T_cw: np.ndarray, dist, plane_z: float = 
 LENS_TUM_FR2 = (0.2312, -0.7849, -0.0033, -0.0001, 0.9172)
 
 
-def lens_stream_frame(k: int, stream: int = 0, dist=LENS_TUM_FR2, noise_sigma: float = 2.0, tex_size: int = 2048):
-    """Frame k of synthetic stream `stream` (the trajectory of stream_frame) seen through the lens `dist`: (raw distorted
-    gray, depth of the undistorted camera, T_cw)."""
+def lens_stream_frame(k: int, stream: int = 0, dist=LENS_TUM_FR2, noise_sigma: float = 2.0, tex_size: int = 2048, raw=None):
+    """Frame k of synthetic stream `stream` (the trajectory of stream_frame) seen through the lens `dist` (of the raw camera
+    raw = (width, height, K), render_plane_lens; None: W x H with K = (FX, FY, CX, CY)): (raw distorted gray, depth of the
+    undistorted camera at W x H, T_cw)."""
     key = (stream, tex_size)
     if key not in _TEX_CACHE:
         _TEX_CACHE[key] = texture(0x59475A00 + stream, tex_size)
     T = trajectory(k)
-    gray, depth = render_plane_lens(_TEX_CACHE[key], T, dist, noise_sigma=noise_sigma, seed=(stream << 16) + k + 1)
+    gray, depth = render_plane_lens(_TEX_CACHE[key], T, dist, noise_sigma=noise_sigma, seed=(stream << 16) + k + 1, raw=raw)
     return gray, depth, T
 
 

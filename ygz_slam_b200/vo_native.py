@@ -43,6 +43,8 @@ def _lib():
         _LIB.ygz_vo_get_camera.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         _LIB.ygz_vo_set_lens.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         _LIB.ygz_vo_get_lens.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        _LIB.ygz_vo_set_frame_format.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]
+        _LIB.ygz_vo_get_frame_format.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         _LIB.ygz_vo_step.argtypes = [C.c_void_p]
         _LIB.ygz_vo_flush.argtypes = [C.c_void_p]
         _LIB.ygz_vo_poll.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
@@ -169,12 +171,23 @@ _COUNTERS = ("n_keyframes", "n_ba", "n_candidates", "n_projected", "n_inliers", 
 
 
 _LENS_VERSION = 2   # YGZ_VO_STREAM_RECORD_VERSION_LENS: a 72-byte lens block (K[4], dist[5]) follows the header
+# YGZ_VO_STREAM_RECORD_VERSION_FORMAT: a 16-byte format block (width, height, channels, has_lens) follows the header, then
+# the lens block if has_lens
+_FORMAT_VERSION = 3
+
+
+def _record_head(rec):
+    """Bytes before a stream record's host state: the 68-byte header and the format and lens blocks its version has."""
+    version = int(rec[4:8].view("<u4")[0])
+    if version == _FORMAT_VERSION:
+        return 68 + 16 + (72 if int(rec[80:84].view("<i4")[0]) else 0)
+    return 68 + (72 if version == _LENS_VERSION else 0)
 
 
 def stream_record_next_frame(rec):
-    """next_frame of a stream record (uint8 array) from its fixed offset: the 68-byte header, in version 2 the 72-byte lens
-    block, n_kf, n_kf key-frames of 116 bytes, the two poses, the four flags and frames_since_kf come before it."""
-    head = 68 + (72 if int(rec[4:8].view("<u4")[0]) == _LENS_VERSION else 0)
+    """next_frame of a stream record (uint8 array) from its fixed offset: the 68-byte header, the format and lens blocks of
+    its version, n_kf, n_kf key-frames of 116 bytes, the two poses, the four flags and frames_since_kf come before it."""
+    head = _record_head(rec)
     n_kf = int(rec[head:head + 4].view("<i4")[0])
     off = head + 4 + 116 * n_kf + 2 * 96 + 4 + 4
     return int(rec[off:off + 4].view("<i4")[0])
@@ -204,7 +217,11 @@ def parse_stream_record(data):
     W, H = take("width", "i4"), take("height", "i4")
     take("cells", "i4"); take("n_levels", "i4"); take("K", "f8", 4)
     mode = take("ref_mode", "i4")
-    if version == _LENS_VERSION:
+    has_lens = version == _LENS_VERSION
+    if version == _FORMAT_VERSION:
+        take("format.width", "i4"); take("format.height", "i4"); take("format.channels", "i4")
+        has_lens = bool(take("format.has_lens", "i4"))
+    if has_lens:
         take("lens.K", "f8", 4); take("lens.dist", "f8", 5)
     n_kf = take("n_kf", "i4")
     for k in range(n_kf):
@@ -247,10 +264,13 @@ class Engine:
     in the local map (ygz_vo_set_map_updates), which poll_map_updates returns.  cameras: None, or one (fx, fy, cx, cy)
     per stream (None: K), set before any push (ygz_vo_set_camera).  lenses: None, or one (K, dist) or None per stream:
     the stream's raw frames are those of camera K = (fx, fy, cx, cy) with distortion dist = (k1, k2, p1, p2, k3), and the
-    engine undistorts them on the device to the stream's camera (ygz_vo_set_lens)."""
+    engine undistorts them on the device to the stream's camera (ygz_vo_set_lens).  frame_formats: None, or one (width,
+    height, channels) or None per stream: the frames the stream pushes, grey (channels 1) or BGR (3), of the context's size
+    or, with a lens whose K is that raw camera's, of any size (ygz_vo_set_frame_format)."""
 
     def __init__(self, ctx, n_streams, window=8, ref_mode="keyframe", kf_min_frames=10, kf_min_rot=0.1, kf_min_trans=0.1,
-                 min_inliers=30, K=None, observations=False, information=False, map_updates=False, cameras=None, lenses=None):
+                 min_inliers=30, K=None, observations=False, information=False, map_updates=False, cameras=None, lenses=None,
+                 frame_formats=None):
         if ref_mode not in _REF_MODES:
             raise ValueError(f"ref_mode must be 'keyframe' or 'previous', not {ref_mode!r}")
         p = ctx.params
@@ -286,6 +306,12 @@ class Engine:
             for s, lens in enumerate(lenses):
                 if lens is not None:
                     self.set_lens(s, *lens)
+        if frame_formats is not None:
+            if len(frame_formats) != self.n_streams:
+                raise ValueError(f"frame_formats: {len(frame_formats)} formats for {self.n_streams} streams")
+            for s, fmt in enumerate(frame_formats):
+                if fmt is not None:
+                    self.set_frame_format(s, *fmt)
 
     def set_camera(self, stream, K):
         """K = (fx, fy, cx, cy) of `stream`'s next sequence (ygz_vo_set_camera): only before its first push or while a
@@ -316,6 +342,20 @@ class Engine:
         has, K, d = C.c_int(0), np.zeros(4, np.float64), np.zeros(5, np.float64)
         self.ctx.check(self.lib.ygz_vo_get_lens(self.h, int(stream), C.byref(has), K.ctypes.data, d.ctypes.data), "ygz_vo_get_lens")
         return (K, d) if has.value else None
+
+    def set_frame_format(self, stream, width, height, channels=1):
+        """The frames of `stream`'s next sequence (ygz_vo_set_frame_format): width x height, grey (channels 1) or BGR (3).
+        A size other than the context's needs a lens (set_lens) by the sequence's first push.  At the times set_camera is
+        accepted; frames pushed before the restart keep the old format."""
+        self.ctx.check(self.lib.ygz_vo_set_frame_format(self.h, int(stream), int(width), int(height), int(channels)),
+                       "ygz_vo_set_frame_format")
+
+    def frame_format(self, stream):
+        """The format (width, height, channels) set_frame_format last gave `stream` (the context's size, grey, until then)."""
+        w, h, c = C.c_int(0), C.c_int(0), C.c_int(0)
+        self.ctx.check(self.lib.ygz_vo_get_frame_format(self.h, int(stream), C.byref(w), C.byref(h), C.byref(c)),
+                       "ygz_vo_get_frame_format")
+        return w.value, h.value, c.value
 
     def set_observations(self, on):
         """Switch the observation rows of the results on or off (ygz_vo_set_observations): only while the engine is
@@ -378,14 +418,17 @@ class Engine:
         return upd, rows
 
     def push(self, stream, image, depth=None, tag=None):
-        """Queue grey `image` (H, W) uint8 of `stream` with its depth map (H, W) float64, or None to keep the stream's current
+        """Queue `image` of `stream` in the stream's frame format (frame_format: (h, w) grey or (h, w, 3) BGR uint8; by
+        default (H, W) grey) with its depth map (H, W) float64 at the context's size, or None to keep the stream's current
         map.  Returns the frame's index in its stream; tag (default: that index) comes back with its result."""
         if not 0 <= stream < self.n_streams:
             raise ValueError(f"stream {stream} out of range [0, {self.n_streams})")
         img = np.ascontiguousarray(image, np.uint8)
         dep = None if depth is None else np.ascontiguousarray(depth, np.float64)
-        if img.shape != self.shape or (dep is not None and dep.shape != self.shape):
-            raise ValueError(f"image and depth must be {self.shape}")
+        w, h, c = self.frame_format(stream)
+        shape = (h, w) if c == 1 else (h, w, c)
+        if img.shape != shape or (dep is not None and dep.shape != self.shape):
+            raise ValueError(f"image must be {shape} and depth {self.shape}, not {img.shape} and {None if dep is None else dep.shape}")
         frame = self._pushed[stream]
         tag = frame if tag is None else int(tag)
         self.ctx.check(self.lib.ygz_vo_push(self.h, int(stream), img.ctypes.data, None if dep is None else dep.ctypes.data, tag),
