@@ -72,13 +72,18 @@ struct ygzb_tracker {
     void* d_cam;
     std::vector<double> cam_K;     // [S][4]
     std::vector<float> cam_F;      // [S][4]
-    // per-stream undistortion maps (ygzb_tracker_set_undistort), allocated on a stream's first maps and kept until destroy:
-    // map_xy then map_a on the device, read only by that stream's uploads on the front stream, and their page-locked
-    // staging with an event behind its last copy
-    std::vector<uint8_t*> d_lens, h_lens;
-    std::vector<cudaEvent_t> e_lens;
-    std::vector<char> has_lens;    // maps set: ygzb_tracker_upload_stream remaps level 0
-    std::vector<RawFormat> src;    // per stream: the raw frames ygzb_tracker_upload_stream reads (ygzb_tracker_set_source)
+    // per stream: what ygzb_tracker_upload_stream reads its frames through
+    struct Source {
+        RawFormat raw;                  // the raw frames (ygzb_tracker_set_source)
+        // undistortion maps (ygzb_tracker_set_undistort), allocated on the stream's first maps and kept until destroy:
+        // map_xy then map_a on the device, read only by the stream's uploads on the front stream, and their page-locked
+        // staging with an event behind its last copy
+        uint8_t* d_maps = nullptr;
+        uint8_t* h_maps = nullptr;
+        cudaEvent_t e_maps = nullptr;
+        bool has_maps = false;          // maps set: uploads remap level 0 through them
+    };
+    std::vector<Source> sources;
 };
 
 namespace {
@@ -1058,11 +1063,7 @@ int ygzb_tracker_create(ygzb_frames* f, int n_streams, int max_jobs, const doubl
     if (rc == YGZB_OK) {
         t->start_T.assign(12 * S, 0.0);
         for (size_t s = 0; s < S; ++s) t->start_T[12 * s] = t->start_T[12 * s + 5] = t->start_T[12 * s + 10] = 1.0;
-        t->d_lens.assign(S, nullptr);
-        t->h_lens.assign(S, nullptr);
-        t->e_lens.assign(S, nullptr);
-        t->has_lens.assign(S, 0);
-        t->src.assign(S, RawFormat{st.W, st.H, 1});
+        t->sources.assign(S, {RawFormat{st.W, st.H, 1}});
     }
     if (rc == YGZB_OK) rc = dalloc(ctx, &t->d_kfres, S);
     // (a result record carries YGZB_TRACK_RING pose slots and only the first n_local are written by a job: the whole record is
@@ -1120,10 +1121,10 @@ void ygzb_tracker_destroy(ygzb_tracker* t) {
     }
     for (cudaEvent_t e : {t->e_fill, t->e_front, t->e_main, t->e_up})
         if (e) cudaEventDestroy(e);
-    for (size_t s = 0; s < t->d_lens.size(); ++s) {
-        if (t->e_lens[s]) cudaEventDestroy(t->e_lens[s]);
-        if (t->d_lens[s]) cudaFree(t->d_lens[s]);
-        if (t->h_lens[s]) cudaFreeHost(t->h_lens[s]);
+    for (const ygzb_tracker::Source& s : t->sources) {
+        if (s.e_maps) cudaEventDestroy(s.e_maps);
+        if (s.d_maps) cudaFree(s.d_maps);
+        if (s.h_maps) cudaFreeHost(s.h_maps);
     }
     delete t;
 }
@@ -1258,24 +1259,25 @@ int ygzb_tracker_set_undistort(ygzb_tracker* t, int stream, const int16_t* map_x
     ygzb_ctx* ctx = t->ctx;
     if (stream < 0 || stream >= t->st.S) return set_error(ctx, YGZB_ERR_INVALID, "set_undistort: stream %d out of range", stream);
     if (!map_xy != !map_a) return set_error(ctx, YGZB_ERR_INVALID, "set_undistort: map_xy and map_a must both be given, or both be NULL");
+    ygzb_tracker::Source& s = t->sources[stream];
     if (!map_xy) {   // uploads enqueued before keep reading the maps, which stay allocated until the tracker is destroyed
-        t->has_lens[stream] = 0;
+        s.has_maps = false;
         return YGZB_OK;
     }
     ygzb_frames* f = t->f;
     if (f->undistort) return set_error(ctx, YGZB_ERR_INVALID, "set_undistort: the frame pool has undistortion maps of its own");
     cudaSetDevice(ctx->device);
     const size_t n = (size_t)t->st.W * t->st.H, a_off = lens_a_offset(n);
-    if (!t->h_lens[stream]) {
-        YGZB_CUDA(ctx, cudaMallocHost((void**)&t->h_lens[stream], lens_bytes(n)));
-        YGZB_CUDA(ctx, cudaMalloc((void**)&t->d_lens[stream], lens_bytes(n)));
-        YGZB_CUDA(ctx, cudaEventCreateWithFlags(&t->e_lens[stream], cudaEventDisableTiming));
+    if (!s.h_maps) {
+        YGZB_CUDA(ctx, cudaMallocHost((void**)&s.h_maps, lens_bytes(n)));
+        YGZB_CUDA(ctx, cudaMalloc((void**)&s.d_maps, lens_bytes(n)));
+        YGZB_CUDA(ctx, cudaEventCreateWithFlags(&s.e_maps, cudaEventDisableTiming));
     } else {   // the staging's last copy to the device has run (it waited for nothing but earlier front-stream work)
-        YGZB_CUDA(ctx, cudaEventSynchronize(t->e_lens[stream]));
+        YGZB_CUDA(ctx, cudaEventSynchronize(s.e_maps));
     }
     if (!f->e_stage) YGZB_CUDA(ctx, cudaEventCreateWithFlags(&f->e_stage, cudaEventDisableTiming));
     // the maps (host or device memory) are read into the staging and checked before anything an upload reads changes
-    uint8_t* h = t->h_lens[stream];
+    uint8_t* h = s.h_maps;
     const uint16_t* a = reinterpret_cast<const uint16_t*>(h + a_off);
     YGZB_CUDA(ctx, cudaMemcpy(h, map_xy, n * sizeof(short2), cudaMemcpyDefault));
     YGZB_CUDA(ctx, cudaMemcpy(h + a_off, map_a, n * sizeof(uint16_t), cudaMemcpyDefault));
@@ -1284,9 +1286,9 @@ int ygzb_tracker_set_undistort(ygzb_tracker* t, int stream, const int16_t* map_x
             return set_error(ctx, YGZB_ERR_INVALID, "set_undistort: map_a[%zu] = %d is not a 5 + 5-bit fraction (< 1024)", i, (int)a[i]);
     // in order on the front stream, which runs every upload: the ones enqueued before read the old maps, the ones enqueued
     // after the new; nothing waits for the key-frame insertion or a local BA in flight
-    YGZB_CUDA(ctx, cudaMemcpyAsync(t->d_lens[stream], h, lens_bytes(n), cudaMemcpyHostToDevice, t->front));
-    YGZB_CUDA(ctx, cudaEventRecord(t->e_lens[stream], t->front));
-    t->has_lens[stream] = 1;
+    YGZB_CUDA(ctx, cudaMemcpyAsync(s.d_maps, h, lens_bytes(n), cudaMemcpyHostToDevice, t->front));
+    YGZB_CUDA(ctx, cudaEventRecord(s.e_maps, t->front));
+    s.has_maps = true;
     return YGZB_OK;
 }
 
@@ -1300,7 +1302,7 @@ int ygzb_tracker_set_source(ygzb_tracker* t, int stream, int width, int height, 
     if (channels != 1 && channels != 3) return set_error(ctx, YGZB_ERR_INVALID, "set_source: channels must be 1 or 3, not %d", channels);
     // read when an upload is enqueued, so the uploads enqueued before the call read the old format and those after it the new
     // one, in order on the front stream like the maps (ygzb_tracker_set_undistort)
-    t->src[stream] = RawFormat{width, height, channels};
+    t->sources[stream].raw = RawFormat{width, height, channels};
     return YGZB_OK;
 }
 
@@ -1331,18 +1333,14 @@ int ygzb_tracker_upload_stream(ygzb_tracker* t, int stream, int first, int count
     if (!t) return YGZB_ERR_INVALID;
     ygzb_ctx* ctx = t->ctx;
     if (stream < 0 || stream >= t->st.S) return set_error(ctx, YGZB_ERR_INVALID, "upload_stream: stream %d out of range", stream);
-    const RawFormat src = t->src[stream];
-    const bool grey_l0 = src.w == t->st.W && src.h == t->st.H && src.channels == 1;
-    if (!t->has_lens[stream] && grey_l0) return ygzb_tracker_upload(t, first, count, host, frame_stride);
+    const ygzb_tracker::Source& s = t->sources[stream];
     ygzb_frames* f = t->f;
-    if (!t->has_lens[stream])   // a BGR frame of level 0's size: converted, or remapped through the pool's maps
-        return upload_front(t, first, count, host, src, frame_stride, f->undistort ? f->d_map_xy : nullptr, f->d_map_a);
-    if (f->undistort)
+    if (s.has_maps && f->undistort)
         return set_error(ctx, YGZB_ERR_INVALID, "upload_stream: stream %d and the frame pool both have undistortion maps", stream);
-    const uint8_t* d = t->d_lens[stream];
-    const size_t n = (size_t)t->st.W * t->st.H;
-    return upload_front(t, first, count, host, src, frame_stride, reinterpret_cast<const short2*>(d),
-                        reinterpret_cast<const uint16_t*>(d + lens_a_offset(n)));
+    // level 0 is remapped through the stream's maps, else through the pool's, else converted or copied at level 0's size
+    const short2* map_xy = s.has_maps ? reinterpret_cast<const short2*>(s.d_maps) : f->undistort ? f->d_map_xy : nullptr;
+    const uint16_t* map_a = s.has_maps ? reinterpret_cast<const uint16_t*>(s.d_maps + lens_a_offset((size_t)t->st.W * t->st.H)) : f->d_map_a;
+    return upload_front(t, first, count, host, s.raw, frame_stride, map_xy, map_a);
 }
 
 int ygzb_tracker_track(ygzb_tracker* t, int n_jobs, const ygzb_track_job* jobs, ygzb_track_result* results) {

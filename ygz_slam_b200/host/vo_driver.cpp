@@ -567,14 +567,16 @@ struct QFrame {
     bool restart = false;  // first frame of a new sequence (ygz_vo_restart): it becomes a first key-frame
 };
 using Camera = std::array<double, 4>;   // fx, fy, cx, cy
+// bit for bit, as records compare cameras
+bool same_camera(const Camera& a, const Camera& b) { return std::memcmp(a.data(), b.data(), sizeof a) == 0; }
 // a lens (ygz_vo_set_lens): the raw camera K and its distortion dist = {k1, k2, p1, p2, k3}; on = false: none
 struct Lens {
     bool on = false;
-    std::array<double, 4> K{};
+    Camera K{};
     std::array<double, 5> dist{};
     // bit for bit, as records compare cameras
     bool same(const Lens& o) const {
-        return on == o.on && (!on || (std::memcmp(K.data(), o.K.data(), sizeof K) == 0 && std::memcmp(dist.data(), o.dist.data(), sizeof dist) == 0));
+        return on == o.on && (!on || (same_camera(K, o.K) && std::memcmp(dist.data(), o.dist.data(), sizeof dist) == 0));
     }
 };
 // the frames a stream pushes (ygz_vo_set_frame_format): w x h pixels of `channels` bytes (1 grey, 3 BGR), rows packed
@@ -583,20 +585,27 @@ struct Format {
     size_t bytes() const { return (size_t)w * h * channels; }
     bool operator==(const Format&) const = default;
 };
+// what a sequence of a stream is pushed under: its camera (ygz_vo_set_camera), its lens (ygz_vo_set_lens) and the format of
+// its frames (ygz_vo_set_frame_format)
+struct Source {
+    Camera K{};
+    Lens lens;
+    Format fmt;
+    // bit for bit, as records compare K and the lens
+    bool operator==(const Source& o) const { return same_camera(K, o.K) && lens.same(o.lens) && fmt == o.fmt; }
+    // frames of a size other than the context's W x H are only resampled by a lens
+    bool pushable(int W, int H) const { return lens.on || (fmt.w == W && fmt.h == H); }
+};
 struct SeqStart {
     Mat34 T;                  // pose of the sequence's first key-frame
-    Camera K;                 // camera of the sequence
-    Lens lens;                // lens of the sequence
-    Format fmt;               // frame format of the sequence
+    Source src;               // camera, lens and frame format of the sequence
 };
 struct EStream : Counters {
     std::deque<KfInfo> kfs;   // at most YGZB_TRACK_RING, the newest is the reference key-frame; the last kLocalKeyframes are local
     std::deque<QFrame> queue; // frames without a final result, oldest first; the first one is frame next_frame
     Mat34 T = identity();
     Mat34 start = identity(); // pose of the next sequence's first key-frame (ygz_vo_restart)
-    Camera cam{};             // camera of the current sequence, or of the next one while a restart is pending (ygz_vo_set_camera)
-    Lens lens;                // lens of the current sequence, or of the next one while a restart is pending (ygz_vo_set_lens)
-    Format fmt;               // frame format of the current sequence, or of the next one ... (ygz_vo_set_frame_format)
+    Source src;               // source of the current sequence, or of the next one while a restart is pending
     std::deque<SeqStart> starts;   // the queued frames that start a sequence (the stream's first, restarts), in order
     bool has_pose = false, lost = false, has_depth = false;
     bool restart_pending = false;   // the next push starts a new sequence at `start`
@@ -732,9 +741,6 @@ class Engine {
   public:
     Engine(ygzb_ctx* ctx, int n_streams, int window, const Params& p) : ctx_(ctx), S_(n_streams), F_(std::max(1, window)), prm_(p), st_(n_streams) {
         for (int i = 0; i < S_; ++i) order_.push_back(i);
-        for (EStream& s : st_) std::copy_n(prm_.K, 4, s.cam.begin());
-        tr_cam_.assign(S_, st_[0].cam);
-        tr_lens_.assign(S_, TrLens{});
         // YGZ_VO_BLOCKING_SYNC=1: sleep instead of spinning in the one synchronisation per round (hosts with fewer CPUs than
         // engine threads; bench.py sets it when the threads of all ranks outnumber the CPUs it may use)
         const char* e = std::getenv("YGZ_VO_BLOCKING_SYNC");
@@ -755,8 +761,10 @@ class Engine {
         CHK(ygzb_get_params(ctx_, &cp));
         W_ = cp.image_width;
         H_ = cp.image_height;
-        for (EStream& s : st_) s.fmt = default_format();
-        tr_fmt_.assign(S_, default_format());
+        // every stream starts with the tracker's camera, no lens and grey frames of the context's size
+        const Source dflt{{prm_.K[0], prm_.K[1], prm_.K[2], prm_.K[3]}, {}, {W_, H_, 1}};
+        for (EStream& s : st_) s.src = dflt;
+        tr_src_.assign(S_, dflt);
         int rows = 0, cols = 0;
         CHK(ygzb_grid_dims(ctx_, &rows, &cols));
         ring_cells_ = (size_t)YGZB_TRACK_RING * rows * cols;
@@ -794,7 +802,7 @@ class Engine {
         QFrame f{image, depth, tag, stacked};
         if (pushed(i) == 0 || s.restart_pending) {
             f.restart = s.restart_pending;
-            s.starts.push_back({s.start, s.cam, s.lens, s.fmt});
+            s.starts.push_back({s.start, s.src});
             s.restart_pending = false;
         }
         s.queue.push_back(f);
@@ -813,44 +821,15 @@ class Engine {
         s.restart_pending = pushed(i) > 0;
         return YGZB_OK;
     }
-    // the camera of stream i's next sequence: only before its first push or while a restart is pending (the caller has
-    // checked K); it reaches the tracker when that sequence's first key-frame is decided (use_camera)
-    int set_camera(int i, const Camera& K) {
+    // the source of stream i's next sequence: only before its first push or while a restart is pending (the caller has
+    // checked it); it reaches the tracker when that sequence's first frame is uploaded (use_source)
+    int set_source(int i, const Source& src) {
         EStream& s = st_[i];
         if (pushed(i) > 0 && !s.restart_pending) return YGZB_ERR_INVALID;
-        s.cam = K;
+        s.src = src;
         return YGZB_OK;
     }
-    // the lens of stream i's next sequence, at the times set_camera accepts (the caller has checked it); its maps, built for
-    // the camera that sequence ends up with, reach the tracker when the sequence's first frame is uploaded (use_lens)
-    int set_lens(int i, const Lens& L) {
-        EStream& s = st_[i];
-        if (pushed(i) > 0 && !s.restart_pending) return YGZB_ERR_INVALID;
-        s.lens = L;
-        return YGZB_OK;
-    }
-    // some stream has a lens, now or for its next sequence: its records carry a lens block
-    bool any_lens() const {
-        for (const EStream& s : st_)
-            if (s.lens.on) return true;
-        return false;
-    }
-    // the frame format of stream i's next sequence, at the times set_camera accepts (the caller has checked it); it reaches
-    // the tracker when the sequence's first frame is uploaded (use_format)
-    int set_frame_format(int i, const Format& F) {
-        EStream& s = st_[i];
-        if (pushed(i) > 0 && !s.restart_pending) return YGZB_ERR_INVALID;
-        s.fmt = F;
-        return YGZB_OK;
-    }
-    // the format of a stream that was never given one: grey frames of the context's size
-    Format default_format() const { return {W_, H_, 1}; }
-    // some stream has a format other than the default, now or for its next sequence: its records carry a format block
-    bool any_format() const {
-        for (const EStream& s : st_)
-            if (s.fmt != default_format()) return true;
-        return false;
-    }
+    const Source& source(int i) const { return st_[i].src; }
     // final results go to `traj` (this group's [S][n_frames][12], rows in the caller's stream order; NULL: none) and, with
     // collect, to the result queue that pop_results drains
     void set_outputs(double* traj, int n_frames, bool collect) {
@@ -973,12 +952,15 @@ class Engine {
                     if (s.queue[t].restart) w = t;
             }
             w = std::min(w, (int)s.queue.size());
-            // a sequence's lens reaches the tracker with its first frame's upload: every frame of the old sequence has been
-            // uploaded before (a window never crosses a restart), and the tracker orders the maps behind those uploads
-            if (first) {   // (the format likewise)
-                CHK(use_lens(i, s.starts.front().lens, s.starts.front().K));
-                CHK(use_format(i, s.starts.front().fmt));
-            }
+            // a sequence's source reaches the tracker right before its first frame's upload.  Every frame of the old sequence
+            // has been uploaded by then (a window never crosses a restart), and the tracker orders the maps and the format
+            // behind those uploads.  The old sequence is done with the camera too.  Its device readers are kf_fill_kernel,
+            // track_prep_kernel and candidate projection (ba_build_kernel and kf_points_kernel read none, and a local BA
+            // takes its cameras as kernel parameters when it is enqueued).  ygzb_tracker_set_camera waits on the front stream
+            // for e_fill and e_main, which follow the old sequence's last such readers: its last insertion was enqueued in
+            // step 1 of this round, and its last tracking chain ran in an earlier round.  The new sequence's first insertion
+            // waits for e_up
+            if (first) CHK(use_source(i, s.starts.front().src));
             CHK(upload(i, w));
             if (first) {
                 wins_.push_back({i, s.next_frame, 1, -1});
@@ -1043,7 +1025,6 @@ class Engine {
                     s.n_restarts += 1;
                 }
                 s.T = s.starts.front().T;
-                CHK(use_camera(b.stream, s.starts.front().K));   // (nothing of the old sequence is left to run)
                 s.starts.pop_front();
                 s.has_pose = true;
                 pend_keyframe(b.stream, b.stream * F_, -1, 0);
@@ -1102,9 +1083,7 @@ class Engine {
             slots.push_back(S_ * F_ + i * YGZB_TRACK_RING + kf.entry);
         }
         if (rec->n_keyframes != (int)entries.size()) return YGZB_ERR_INVALID;
-        CHK(use_camera(i, s.cam));
-        CHK(use_lens(i, s.lens, s.cam));
-        CHK(use_format(i, s.fmt));
+        CHK(use_source(i, s.src));
         CHK(ygzb_tracker_import(tr_, i, entries.data(), slots.data(), rec));
         if (ref) CHK(ygzb_tracker_import_reference(tr_, i, ref));
         st_[i] = s;
@@ -1125,62 +1104,50 @@ class Engine {
     int check_start_pose(int i, const Mat34& T) { return ygzb_tracker_set_start_pose(tr_, i, T.m); }
 
   private:
-    // the tracker's camera of stream i becomes K for everything enqueued from here on (nothing is enqueued when it is K already)
-    int use_camera(int i, const Camera& K) {
-        if (tr_cam_[i] == K) return YGZB_OK;
-        CHK(ygzb_tracker_set_camera(tr_, i, K.data()));
-        tr_cam_[i] = K;
-        return YGZB_OK;
-    }
-    // the tracker's undistortion maps of stream i become those of lens L seen through camera K (none without a lens) for
-    // every upload enqueued from here on; nothing is enqueued when they are already
-    int use_lens(int i, const Lens& L, const Camera& K) {
-        TrLens& cur = tr_lens_[i];
-        if (cur.lens.same(L) && (!L.on || cur.K == K)) return YGZB_OK;
-        if (L.on) {
-            const size_t n = (size_t)W_ * H_;
-            if (!(maps_for_.lens.same(L) && maps_for_.K == K)) {   // (streams of one lens and camera share the host maps)
-                map_xy_.resize(2 * n);
-                map_a_.resize(n);
-                maps_for_ = {};
-                CHK(ygzb_undistort_map(W_, H_, L.K.data(), L.dist.data(), K.data(), map_xy_.data(), map_a_.data()));
-                maps_for_ = {L, K};
+    // the tracker's camera, undistortion maps and raw frame format of stream i become those of `src`, in that order, for
+    // everything enqueued from here on; nothing is enqueued for a part the tracker has already.  The maps are those of the
+    // lens seen through the camera (none without a lens)
+    int use_source(int i, const Source& src) {
+        Source& cur = tr_src_[i];
+        const bool new_K = !same_camera(cur.K, src.K);
+        if (new_K) CHK(ygzb_tracker_set_camera(tr_, i, src.K.data()));
+        cur.K = src.K;
+        if (!cur.lens.same(src.lens) || (src.lens.on && new_K)) {
+            const Lens& L = src.lens;
+            if (L.on) {
+                const size_t n = (size_t)W_ * H_;
+                if (!(maps_lens_.same(L) && same_camera(maps_K_, src.K))) {   // (streams of one lens and camera share the host maps)
+                    map_xy_.resize(2 * n);
+                    map_a_.resize(n);
+                    maps_lens_ = {};
+                    CHK(ygzb_undistort_map(W_, H_, L.K.data(), L.dist.data(), src.K.data(), map_xy_.data(), map_a_.data()));
+                    maps_lens_ = L;
+                    maps_K_ = src.K;
+                }
+                CHK(ygzb_tracker_set_undistort(tr_, i, map_xy_.data(), map_a_.data()));
+                h2d_other_bytes += (long long)(n * 6);
+            } else {
+                CHK(ygzb_tracker_set_undistort(tr_, i, nullptr, nullptr));
             }
-            CHK(ygzb_tracker_set_undistort(tr_, i, map_xy_.data(), map_a_.data()));
-            h2d_other_bytes += (long long)(n * 6);
-        } else {
-            CHK(ygzb_tracker_set_undistort(tr_, i, nullptr, nullptr));
+            cur.lens = L;
         }
-        cur = {L, K};
-        return YGZB_OK;
-    }
-    // the tracker reads the raw frames of stream i in format F for every upload enqueued from here on; nothing is enqueued
-    // when it does already
-    int use_format(int i, const Format& F) {
-        if (tr_fmt_[i] == F) return YGZB_OK;
-        CHK(ygzb_tracker_set_source(tr_, i, F.w, F.h, F.channels));
-        tr_fmt_[i] = F;
+        if (cur.fmt != src.fmt) CHK(ygzb_tracker_set_source(tr_, i, src.fmt.w, src.fmt.h, src.fmt.channels));
+        cur.fmt = src.fmt;
         return YGZB_OK;
     }
     // the first w queued frames of stream i into its frame slots: one strided copy when they are equally spaced in one
     // stacked sequence, one copy per frame otherwise (frames pushed one by one may sit in separate allocations, which one
     // strided copy cannot span even when their addresses happen to be equally spaced).  The frames are in the tracker's
-    // format of the stream (use_format), that of their sequence
+    // format of the stream (use_source), that of their sequence
     int upload(int i, int w) {
         const std::deque<QFrame>& q = st_[i].queue;
-        const size_t fb = tr_fmt_[i].bytes();
+        const size_t fb = tr_src_[i].fmt.bytes();
         const ptrdiff_t stride = w > 1 ? q[1].image - q[0].image : (ptrdiff_t)fb;
         bool strided = stride >= (ptrdiff_t)fb;
         for (int t = 0; t < w && strided; ++t) strided = q[t].stacked && (t < 2 || q[t].image - q[t - 1].image == stride);
         h2d_image_bytes += (long long)w * (long long)fb;
-        // a stream without a lens, of the default format, uploads exactly as before lenses and formats existed
-        const bool own = tr_lens_[i].lens.on || tr_fmt_[i] != default_format();
-        auto up = [&](int first, int count, const uint8_t* src, size_t frame_stride) {
-            return own ? ygzb_tracker_upload_stream(tr_, i, first, count, src, frame_stride)
-                       : ygzb_tracker_upload(tr_, first, count, src, frame_stride);
-        };
-        if (strided) return up(i * F_, w, q[0].image, (size_t)stride);
-        for (int t = 0; t < w; ++t) CHK(up(i * F_ + t, 1, q[t].image, fb));
+        if (strided) return ygzb_tracker_upload_stream(tr_, i, i * F_, w, q[0].image, (size_t)stride);
+        for (int t = 0; t < w; ++t) CHK(ygzb_tracker_upload_stream(tr_, i, i * F_ + t, 1, q[t].image, fb));
         return YGZB_OK;
     }
     // the map update of key-frame job kj, whose result r and rows (r.ba_points moved, then r.n_features new) have just come
@@ -1276,16 +1243,13 @@ class Engine {
     std::vector<ygzb_keyframe_job> kjobs_;   // key-frame insertions for the next round ...
     RowQueue<KfFrame, ygzb_observation> kframes_;   // ... and their frames, with their observation rows
     std::vector<int> order_;
-    std::vector<Camera> tr_cam_;   // the tracker's camera of every stream (ygzb_tracker_set_camera), as last set
-    struct TrLens {
-        Lens lens;
-        Camera K;
-    };
-    std::vector<TrLens> tr_lens_;  // the lens and camera the tracker's maps of every stream were built for (ygzb_tracker_set_undistort)
-    std::vector<Format> tr_fmt_;   // the tracker's raw frame format of every stream (ygzb_tracker_set_source), as last set
-    std::vector<int16_t> map_xy_;  // host maps of use_lens, built for the lens and camera maps_for_ (lens off: none)
+    // the source the tracker has of every stream, as use_source last set it: its camera (ygzb_tracker_set_camera), the lens
+    // its maps were built for with that camera (ygzb_tracker_set_undistort) and its raw frame format (ygzb_tracker_set_source)
+    std::vector<Source> tr_src_;
+    std::vector<int16_t> map_xy_;  // host maps of use_source, built for lens maps_lens_ seen through camera maps_K_ (lens off: none)
     std::vector<uint16_t> map_a_;
-    TrLens maps_for_;
+    Lens maps_lens_;
+    Camera maps_K_{};
     double* traj_ = nullptr;
     int traj_frames_ = 0;
     bool collect_ = false;
@@ -1334,23 +1298,26 @@ struct RefBuf {
 static_assert(std::endian::native == std::endian::little, "stream records are little-endian and copied field by field");
 constexpr uint8_t kRecordMagic[4] = {'Y', 'G', 'Z', 'S'};
 
-// what a record is made under and must be loaded under: the engine's image size, grid, pyramid, camera and reference mode,
-// and the stream's lens and frame format
+// what a record is made under and must be loaded under: the engine's image size, grid, pyramid and reference mode, and the
+// stream's source
 struct RecordGeom {
-    int32_t width, height, cells, n_levels;
-    double K[4];
-    int32_t ref_mode;
-    Lens lens{};
-    Format fmt{};   // (save and load set it; read_record's is the record's)
+    int32_t width, height, cells, n_levels, ref_mode;
+    Source src{};   // (save and load set it; read_record's is the record's)
     size_t wh() const { return (size_t)width * height; }
-    bool default_fmt() const { return fmt == Format{width, height, 1}; }
+    Format default_fmt() const { return {width, height, 1}; }
 };
 constexpr size_t kRecordLensBytes = 9 * sizeof(double);   // version 2's lens block: K[4], dist[5]
 constexpr size_t kRecordFormatBytes = 4 * sizeof(int32_t);   // version 3's format block: width, height, channels, has_lens
 
-// the largest record of an engine: a full ring at capacity, a full reference, a depth map (the sections of write_record),
-// with lens, a lens block, and with fmt, a format block
-size_t record_bound(const RecordGeom& g, bool lens, bool fmt) {
+// the largest record of an engine whose streams are `st`: a full ring at capacity, a full reference, a depth map (the
+// sections of write_record), with a lens block while some stream has a lens and a format block while some stream has a
+// format other than the default, now or for its next sequence
+size_t record_bound(const RecordGeom& g, const std::vector<EStream>& st) {
+    bool lens = false, fmt = false;
+    for (const EStream& s : st) {
+        lens |= s.src.lens.on;
+        fmt |= s.src.fmt != g.default_fmt();
+    }
     const size_t R = YGZB_TRACK_RING, F = R * g.cells, O = R * YGZB_MAP_OBS_PER_CELL * g.cells;
     const size_t C = (size_t)YGZB_TRACK_REF_FEATURES_PER_CELL * g.cells, WH = g.wh();
     return 68 + (fmt ? kRecordFormatBytes : 0) + (lens ? kRecordLensBytes : 0)   // header, format, lens
@@ -1391,6 +1358,41 @@ struct RecordReader {
     }
 };
 
+// the version of a record of the stream's source g.src: 3 with a format other than the default, else 2 with a lens, else 1
+uint32_t record_version(const RecordGeom& g) {
+    if (g.src.fmt != g.default_fmt()) return YGZ_VO_STREAM_RECORD_VERSION_FORMAT;
+    return g.src.lens.on ? YGZ_VO_STREAM_RECORD_VERSION_LENS : YGZ_VO_STREAM_RECORD_VERSION;
+}
+// the header's blocks behind the reference mode: the format block (version 3), then the lens block (with a lens)
+void write_source_blocks(RecordWriter& w, const RecordGeom& g) {
+    const Source& s = g.src;
+    if (record_version(g) == YGZ_VO_STREAM_RECORD_VERSION_FORMAT) {
+        w.put<int32_t>(s.fmt.w); w.put<int32_t>(s.fmt.h); w.put<int32_t>(s.fmt.channels); w.put<int32_t>(s.lens.on);
+    }
+    if (s.lens.on) {
+        w.bytes(s.lens.K.data(), sizeof s.lens.K);
+        w.bytes(s.lens.dist.data(), sizeof s.lens.dist);
+    }
+}
+// reads the blocks of a record of `version` into rg.src (whose camera is read already): false unless they are well formed
+// and the record's version is that of the source they give (a default format is always written as version 1 or 2)
+bool read_source_blocks(RecordReader& r, uint32_t version, RecordGeom& rg) {
+    Source& s = rg.src;
+    s.lens.on = version == YGZ_VO_STREAM_RECORD_VERSION_LENS;
+    s.fmt = rg.default_fmt();
+    if (version == YGZ_VO_STREAM_RECORD_VERSION_FORMAT) {
+        s.fmt.w = r.get<int32_t>(); s.fmt.h = r.get<int32_t>(); s.fmt.channels = r.get<int32_t>();
+        const int32_t has_lens = r.get<int32_t>();
+        if (has_lens != 0 && has_lens != 1) return false;
+        s.lens.on = has_lens;
+    }
+    if (s.lens.on) {
+        r.bytes(s.lens.K.data(), sizeof s.lens.K);
+        r.bytes(s.lens.dist.data(), sizeof s.lens.dist);
+    }
+    return r.ok && record_version(rg) == version;
+}
+
 // the record of stream `s` with its map `m` (exported from the ring entries of s.kfs), its reference `r` (previous-frame
 // mode once it has a key-frame, else NULL) and its depth map (NULL unless s.has_depth)
 void write_record(RecordWriter& w, const RecordGeom& g, const EStream& s, const ygzb_map_record& m, const ygzb_reference_record* r,
@@ -1398,20 +1400,13 @@ void write_record(RecordWriter& w, const RecordGeom& g, const EStream& s, const 
     const size_t WH = g.wh();
     // 1. header (the size is written last)
     w.bytes(kRecordMagic, 4);
-    const bool v3 = !g.default_fmt();
-    w.put<uint32_t>(v3 ? YGZ_VO_STREAM_RECORD_VERSION_FORMAT : g.lens.on ? YGZ_VO_STREAM_RECORD_VERSION_LENS : YGZ_VO_STREAM_RECORD_VERSION);
+    w.put<uint32_t>(record_version(g));
     const size_t size_at = w.n;
     w.put<uint64_t>(0);
     w.put<int32_t>(g.width); w.put<int32_t>(g.height); w.put<int32_t>(g.cells); w.put<int32_t>(g.n_levels);
-    w.bytes(g.K, sizeof g.K);
+    w.bytes(g.src.K.data(), sizeof g.src.K);
     w.put<int32_t>(g.ref_mode);
-    if (v3) {
-        w.put<int32_t>(g.fmt.w); w.put<int32_t>(g.fmt.h); w.put<int32_t>(g.fmt.channels); w.put<int32_t>(g.lens.on);
-    }
-    if (g.lens.on) {   // version 2, or 3 with has_lens
-        w.bytes(g.lens.K.data(), sizeof g.lens.K);
-        w.bytes(g.lens.dist.data(), sizeof g.lens.dist);
-    }
+    write_source_blocks(w, g);
     // 2. host state
     w.put<int32_t>((int32_t)s.kfs.size());
     for (const KfInfo& kf : s.kfs) {
@@ -1474,27 +1469,12 @@ int read_record(const uint8_t* in, size_t size, const RecordGeom& g, StreamRecor
     const uint64_t total = r.get<uint64_t>();
     RecordGeom rg{};
     rg.width = r.get<int32_t>(); rg.height = r.get<int32_t>(); rg.cells = r.get<int32_t>(); rg.n_levels = r.get<int32_t>();
-    r.bytes(rg.K, sizeof rg.K);
+    r.bytes(rg.src.K.data(), sizeof rg.src.K);
     rg.ref_mode = r.get<int32_t>();
     if (!r.ok || std::memcmp(magic, kRecordMagic, 4) != 0 || total != size) return YGZB_ERR_INVALID;
-    if (version != YGZ_VO_STREAM_RECORD_VERSION && version != YGZ_VO_STREAM_RECORD_VERSION_LENS &&
-        version != YGZ_VO_STREAM_RECORD_VERSION_FORMAT)
-        return YGZB_ERR_INVALID;
-    rg.lens.on = version == YGZ_VO_STREAM_RECORD_VERSION_LENS;
-    rg.fmt = {rg.width, rg.height, 1};
-    if (version == YGZ_VO_STREAM_RECORD_VERSION_FORMAT) {
-        rg.fmt.w = r.get<int32_t>(); rg.fmt.h = r.get<int32_t>(); rg.fmt.channels = r.get<int32_t>();
-        const int32_t has_lens = r.get<int32_t>();
-        // (a default format is always written as version 1 or 2)
-        if (!r.ok || (has_lens != 0 && has_lens != 1) || rg.default_fmt()) return YGZB_ERR_INVALID;
-        rg.lens.on = has_lens;
-    }
-    if (rg.lens.on) {
-        r.bytes(rg.lens.K.data(), sizeof rg.lens.K);
-        r.bytes(rg.lens.dist.data(), sizeof rg.lens.dist);
-    }
-    if (!r.ok || rg.width != g.width || rg.height != g.height || rg.cells != g.cells || rg.n_levels != g.n_levels || rg.ref_mode != g.ref_mode ||
-        std::memcmp(rg.K, g.K, sizeof g.K) != 0 || !rg.lens.same(g.lens) || rg.fmt != g.fmt)   // K and the lens bit for bit
+    if (!read_source_blocks(r, version, rg)) return YGZB_ERR_INVALID;
+    if (rg.width != g.width || rg.height != g.height || rg.cells != g.cells || rg.n_levels != g.n_levels || rg.ref_mode != g.ref_mode ||
+        rg.src != g.src)   // K and the lens bit for bit
         return YGZB_ERR_INVALID;
     // 2. host state
     EStream& s = out.s;
@@ -1541,7 +1521,7 @@ int read_record(const uint8_t* in, size_t size, const RecordGeom& g, StreamRecor
     // 3. map: the key-frames of the host state, in the same order
     ygzb_map_record& m = out.map.rec;
     m.width = g.width; m.height = g.height; m.cells = g.cells; m.n_levels = g.n_levels;
-    std::memcpy(m.K, g.K, sizeof m.K);
+    std::memcpy(m.K, g.src.K.data(), sizeof m.K);
     m.n_keyframes = r.get<int32_t>();
     if (!r.ok || m.n_keyframes != n_kf) return YGZB_ERR_INVALID;
     size_t F = 0, O = 0;
@@ -1565,7 +1545,7 @@ int read_record(const uint8_t* in, size_t size, const RecordGeom& g, StreamRecor
     if (out.has_ref) {
         ygzb_reference_record& q = out.ref.rec;
         q.width = g.width; q.height = g.height; q.cells = g.cells; q.n_levels = g.n_levels;
-        std::memcpy(q.K, g.K, sizeof q.K);
+        std::memcpy(q.K, g.src.K.data(), sizeof q.K);
         q.n = r.get<int32_t>();
         if (!r.ok || q.n < 0 || q.n > q.capacity) return YGZB_ERR_INVALID;
         r.bytes(q.T_cw, sizeof q.T_cw);
@@ -1905,7 +1885,7 @@ int ygz_vo_create(ygzb_ctx* ctx, const ygz_vo_config* cfg, ygz_vo** out) {
     if (!vo) return YGZB_ERR_INVALID;
     int rows = 0, cols = 0;
     CHK(ygzb_grid_dims(ctx, &rows, &cols));
-    vo->geom = RecordGeom{cp.image_width, cp.image_height, rows * cols, cp.n_levels, {cfg->K[0], cfg->K[1], cfg->K[2], cfg->K[3]}, cfg->ref_mode};
+    vo->geom = RecordGeom{cp.image_width, cp.image_height, rows * cols, cp.n_levels, cfg->ref_mode};
     vo->eng = std::make_unique<Engine>(ctx, cfg->n_streams, cfg->window, prm);
     vo->eng->set_outputs(nullptr, 0, true);
     CHK(vo->eng->init(nullptr));
@@ -1917,9 +1897,9 @@ int ygz_vo_push(ygz_vo* vo, int stream, const uint8_t* image, const double* dept
     if (!vo || stream < 0 || stream >= vo->n_streams || !image) return YGZB_ERR_INVALID;
     const EStream& s = vo->eng->streams()[stream];
     if (!depth && (!s.has_depth || s.restart_pending)) return YGZB_ERR_INVALID;
-    // a sequence's first frame fixes its format and lens: a raw size other than the context's is only resampled by a lens
+    // a sequence's first frame fixes its source
     const bool starts = vo->eng->pushed(stream) == 0 || s.restart_pending;
-    if (starts && (s.fmt.w != vo->eng->width() || s.fmt.h != vo->eng->height()) && !s.lens.on) return YGZB_ERR_INVALID;
+    if (starts && !s.src.pushable(vo->eng->width(), vo->eng->height())) return YGZB_ERR_INVALID;
     vo->eng->push(stream, image, depth, tag);
     return YGZB_OK;
 }
@@ -1936,7 +1916,9 @@ int ygz_vo_set_camera(ygz_vo* vo, int stream, const double K[4]) {
     for (int c = 0; c < 4; ++c)
         if (!std::isfinite(K[c])) return YGZB_ERR_INVALID;
     if (!(K[0] > 0 && K[1] > 0)) return YGZB_ERR_INVALID;
-    return vo->eng->set_camera(stream, Camera{K[0], K[1], K[2], K[3]});
+    Source src = vo->eng->source(stream);
+    src.K = Camera{K[0], K[1], K[2], K[3]};
+    return vo->eng->set_source(stream, src);
 }
 
 int ygz_vo_set_lens(ygz_vo* vo, int stream, const double K[4], const double dist[5]) {
@@ -1952,12 +1934,14 @@ int ygz_vo_set_lens(ygz_vo* vo, int stream, const double K[4], const double dist
         std::copy_n(K, 4, L.K.begin());
         std::copy_n(dist, 5, L.dist.begin());
     }
-    return vo->eng->set_lens(stream, L);
+    Source src = vo->eng->source(stream);
+    src.lens = L;
+    return vo->eng->set_source(stream, src);
 }
 
 int ygz_vo_get_lens(const ygz_vo* vo, int stream, int* has_lens, double K[4], double dist[5]) {
     if (!vo || !has_lens || !K || !dist || stream < 0 || stream >= vo->n_streams) return YGZB_ERR_INVALID;
-    const Lens& L = vo->eng->streams()[stream].lens;
+    const Lens& L = vo->eng->source(stream).lens;
     *has_lens = L.on ? 1 : 0;
     std::copy(L.K.begin(), L.K.end(), K);   // (zeros without a lens)
     std::copy(L.dist.begin(), L.dist.end(), dist);
@@ -1967,12 +1951,14 @@ int ygz_vo_get_lens(const ygz_vo* vo, int stream, int* has_lens, double K[4], do
 int ygz_vo_set_frame_format(ygz_vo* vo, int stream, int width, int height, int channels) {
     if (!vo || stream < 0 || stream >= vo->n_streams) return YGZB_ERR_INVALID;
     if (width < 1 || height < 1 || width > 32767 || height > 32767 || (channels != 1 && channels != 3)) return YGZB_ERR_INVALID;
-    return vo->eng->set_frame_format(stream, Format{width, height, channels});
+    Source src = vo->eng->source(stream);
+    src.fmt = Format{width, height, channels};
+    return vo->eng->set_source(stream, src);
 }
 
 int ygz_vo_get_frame_format(const ygz_vo* vo, int stream, int* width, int* height, int* channels) {
     if (!vo || !width || !height || !channels || stream < 0 || stream >= vo->n_streams) return YGZB_ERR_INVALID;
-    const Format& F = vo->eng->streams()[stream].fmt;
+    const Format& F = vo->eng->source(stream).fmt;
     *width = F.w;
     *height = F.h;
     *channels = F.channels;
@@ -1981,7 +1967,7 @@ int ygz_vo_get_frame_format(const ygz_vo* vo, int stream, int* width, int* heigh
 
 int ygz_vo_get_camera(const ygz_vo* vo, int stream, double K[4]) {
     if (!vo || !K || stream < 0 || stream >= vo->n_streams) return YGZB_ERR_INVALID;
-    const Camera& c = vo->eng->streams()[stream].cam;
+    const Camera& c = vo->eng->source(stream).K;
     std::copy(c.begin(), c.end(), K);
     return YGZB_OK;
 }
@@ -2054,7 +2040,7 @@ int ygz_vo_export_map(ygz_vo* vo, int stream, ygzb_map_record* out) {
 
 int ygz_vo_stream_record_bound(const ygz_vo* vo, size_t* bytes) {
     if (!vo || !bytes) return YGZB_ERR_INVALID;
-    *bytes = record_bound(vo->geom, vo->eng->any_lens(), vo->eng->any_format());
+    *bytes = record_bound(vo->geom, vo->eng->streams());
     return YGZB_OK;
 }
 
@@ -2066,10 +2052,8 @@ int ygz_vo_save_stream(ygz_vo* vo, int stream, void* buf, size_t capacity, size_
     if (!e.settled(stream)) return YGZB_ERR_INVALID;
     if (!vo->stage.mem) CHK(vo->stage.init(vo->geom));
     const EStream& s = e.streams()[stream];
-    RecordGeom g = vo->geom;   // with the stream's own camera, lens and frame format
-    std::copy(s.cam.begin(), s.cam.end(), g.K);
-    g.lens = s.lens;
-    g.fmt = s.fmt;
+    RecordGeom g = vo->geom;
+    g.src = s.src;
     SaveStage& st = vo->stage;
     CHK(e.export_map(stream, &st.map));
     const bool ref = e.has_reference(stream);
@@ -2091,18 +2075,11 @@ int ygz_vo_load_stream(ygz_vo* vo, int stream, const void* buf, size_t size) {
     if (!vo || !buf || stream < 0 || stream >= vo->n_streams) return YGZB_ERR_INVALID;
     Engine& e = *vo->eng;
     if (!e.settled(stream)) return YGZB_ERR_INVALID;
-    const Camera cam = e.streams()[stream].cam;   // the record's K, lens and format must be the destination stream's
-    const Lens lens = e.streams()[stream].lens;
-    const Format fmt = e.streams()[stream].fmt;
     RecordGeom g = vo->geom;
-    std::copy(cam.begin(), cam.end(), g.K);
-    g.lens = lens;
-    g.fmt = fmt;
+    g.src = e.source(stream);   // the record's source must be the destination stream's
     StreamRecord rec(g);
     CHK(read_record(static_cast<const uint8_t*>(buf), size, g, rec));
-    rec.s.cam = cam;
-    rec.s.lens = lens;
-    rec.s.fmt = fmt;
+    rec.s.src = g.src;
     CHK(e.check_start_pose(stream, rec.s.start));
     CHK(e.adopt(stream, rec.s, &rec.map.rec, rec.has_ref ? &rec.ref.rec : nullptr));
     if (rec.s.has_depth) CHK(e.set_depth(stream, rec.depth.data()));

@@ -294,24 +294,16 @@ class Engine:
         self.map_updates = False
         if map_updates:
             self.set_map_updates(True)
-        if cameras is not None:
-            if len(cameras) != self.n_streams:
-                raise ValueError(f"cameras: {len(cameras)} cameras for {self.n_streams} streams")
-            for s, cam in enumerate(cameras):
-                if cam is not None:
-                    self.set_camera(s, cam)
-        if lenses is not None:
-            if len(lenses) != self.n_streams:
-                raise ValueError(f"lenses: {len(lenses)} lenses for {self.n_streams} streams")
-            for s, lens in enumerate(lenses):
-                if lens is not None:
-                    self.set_lens(s, *lens)
-        if frame_formats is not None:
-            if len(frame_formats) != self.n_streams:
-                raise ValueError(f"frame_formats: {len(frame_formats)} formats for {self.n_streams} streams")
-            for s, fmt in enumerate(frame_formats):
-                if fmt is not None:
-                    self.set_frame_format(s, *fmt)
+        for name, noun, per_stream, apply in (("cameras", "cameras", cameras, self.set_camera),
+                                              ("lenses", "lenses", lenses, lambda s, lens: self.set_lens(s, *lens)),
+                                              ("frame_formats", "formats", frame_formats, lambda s, fmt: self.set_frame_format(s, *fmt))):
+            if per_stream is None:
+                continue
+            if len(per_stream) != self.n_streams:
+                raise ValueError(f"{name}: {len(per_stream)} {noun} for {self.n_streams} streams")
+            for s, v in enumerate(per_stream):
+                if v is not None:
+                    apply(s, v)
 
     def set_camera(self, stream, K):
         """K = (fx, fy, cx, cy) of `stream`'s next sequence (ygz_vo_set_camera): only before its first push or while a
